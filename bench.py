@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — rays/sec of the eval-mode MultiPly forward on B200 (BASELINE.json metric).
+"""bench.py — rays/sec of the eval-mode MultiPly forward on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N ...            # the reference algorithm on the host CPU
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/*.npy
 
 A "step" is one pass of the hot path (Multiply.forward, eval) over one batch of synthetic rays:
 BASELINE.json configs[1] = 2-person synthetic SMPL scene, 4096 rays x 128 samples (S/E/X = 128/256/64),
-1 x B200.  With N GPUs every rank renders its own 4096-ray block of a 4096*N-ray batch (weak scaling)
+1 x H100.  With N GPUs every rank renders its own 4096-ray block of a 4096*N-ray batch (weak scaling)
 and the rendered pixels are all-gathered over NCCL; `value` = all rays / max-over-ranks device time.
 
 `value`  : inputs (rays, hit lists, posed bodies) resident on the device, engine.Renderer.render.
@@ -43,9 +44,10 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(bf16_sustained=d.get("bf16_tflops_sustained", 1400.0), bf16_burst=d.get("bf16_tflops", 1590.0),
-                    hbm=d.get("hbm_gbs", 6650.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_sustained=1400.0, bf16_burst=1590.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+        return dict(bf16_sustained=d.get("bf16_tflops_sustained", 989.0), bf16_burst=d.get("bf16_tflops", 989.0),
+                    hbm=d.get("hbm_gbs", 3350.0), source="measured (MEASURED_PEAKS.json)")
+    # data-sheet figures of the H100 SXM at 700 W (dense fp16/bf16, HBM3); a card with a lower power limit reaches less
+    return dict(bf16_sustained=989.0, bf16_burst=989.0, hbm=3350.0, source="H100 SXM data sheet (700 W), not measured")
 
 
 class ClockSampler(threading.Thread):
@@ -89,7 +91,7 @@ def config_dict(world):
                         "SDF/colour MLPs + composite + background" % (RAYS_PER_GPU, S_SAMPLES),
             "rays_per_gpu": RAYS_PER_GPU, "persons": PERSONS, "N_samples": S_SAMPLES,
             "global_rays": RAYS_PER_GPU * world,
-            "precision": "fp16 hi/lo split x3 tcgen05 MMAs, fp32 accumulate (parity mode, RGB/SDF within 1e-4)",
+            "precision": "fp16 hi/lo split x3 wgmma MMAs, fp32 accumulate (parity mode, RGB/SDF within 1e-4)",
             "scene": "bodies from the device SMPL server (mp_smpl_forward) on a synthetic SMPL-shaped model, "
                      "geometric-init networks (multiply_b200/scene.py:make_smpl_scene)",
             "rays": "uniform in the persons' image-space bounding rectangle; `value`: hit lists resident (host slab test, "
@@ -364,7 +366,7 @@ def extras_sdf_grid(dev):
 
 
 def extras_precision(timer, r, d_inp, d_hits, R, steps, oracle_check):
-    """The tcgen05 precision modes side by side (mp_set_precision): `parity` (three split terms everywhere, the headline),
+    """The tensor-core precision modes side by side (mp_set_precision): `parity` (three split terms everywhere, the headline),
     `colour1` (single-term colour layers), `throughput` (one fp16 term everywhere): rays/s of the resident-input step and,
     when the oracle sample is available, the measured L-inf of each mode against it."""
     from multiply_b200 import engine
@@ -394,8 +396,10 @@ def main():
     ap.add_argument("--engine", default=os.environ.get("MP_ENGINE", "tc"))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the pixel outputs of the last timed step (resident-input render) as DIR/<name>.npy")
     ap.add_argument("--precision", default="parity", choices=["parity", "colour1", "throughput"],
-                    help="tcgen05 precision mode of the main measurement (default parity: RGB/SDF within 1e-4)")
+                    help="tensor-core precision mode of the main measurement (default parity: RGB/SDF within 1e-4)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -446,6 +450,13 @@ def main():
     clocks = ClockSampler(local)
     clocks.start()
     ms_value, launches = timer.run(step_resident, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path receives: every pixel output of the last step (the gathered frame with N GPUs),
+        # float32, 48 B per ray
+        outs = parallel.PixelBuffer.frame(gathered, world, R, PERSONS) if world > 1 else buf.views
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k in parallel.PIXEL_KEYS:
+            np.save(os.path.join(args.dump_outputs, k + ".npy"), outs[k].detach().float().cpu().numpy())
     with torch.no_grad():
         ms_e2e, launches_e2e = timer.run(step_e2e, args.steps, args.warmup)
     model._renderer.check_status()
@@ -546,14 +557,6 @@ def main():
             all_flops += hits[p].numel() * (trips[p] * E * F_SDF + n * (F_SDF + B_SDF + F_RGB))
         all_flops += R * 32 * F_BG
         h2d = sum(v.numel() * v.element_size() for v in h_inp.values())
-        traffic, traffic_src = None, None
-        for tag in ("r2", "r1"):
-            tp = os.path.join(ROOT, "profiles", tag + "_traffic.json")
-            if os.path.exists(tp):
-                tj = json.load(open(tp))
-                traffic = tj["tc_chain_kernel_dram_bytes_per_step"]
-                traffic_src = "profiles/%s_traffic.json (%s)" % (tag, tj.get("captured", "ncu --set full capture of this workload"))
-                break
         line = {
             "metric": "rays/sec", "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_value / args.steps, "higher_is_better": True, "scaling": "weak",
@@ -568,10 +571,9 @@ def main():
             "gpu_launches": launches,
             "clocks": clocks.summary(),
             "roofline": {"bound": "tensor", "achieved": ach, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
-                         "frac": ach / peaks["bf16_sustained"], "traffic": traffic, "traffic_source": traffic_src,
-                         "traffic_note": "DRAM bytes of the kernel's launches of one step; achieved is likewise aggregated over "
-                                         "the step's launches.  Algorithmic bytes are ~6.6 MB of weights per field plus "
-                                         "~100 B of I/O per point",
+                         "frac": ach / peaks["bf16_sustained"],
+                         "traffic_note": "achieved is aggregated over the step's launches.  Algorithmic bytes are ~6.6 MB "
+                                         "of weights per field plus ~100 B of I/O per point",
                          "kernel": "tc_chain_kernel (fused SDF/grad/colour MLP chain)",
                          "peak_source": peaks["source"] + ", sustained bf16 (kernel timed inside a long step)",
                          "kernel_timing": "CUDA events per launch, %d-step pass on the single-stream schedule "

@@ -1,5 +1,5 @@
 /*
- * multiply_b200 — C ABI of the B200-native (sm_100a) MultiPly volume-rendering hot path.
+ * multiply_b200 — C ABI of the H100-native (sm_90a) MultiPly volume-rendering hot path.
  *
  * The reference (eth-ait/MultiPly) has no FFI / plugin registry: its boundary for this path
  * is the Python operator surface of code/lib/model (SURVEY.md §8b).  Each entry point below
@@ -81,7 +81,7 @@ typedef struct {
 /* A foreground field = ImplicitNet + RenderingNet of one person; background field = bg pair.
  * Packing folds weight-norm (networks.py:82-83), the 1/sqrt(2) of the skip layer (:166-167) and
  * lays the weights out for the kernels (fp32 transposed for the SIMT engine, fp16 hi/lo
- * swizzled K-major tiles for the tcgen05 engine).  The handle is immutable afterwards. */
+ * swizzled K-major tiles for the tensor-core engine).  The handle is immutable afterwards. */
 size_t mp_field_pack_bytes(void);
 int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background,
                   void* storage, size_t storage_bytes, mp_net_t** out, void* stream);
@@ -90,10 +90,10 @@ void mp_field_free(mp_net_t* f);
  * the layer-0 bias and lin_pose(body_pose) (networks.py:277-281) / frame code into the colour layer-0 bias. */
 int mp_field_set_cond(mp_net_t* f, const float* cond /*[cond_dim]*/, void* stream);
 
-/* engine selection: 0 = fp32 SIMT (validation engine), 1 = tcgen05 split-fp16 tensor-core engine */
+/* engine selection: 0 = fp32 SIMT (validation engine), 1 = wgmma split-fp16 tensor-core engine */
 int mp_set_engine(int engine);
 int mp_get_engine(void);
-/* Precision mode of the tcgen05 engine: which split-precision product terms each MLP layer issues (fp16 hi/lo operand
+/* Precision mode of the tensor-core engine: which split-precision product terms each MLP layer issues (fp16 hi/lo operand
  * pairs, fp32 accumulation).  0 = parity (default): A_hi.W_hi + A_lo.W_hi + A_hi.W_lo everywhere (RGB / SDF within 1e-4 of
  * the fp32 reference); 1 = the colour layers issue A_hi.W_hi only (SDF / normals unchanged, RGB ~2e-5); 2 = throughput:
  * every layer single-term, i.e. plain fp16 operands — outside the 1e-4 gate, reported separately. */
@@ -103,14 +103,13 @@ int mp_get_precision(void);
  * 0 = everything on the caller's stream (used for per-kernel timing).  Environment override: MP_RENDER_STREAMS. */
 int mp_set_streams(int on);
 
-/* Per-launch timing of the tcgen05 MLP kernel (CUDA events on the launching stream), by program kind:
+/* Per-launch timing of the tensor-core MLP kernel (CUDA events on the launching stream), by program kind:
  * [0] sdf-only, [1] forward (sdf + features), [2] full shade, [3] background.  mp_profile_read synchronises
  * on the recorded events and returns summed milliseconds, launch counts and processed points (host arrays of 4). */
 int mp_profile_enable(int on);
 int mp_profile_read(double* ms_host, long long* launches_host, double* points_host, int reset);
-/* Diagnostics: cycle stamps of one tile of CTA 0 of the last tcgen05 launch (recorded when MP_TC_KNOBS has bit 1 set):
- * out[s*8 + 0..6] epilogue warp (step start, accumulator ready, chunk 0..3 done, step end), out[2048 + s*8 + 0..4] MMA
- * issuer (operand K-block 0..3 ready, commit).  scripts/gpu_trace.py prints them. */
+/* Diagnostics: copies out the device buffer of per-tile cycle stamps (up to 4096 values).  The wgmma kernel records no
+ * stamps, so it reads back zeros; the entry point is kept so that callers built against this header keep linking. */
 int mp_tc_trace_read(unsigned long long* out, int n);
 
 /* ImplicitNet.forward (networks.py:126-208): x [N,d_in] -> out [N,257] (sdf | feature).

@@ -1,2 +1,2 @@
-"""multiply_b200 — B200-native (sm_100a) implementation of MultiPly's volume-rendering hot path."""
+"""multiply_b200 — H100-native (sm_90a) implementation of MultiPly's volume-rendering hot path."""
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-// Shared declarations of the multiply_b200 CUDA library (sm_100a only).
+// Shared declarations of the multiply_b200 CUDA library (sm_90a only).
 #pragma once
 #include <atomic>
 #include <cuda_runtime.h>
@@ -121,7 +121,7 @@ struct Field {
   int ren_in[MP_MAX_LAYERS], ren_out[MP_MAX_LAYERS];
   int ren_extra;          // leading inputs of colour layer 0 handled outside the 256-wide feature block
   // fp32 SIMT layout: Wt[l] is [in][out] (transposed), folded weight norm / skip scale
-  float* imp_W[MP_MAX_LAYERS];      // natural [out][in] (backward pass, tcgen05 packing)
+  float* imp_W[MP_MAX_LAYERS];      // natural [out][in] (backward pass, tensor-core packing)
   float* ren_W[MP_MAX_LAYERS];
   float* imp_Wt[MP_MAX_LAYERS];
   float* imp_b[MP_MAX_LAYERS];     // layer 0: raw bias; imp_b0_eff has the cond folded in
@@ -134,8 +134,8 @@ struct Field {
   float* ren_b0_base;              // [out0] : b0 + W0[:,6:14] @ lin_pose.b  (mode 0) ; b0 (mode 1)
   int ren_cond_dim;
   float* ren_cb;                   // [out0] Wc0[:, feat] . b8[1:]  (colour layer 0 folded onto the feature layer)
-  float* ren_b0_fold;              // [out0] ren_b0_eff + ren_cb : bias of the folded layer (tcgen05 chains)
-  // tcgen05 engine blobs (mlp_tc.cu); null until packed
+  float* ren_b0_fold;              // [out0] ren_b0_eff + ren_cb : bias of the folded layer (tensor-core chains)
+  // tensor-core engine blobs (mlp_tc.cu); null until packed
   void* tc;
   char* storage;
   size_t storage_bytes;

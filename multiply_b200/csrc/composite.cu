@@ -4,7 +4,7 @@
 //   render_weight_from_density / pack_info / accumulate_along_rays (:455-478), and the
 //   background transmittance taken at the START of each ray's last sample (:457-463).
 //
-// B200 design: no global sort.  Each person's per-ray list is already sorted, so one warp per
+// Design: no global sort.  Each person's per-ray list is already sorted, so one warp per
 // ray merges the P lists by rank (binary searches in shared memory), scans sigma*delta with a
 // warp scan and reduces the weighted sums in registers — one kernel, one pass over the samples.
 // Tie order on equal t_end: (person, sample) ascending — the order oracle/port.py uses.

@@ -2,7 +2,7 @@
 //   reference: /root/reference/code/lib/model/deformer.py:19-50 (forward, forward_skinning,
 //   query_skinning_weights_smpl_multi), :72-89 (skinning) and the pytorch3d knn_points call at :39.
 //
-// B200 design: the 6890 vertices are binned into a uniform grid (cell >= the 0.1 outlier
+// Design: the 6890 vertices are binned into a uniform grid (cell >= the 0.1 outlier
 // radius of deformer.py:49) and stored cell-sorted as float4 (x,y,z,index) so that one warp of
 // neighbouring sample points streams the same few cells with 128-bit loads out of L1.  The
 // nearest vertex is EXACT: d2 = (dx*dx + dy*dy) + dz*dz with separately rounded operations and

@@ -142,7 +142,7 @@ int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, in
     nat[l] = a.take<float>((size_t)o * in);
     f.imp_W[l] = nat[l];
     f.imp_Wt[l] = a.take<float>((size_t)in * o);
-    f.imp_b[l] = a.take<float>(o < 264 ? 264 : o);   // padded: the tcgen05 epilogue reads 256 columns
+    f.imp_b[l] = a.take<float>(o < 264 ? 264 : o);   // padded: the tensor-core epilogue reads 256 columns
     if (!a.ok) break;
     float scale = (l == f.skip_layer) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
     rc = fold(imp->lin.weight_v[l], imp->lin.weight_g[l], o, in, scale, nat[l], st);

@@ -3,7 +3,7 @@
 //              :263-312 (RenderingNet.forward), embedders.py:8-34,
 //              lib/model/multiply.py:620-661 (forward_gradient: d sdf / d x_c, normals)
 // Plain tiled SGEMM per layer with the activation fused into the store; activations live in
-// global memory between layers.  It exists so that the tcgen05 engine (mlp_tc.cu) can be
+// global memory between layers.  It exists so that the tensor-core engine (mlp_tc.cu) can be
 // checked against an independent fp32 implementation ON THE GPU and so the pipeline is
 // testable end to end; it is not the fast path.
 #include "common.cuh"

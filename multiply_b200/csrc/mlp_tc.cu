@@ -1,25 +1,30 @@
-// tcgen05 engine: the fused ImplicitNet (+ backward for normals) + RenderingNet chain on the
-// 5th-generation tensor cores of sm_100a.
-//   reference: /root/reference/code/lib/model/networks.py:126-208 (ImplicitNet.forward),
+// Tensor-core engine: the fused ImplicitNet (+ backward for normals) + RenderingNet chain on the
+// Hopper tensor cores of sm_90a (wgmma, TMA bulk copies, mbarrier).
+//   reference: lib/model/networks.py:126-208 (ImplicitNet.forward),
 //              :263-312 (RenderingNet.forward), lib/model/multiply.py:620-661 (forward_gradient)
 //
 // Design (DESIGN.md §3.1):
-//   * one persistent CTA per SM; a tile is 128 sample points (MMA M = 128, cta_group::1).
-//   * every layer is D[128 x 256] (fp32, 256 TMEM columns) = A[128 x K] . W^T, K in chunks of 64.
-//     A (the activations) lives in shared memory as fp16 hi + fp16 lo (K-major, 128B swizzle);
-//     the weights are streamed as pre-swizzled fp16 hi/lo tiles ("slots", 256 x 64, 32 KB) by
-//     the TMA engine (cp.async.bulk + mbarrier complete_tx) through a 3-slot ring.
-//   * split precision: D = A_hi.W_hi + A_lo.W_hi + A_hi.W_lo (three kind::f16 MMAs per K-step,
+//   * one persistent CTA per SM; a tile is 128 sample points.  Two consumer warpgroups own 64 rows each and
+//     run the whole chain of their rows: every layer is D[64 x 256] (fp32, in registers) = A[64 x K] . W^T,
+//     K in chunks of 64, as wgmma.m64n256k16 issued by the warpgroup.
+//     A (the activations) lives in shared memory as fp16 hi + fp16 lo (K-major, 128B swizzle).  A warpgroup
+//     only ever reads and writes its own 64 rows of A, so handing the operand to the next layer is a
+//     128-thread barrier, and the two warpgroups drift freely against each other (one's epilogue overlaps
+//     the other's MMAs).
+//   * the weights are streamed as pre-swizzled fp16 hi/lo tiles ("slots", 256 x 64, 32 KB) by the
+//     TMA engine (cp.async.bulk + mbarrier complete_tx) through a 3-slot ring that both warpgroups read.
+//   * split precision: D = A_hi.W_hi + A_lo.W_hi + A_hi.W_lo (three f16 MMAs per K-step,
 //     fp32 accumulate) — 22 significand bits per operand, which is what keeps RGB/SDF within the
 //     1e-4 gate that a single bf16/fp16 pass misses by two orders of magnitude.
-//   * warp roles: warp 0 = weight loader, warp 1 = MMA issuer (one elected lane),
-//     warps 2..17 = epilogue (TMEM -> registers -> activation -> fp16 hi/lo -> shared memory):
-//     TMEM lane quadrant x column part; a part owns 16 columns of each 64-wide K-block of the next
-//     operand and hands them over K-block by K-block, so the next layer's MMAs start after a quarter
-//     of the epilogue, into the other of two accumulators (512 TMEM columns in all).
+//   * warp roles: warpgroup 0 = weight loader (one lane), warpgroups 1, 2 = MMA issue + epilogue
+//     (accumulator registers -> activation -> fp16 hi/lo -> shared memory through stmatrix).
 //   * the whole per-sample chain runs inside the tile: embed, L0..L7 (+ sigma' stash), SDF dot,
 //     the reverse sweep B7..B0 (d sdf / d x_c), normals, colour layers (the feature layer L8 folded
 //     into colour layer 0, its extra inputs as a fifth K-block), RGB.
+//
+// Accumulator layout of wgmma.m64n256k16 (f32): thread t of a warpgroup (warp w = t / 32, lane l) holds
+// register i at row 16 w + l / 4 + 8 ((i >> 1) & 1) and column 8 (i >> 2) + 2 (l % 4) + (i & 1): two rows, 64
+// columns each.  Per-row results (dots, normals) are reduced over the four lanes of a quad.
 #include "common.cuh"
 #include <vector>
 #include <mutex>
@@ -87,25 +92,25 @@ struct TcIO {
   float* nrm_out;        // [slots,3]
   float* grad_out;       // [cap,3] dense or nullptr
   float* feat_out;       // [cap,256] dense or nullptr
-  int knobs;             // diagnostics (MP_TC_KNOBS bit mask): bit 1 = record the cycle stamps of mp_tc_trace_read,
-                         // bit 2 = keep the dead scratch lines (no discard.global.L2)
+  int knobs;             // diagnostics (MP_TC_KNOBS bit mask): bit 2 = keep the dead scratch lines (no discard.global.L2)
   float rz;              // relative truncation loss of ONE tensor-core accumulation (see kRzPerMma)
   char* scratch;         // per-CTA scratch
   size_t scratch_per_cta;
 };
 
-// per-CTA scratch layout (bytes)
-constexpr size_t kSigBytes = (size_t)8 * 64 * 128 * 16;      // sigma' [8][64][128] float4
-constexpr size_t kFeatBytes = (size_t)2 * 32 * 128 * 16;     // features hi/lo chunks
-constexpr size_t kGeBytes = (size_t)96 * 128 * 4;            // skip gradient [E<=96][128]
-constexpr size_t kMiscBytes = (size_t)128 * 32 * 4;          // partial sums / normals [128][32]
-constexpr size_t kEmbBytes = (size_t)96 * 128 * 4;           // input embedding of the tile [E<=96][128]
-constexpr size_t kScratchPerCta = kSigBytes + kFeatBytes + kGeBytes + kMiscBytes + kEmbBytes;
+constexpr int kConsumers = 2;                                 // consumer warpgroups (64 rows each)
+constexpr int kThreads = 128 * (1 + kConsumers);
+
+// per-CTA scratch layout (bytes); sigma' and the stashed features are indexed by (warpgroup, register group, thread)
+constexpr size_t kSigBytes = (size_t)8 * kConsumers * 32 * 128 * 16;   // sigma' [8][2][32][128] float4
+constexpr size_t kFeatBytes = (size_t)kConsumers * 32 * 128 * 16;      // features [2][hi 16 | lo 16][128] uint4
+constexpr size_t kGeBytes = (size_t)96 * 128 * 4;            // skip gradient [E<=96][128 rows]
+constexpr size_t kEmbBytes = (size_t)96 * 128 * 4;           // input embedding of the tile [E<=96][128 rows]
+constexpr size_t kScratchPerCta = kSigBytes + kFeatBytes + kGeBytes + kEmbBytes;
 
 // shared memory carve-up
 constexpr int kABytes = 2 * 4 * 128 * 128;                   // hi + lo, 4 K-blocks of [128 x 128B]
-constexpr int kXchBytes = 2 * 128 * 4;                        // d sdf / d x_1, d x_2 of the tile's rows (final-gradient step)
-constexpr int kSmemBytes = kABytes + kRing * kSlotBytes + 256 + kXchBytes + 1024;
+constexpr int kSmemBytes = kABytes + kRing * kSlotBytes + 256 + 1024;
 static_assert(kSmemBytes <= 232448, "shared memory budget of one CTA (227 KB)");
 
 // ---------------------------------------------------------------------------------------------
@@ -141,48 +146,55 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// barrier of one consumer warpgroup (ids 1, 2)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// The MMAs write the accumulator registers asynchronously: after a wait, this tells the compiler that every register
+// may have changed, so that no read of the accumulator is scheduled before the wait.
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define MP_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define MP_D16(i) MP_D4(i), MP_D4(i + 4), MP_D4(i + 8), MP_D4(i + 12)
+// D[64 x 256] (+)= A[64 x 16] . B[256 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : MP_D16(0), MP_D16(16), MP_D16(32), MP_D16(48), MP_D16(64), MP_D16(80), MP_D16(96), MP_D16(112)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
+#undef MP_D16
+#undef MP_D4
 
-// K-major, 128-byte swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
+// K-major, 128-byte swizzle shared-memory matrix descriptor of wgmma:
 //   [0,14) start>>4, [16,30) LBO>>4 (unused for swizzled K-major, 1), [32,46) SBO>>4 = 1024B between
-//   8-row groups, [46,48) version = 1 (sm_100), [61,64) layout = 2 (SWIZZLE_128B)
+//   8-row groups, [62,64) layout = 1 (SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// kind::f16 instruction descriptor: D = F32, A = B = F16, both K-major, N = 256, M = 128
-__device__ __forceinline__ uint32_t make_idesc() { return (1u << 4) | ((256u >> 3) << 17) | ((128u >> 4) << 24); }
 
 // ---------------------------------------------------------------------------------------------
 // epilogue helpers
@@ -192,25 +204,27 @@ __device__ __forceinline__ uint32_t a_off(int row, int kb, int ch) {
   return (uint32_t)(kb * 16384 + row * 128 + ((ch ^ (row & 7)) << 4));
 }
 
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __half2 h = __floats2half2_rn(a, b);
+  float2 f = __half22float2(h);
+  __half2 l = __floats2half2_rn(a - f.x, b - f.y);
+  hi = *(uint32_t*)&h;
+  lo = *(uint32_t*)&l;
+}
 __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
-  __half2 h[4], l[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    float2 f = __half22float2(h[i]);
-    l[i] = __floats2half2_rn(v[2 * i] - f.x, v[2 * i + 1] - f.y);
-  }
-  hi = make_uint4(*(uint32_t*)&h[0], *(uint32_t*)&h[1], *(uint32_t*)&h[2], *(uint32_t*)&h[3]);
-  lo = make_uint4(*(uint32_t*)&l[0], *(uint32_t*)&l[1], *(uint32_t*)&l[2], *(uint32_t*)&l[3]);
+  split2(v[0], v[1], hi.x, lo.x);
+  split2(v[2], v[3], hi.y, lo.y);
+  split2(v[4], v[5], hi.z, lo.z);
+  split2(v[6], v[7], hi.w, lo.w);
 }
 
-// 16-byte store into the operand image through a 32-bit shared-window address.  (A pointer derived from the aligned
-// dynamic-shared base loses its address space: the compiler emitted generic ST.E.128 with 64-bit address arithmetic.)
-// (volatile, no memory clobber: ordered against the volatile proxy fence / mbarrier arrive that publish the image; no
-// C++ access reads these bytes back.)
+// 16-byte store into the operand image through a 32-bit shared-window address.
+// (volatile, no memory clobber: ordered against the volatile proxy fence that publishes the image; no C++ access reads
+// these bytes back.)
 __device__ __forceinline__ void sts128(uint32_t A32, uint32_t off, const uint4& v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(A32 + off), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
 }
+// eight consecutive columns of one row
 __device__ __forceinline__ void store_a8(uint32_t A32, int row, int col, const float* v) {
   uint4 hi, lo;
   split8(v, hi, lo);
@@ -218,18 +232,34 @@ __device__ __forceinline__ void store_a8(uint32_t A32, int row, int col, const f
   sts128(A32, o, hi);
   sts128(A32, 65536 + o, lo);
 }
+__device__ __forceinline__ void stsm4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t e) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
+               "r"(e));
+}
+// Accumulator registers 8 jp .. 8 jp + 7 (columns 16 jp .. 16 jp + 15 of the thread's two rows), already split into
+// fp16 hi / lo pairs, -> A.  stmatrix writes four 8 x 8 blocks: (column group 2 jp, rows 0-7 | rows 8-15 of the warp's
+// 16), then column group 2 jp + 1; lane l gives the address of row l % 8 of block l / 8.  `lane_base` is A + that
+// row * 128, `lane_x` the swizzle term ((l / 16) ^ (row & 7)) of the block's 16-byte chunk.
+__device__ __forceinline__ void store_pairs(uint32_t lane_base, uint32_t lane_x, int jp, const uint4& hi, const uint4& lo) {
+  const uint32_t addr = lane_base + (uint32_t)(jp >> 2) * 16384u + ((((uint32_t)(2 * jp) & 7u) ^ lane_x) << 4);
+  stsm4(addr, hi.x, hi.y, hi.z, hi.w);
+  stsm4(addr + 65536u, lo.x, lo.y, lo.z, lo.w);
+}
+__device__ __forceinline__ void store_acc16(uint32_t lane_base, uint32_t lane_x, int jp, const float* v) {
+  uint4 hi, lo;
+  split8(v, hi, lo);
+  store_pairs(lane_base, lane_x, jp, hi, lo);
+}
 
-// element k of the positional embedding of x (embedders.py:8-34)
-__device__ __forceinline__ float embed_elem(const float* x, int d, int k) {
-  if (k < d) return x[k];
-  int f = (k - d) / (2 * d), r = (k - d) - f * 2 * d;
-  float t = __fmul_rn(x[r < d ? r : r - d], (float)(1 << f));
-  return r < d ? sinf(t) : cosf(t);
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
 }
 
 // The per-CTA scratch (sigma', stashed features) streams: it is written once and read once per tile.  L2-only
 // accesses keep it out of the small L1 that is left beside 224 KB of shared memory, so that the read-only vectors
-// every chunk needs (bias, W8 row, extra-input and rgb weights) stay L1-resident.
+// every column group needs (bias, W8 row, rgb weights) stay L1-resident.
 __device__ __forceinline__ float4 ld_stream(const float4* p) {
   float4 v;
   asm volatile("ld.global.cg.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
@@ -258,12 +288,9 @@ __device__ __forceinline__ void discard_line(const void* p, uint32_t dep) {
   asm volatile("discard.global.L2 [%0], 128;" ::"l"(p), "r"(dep) : "memory");
 }
 
-template <int N>
-__device__ __forceinline__ void ep_bar() { asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory"); }
-
 // softplus(beta=100, threshold=20) and its derivative (networks.py:85)
-// Branch-free so that the elements of a chunk pipeline through the MUFU unit (a per-element branch serialises
-// them: measured 5x slower).  Raw MUFU approximations (ex2 / lg2 / rcp .approx.ftz) without the
+// Branch-free so that the elements pipeline through the MUFU unit (a per-element branch serialises
+// them).  Raw MUFU approximations (ex2 / lg2 / rcp .approx.ftz) without the
 // denormal fix-ups of __expf/__logf: 1+u >= 1, the overflow side is replaced by the linear branch, results only need
 // ~1e-7 absolute accuracy (softplus = log1p(exp(100 z))/100).
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -301,95 +328,19 @@ __device__ __forceinline__ void softplus_fast_grad(float z, float& y, float& d) 
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
-// tcgen05.ld is asynchronous: `tmem_issue` starts the load of CW columns of this thread's row, `tmem_wait`
-// (tcgen05.wait::ld) makes the registers valid.  The wait lists the destination registers as in/out
-// operands so the compiler cannot touch them between the two.
-template <int CW>
-__device__ __forceinline__ void tmem_issue(uint32_t taddr, float* v);
-template <>
-__device__ __forceinline__ void tmem_issue<32>(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-template <>
-__device__ __forceinline__ void tmem_issue<16>(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-template <int CW>
-__device__ __forceinline__ void tmem_wait(float* v);
-template <>
-__device__ __forceinline__ void tmem_wait<16>(float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-template <>
-__device__ __forceinline__ void tmem_wait<32>(float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]),
-                 "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]),
-                 "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-// Step kinds: the chunk loop of a layer step is compiled once per kind (compile-time tag), so that every kind gets its own
-// instruction schedule and register allocation instead of one loop that tests the step descriptor in its body.  (The
-// single generic loop of round 1 was at the mercy of the optimiser: unrelated edits elsewhere in the kernel moved the
-// forward steps between 13.5 k and 18 k cycles.)
+// Step kinds: the epilogue of a layer step is compiled once per kind (compile-time tag), so that every kind gets its own
+// instruction schedule and register allocation instead of one loop that tests the step descriptor in its body.
 enum { K_SP_PLAIN = 0, K_SP_SAVE = 1, K_SP_SEED = 2, K_FEAT = 3, K_BWD = 4, K_RELU = 5 };
 template <int K>
 struct KTag {
   static constexpr int value = K;
 };
 
-// cycle stamps of CTA 0 (MP_TC_KNOBS bit 1): [0..] epilogue warp 2, [2048..] MMA issuer; see mp_tc_trace_read
-#ifndef MP_TC_TRACE
-#define MP_TC_TRACE 0
-#endif
+// kept for the mp_tc_trace_read ABI (cycle stamps of an instrumented build)
 __device__ unsigned long long g_trace[4096];
 
-// NW epilogue warps (8 or 16): warp w owns TMEM lane quadrant w % 4 (rows) and column part (w-2)/4.
-//
-// PIPE (NW = 16 only): K-block-granular hand-over between the epilogue and the MMA issuer.
-//   * a column part no longer owns one 64-column K-block of the next layer's operand; it owns 16 columns of
-//     each of the four, visited in K-block order, and arrives on a per-K-block barrier after each chunk.  The
-//     next layer's MMAs over K-block kb therefore start after a quarter of the epilogue instead of after all
-//     of it;
-//   * those MMAs write a second accumulator (TMEM columns 256..511, alternating per step) because the
-//     epilogue is still draining the first.
-//   The operand A stays single-buffered: all MMAs of a step have completed before its epilogue starts.
-template <int NW, bool PIPE>
-__global__ void __launch_bounds__(64 + 32 * NW, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
-                                                                   const __grid_constant__ TcIO io) {
-  static_assert(!PIPE || NW == 16, "PIPE needs four column parts of 16-column chunks");
-  constexpr int NBAR = PIPE ? 4 : 1;       // operand hand-over barriers (one per K-block when pipelined)
-  constexpr int TCOLS = PIPE ? 512 : 256;  // TMEM columns
-  constexpr int NPART = NW / 4;            // column parts
-  constexpr int PCOLS = 256 / NPART;       // columns per part
-  constexpr int CW = (NW == 16) ? 16 : 32; // columns per TMEM load (register budget)
-  constexpr int G4 = CW / 4;
-  constexpr int NEPI = 32 * NW;
+__global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
+                                                               const __grid_constant__ TcIO io) {
   extern __shared__ uint8_t smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // 1024-byte aligned carve-up (SWIZZLE_128B atoms)
@@ -400,12 +351,6 @@ __global__ void __launch_bounds__(64 + 32 * NW, 1) tc_chain_kernel(const __grid_
   uint64_t* bars = (uint64_t*)(ring + kRing * kSlotBytes);
   uint64_t* full = bars;                            // [kRing]
   uint64_t* empty = bars + kRing;                   // [kRing]
-  uint64_t* d_full = bars + 2 * kRing;
-  uint64_t* a_ready = bars + 2 * kRing + 1;
-  uint64_t* x_free = bars + 2 * kRing + 1 + NBAR;      // K-block 0 of A drained by the MMAs (extra-input steps)
-  uint64_t* x_ready = x_free + 1;                      // extra inputs staged there
-  uint32_t* tmem_slot = (uint32_t*)(x_ready + 1);
-  float* xs = (float*)((char*)bars + 256);             // [2][128] exchange of the final-gradient step
 
   const int count = io.count ? min(io.cap, *io.count) : io.cap;
   const int ntiles = (count + 127) >> 7;
@@ -413,28 +358,16 @@ __global__ void __launch_bounds__(64 + 32 * NW, 1) tc_chain_kernel(const __grid_
   if (threadIdx.x == 0) {
     for (int i = 0; i < kRing; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
+      mbar_init(&empty[i], 4 * kConsumers);      // one arrival per consumer warp
     }
-    mbar_init(d_full, 1);
-    for (int i = 0; i < NBAR; ++i) mbar_init(&a_ready[i], NEPI);
-    mbar_init(x_free, 1);
-    mbar_init(x_ready, NEPI);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(TCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem0 = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== weight loader =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         for (int s = 0; s < P.nsteps; ++s) {
@@ -451,597 +384,428 @@ __global__ void __launch_bounds__(64 + 32 * NW, 1) tc_chain_kernel(const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc();
-      const uint32_t a_hi = smem_u32(A), a_lo = smem_u32(A) + 65536;
-      uint32_t it = 0, ar_ph = 0, buf = 0, xr_ph = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        for (int s = 0; s < P.nsteps; ++s) {
-          if (!PIPE) {
-            mbar_wait(a_ready, ar_ph);
-            tc_fence_after();
-          }
-          const int nk = P.step[s].nk;
-          const bool one_term = P.step[s].terms == 1;
-          const uint32_t tmem = tmem0 + (PIPE ? buf * 256u : 0u);
-          uint32_t acc = 0;
-          for (int kc = 0; kc < nk; ++kc) {
-            if (kc == 4) {
-              // extra-input K-block: lives where K-block 0 was
-              mbar_wait(x_ready, xr_ph);
-              xr_ph ^= 1;
-              tc_fence_after();
-            } else if (PIPE) {
-              mbar_wait(&a_ready[kc], ar_ph);
-              tc_fence_after();
-#if MP_TC_TRACE
-              if ((io.knobs & 2) && blockIdx.x == 0 && tile == (int)(blockIdx.x + gridDim.x)) g_trace[2048 + (P.nsteps > 12 ? 0 : 1024) + s * 8 + kc] = clock64();
-#endif
-            }
-            // hi slot: A_hi.W_hi + A_lo.W_hi
-            int r = it % kRing;
-            mbar_wait(&full[r], (it / kRing) & 1);
-            tc_fence_after();
-            uint32_t wb = smem_u32(ring + (size_t)r * kSlotBytes);
+    return;
+  }
+  // ===================== consumer warpgroups: MMAs + epilogue =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int g = (warp >> 2) - 1;                 // consumer warpgroup: tile rows 64 g .. 64 g + 63
+  const int t = threadIdx.x & 127;               // thread in the warpgroup
+  const int wq = warp & 3, q = lane & 3;
+  const int bar_id = 1 + g;
+  int rowt[2];                                   // this thread's two tile rows
+  rowt[0] = 64 * g + 16 * wq + (lane >> 2);
+  rowt[1] = rowt[0] + 8;
+  // stmatrix addressing (store_pairs)
+  const int mi = lane >> 3, rr = lane & 7;
+  const uint32_t lane_base = A32 + (uint32_t)(64 * g + 16 * wq + 8 * (mi & 1) + rr) * 128u;
+  const uint32_t lane_x = (uint32_t)((mi >> 1) ^ rr);
+  const uint32_t a_hi = A32 + (uint32_t)g * 8192u, a_lo = a_hi + 65536u;   // this warpgroup's 64 rows of A
+
+  char* scr = io.scratch + (size_t)blockIdx.x * io.scratch_per_cta;
+  float4* sig = (float4*)scr;                                  // [8][2][32][128]
+  uint4* fsc = (uint4*)(scr + kSigBytes) + (size_t)g * 32 * 128;   // [hi 16 | lo 16][128] of this warpgroup
+  float* ge = (float*)(scr + kSigBytes + kFeatBytes);          // [96][128]
+  float* emb = (float*)(scr + kSigBytes + kFeatBytes + kGeBytes);   // [96][128]
+  const int d = P.d_in, E = P.E;
+  const bool keep_lines = (io.knobs & 4) != 0;
+
+  float acc[128];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              uint64_t bd = make_desc(wb + ks * 32);
-              umma_f16(tmem, make_desc(a_hi + (kc & 3) * 16384 + ks * 32), bd, idesc, acc);
-              acc = 1;
-              if (!one_term) umma_f16(tmem, make_desc(a_lo + (kc & 3) * 16384 + ks * 32), bd, idesc, 1);
-            }
-            umma_commit(&empty[r]);
-            ++it;
-            if (!one_term) {
-            // lo slot: A_hi.W_lo
-            r = it % kRing;
-            mbar_wait(&full[r], (it / kRing) & 1);
-            tc_fence_after();
-            wb = smem_u32(ring + (size_t)r * kSlotBytes);
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  uint32_t it = 0;                               // ring position
+
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int pt[2], slot[2];
+    bool valid[2];
+    float x[2][4];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks)
-              umma_f16(tmem, make_desc(a_hi + (kc & 3) * 16384 + ks * 32), make_desc(wb + ks * 32), idesc, 1);
-            umma_commit(&empty[r]);
-            ++it;
-            }
-            if (kc == 0 && nk == 5) umma_commit(x_free);   // K-block 0 may be overwritten once these have completed
-          }
-          umma_commit(d_full);
-#if MP_TC_TRACE
-          if ((io.knobs & 2) && blockIdx.x == 0 && tile == (int)(blockIdx.x + gridDim.x)) g_trace[2048 + (P.nsteps > 12 ? 0 : 1024) + s * 8 + 4] = clock64();
-#endif
-          if (PIPE) {
-            // keep the phases of the unused K-block barriers in step
-            for (int kc = nk < 4 ? nk : 4; kc < 4; ++kc) mbar_wait(&a_ready[kc], ar_ph);
-            buf ^= 1;
-          }
-          ar_ph ^= 1;
+    for (int h = 0; h < 2; ++h) {
+      pt[h] = tile * 128 + rowt[h];
+      valid[h] = pt[h] < count;
+      for (int a = 0; a < 4; ++a) x[h][a] = 0.f;
+      if (valid[h])
+        for (int a = 0; a < d; ++a) x[h][a] = io.x[(size_t)pt[h] * d + a];
+      slot[h] = valid[h] ? (io.slot ? io.slot[pt[h]] : pt[h]) : 0;
+    }
+    // ---- tile prologue: embedding -> A (K-blocks 0 .. nk0-1), zero padded ----
+    {
+      // positional embedding (embedders.py:8-34): the (frequency, axis) pairs of a row are split over the four lanes
+      // that hold it, one sincosf each, parked in scratch so that the skip connection of layer 4 and the chain rule at
+      // the end of the reverse sweep re-read instead of recomputing them
+      const int npair = d * P.multires;
+      for (int pi = q; pi < npair; pi += 4) {
+        const int f = pi / d, a = pi - f * d;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float sn, cs;
+          sincosf(__fmul_rn(x[h][a], (float)(1 << f)), &sn, &cs);
+          emb[(size_t)(d + 2 * f * d + a) * 128 + rowt[h]] = sn;
+          emb[(size_t)(d + (2 * f + 1) * d + a) * 128 + rowt[h]] = cs;
         }
+      }
+      if (q == 0)
+        for (int a = 0; a < d; ++a)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) emb[(size_t)a * 128 + rowt[h]] = x[h][a];
+      if (io.extra) {
+        // background: embedding of the view direction (n_extra = 3 + 6 * frequencies values), same split
+        float dv[2][3];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          for (int a = 0; a < 3; ++a) dv[h][a] = valid[h] ? io.extra[(size_t)pt[h] * 3 + a] : 0.f;
+        const int nvp = (P.n_extra - 3) / 2;
+        for (int pi = q; pi < nvp; pi += 4) {
+          const int f = pi / 3, a = pi - f * 3;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float sn, cs;
+            sincosf(__fmul_rn(dv[h][a], (float)(1 << f)), &sn, &cs);
+            ge[(size_t)(3 + 6 * f + a) * 128 + rowt[h]] = sn;
+            ge[(size_t)(3 + 6 * f + 3 + a) * 128 + rowt[h]] = cs;
+          }
+        }
+        if (q == 0)
+          for (int a = 0; a < 3; ++a)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) ge[(size_t)a * 128 + rowt[h]] = dv[h][a];
+      }
+      __threadfence_block();
+      wg_sync(bar_id);
+      const int njp = P.step[0].nk * 4;
+      for (int jp = 0; jp < njp; ++jp) {
+        float v[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int c = 16 * jp + 8 * (i >> 2) + 2 * q + (i & 1);
+          v[i] = (c < E) ? emb[(size_t)c * 128 + rowt[(i >> 1) & 1]] : 0.f;
+        }
+        store_acc16(lane_base, lane_x, jp, v);
       }
     }
-  } else {
-    // ===================== epilogue warps =====================
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int part = (warp - 2) >> 2;       // column part
-    const int row = q * 32 + lane;
-    const uint32_t t_row0 = tmem0 + ((uint32_t)(q * 32) << 16);
-    uint32_t ebuf = 0;                       // accumulator the next step drains (PIPE)
-    char* scr = io.scratch + (size_t)blockIdx.x * io.scratch_per_cta;
-    float4* sig = (float4*)scr;                                  // [8][64][128]
-    uint4* fsc = (uint4*)(scr + kSigBytes);                      // [2][32][128]
-    float* ge = (float*)(scr + kSigBytes + kFeatBytes);          // [96][128]
-    float* misc = (float*)(scr + kSigBytes + kFeatBytes + kGeBytes);   // [128][32]
-    float* emb = (float*)(scr + kSigBytes + kFeatBytes + kGeBytes + kMiscBytes);   // [96][128]
-    uint32_t df_ph = 0, xf_ph = 0;
-    const int d = P.d_in, E = P.E;
-    const int cbeg = part * PCOLS;
-    constexpr int NCH = PCOLS / CW;          // chunks per thread and step
-    // first column of this thread's i-th chunk: contiguous, or 16 columns of every K-block in K order (PIPE)
-    auto col_of = [&](int i) { return PIPE ? i * 64 + part * CW : cbeg + i * CW; };
-#ifndef MP_AOFF
-#define MP_AOFF 1
-#endif
-#if MP_AOFF
-    static_assert(PIPE && CW == 16, "precomputed operand offsets assume 16-column chunks in K order");
-    const uint32_t aoff0 = a_off(row, 0, (part * 2) & 7), aoff1 = a_off(row, 0, (part * 2 + 1) & 7);
-#endif
-    auto arrive_all = [&]() {
+    // colour-net extra inputs: foreground [x_c, n] (networks.py:281) live in registers (n arrives at the end of the
+    // reverse sweep); the background view-dir embedding (:275) was parked in `ge` by the prologue
+    float nrm[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    for (int s = 0; s < P.nsteps; ++s) {
+      const TcStep st = P.step[s];
+      // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
+      const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
+      const bool one_term = st.terms == 1;
+
+      // ---------------- MMAs: acc = A . W^T over st.nk K-blocks ----------------
+      // this warpgroup's rows of A are complete: publish them to the tensor cores
       fence_async_smem();
-      tc_fence_before();
-#pragma unroll
-      for (int i = 0; i < NBAR; ++i) mbar_arrive(&a_ready[i]);
-    };
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      const int pt = tile * 128 + row;
-      const bool valid = pt < count;
-      float x[4] = {0.f, 0.f, 0.f, 0.f};
-      if (valid)
-        for (int a = 0; a < d; ++a) x[a] = io.x[(size_t)pt * d + a];
-      const int slot = valid ? (io.slot ? io.slot[pt] : pt) : 0;
-      // ---- tile prologue: embedding -> A (K-blocks 0 .. nk0-1), zero padded ----
-      {
-        // positional embedding (embedders.py:8-34): the (frequency, axis) pairs of a row are split over its
-        // column-part threads, one sincosf each, parked in scratch so that the skip connection of layer 4 and
-        // the chain rule at the end of the reverse sweep re-read instead of recomputing them
-        const int npair = d * P.multires;
-        for (int pi = part; pi < npair; pi += NPART) {
-          int f = pi / d, a = pi - f * d;
-          float sn, cs;
-          sincosf(__fmul_rn(x[a], (float)(1 << f)), &sn, &cs);
-          emb[(size_t)(d + 2 * f * d + a) * 128 + row] = sn;
-          emb[(size_t)(d + (2 * f + 1) * d + a) * 128 + row] = cs;
+      wg_sync(bar_id);
+      wgmma_fence();
+      // Every weight slot's MMAs form one commit group.  A slot is released as soon as the group after it has been
+      // committed and all but that newest group have completed, so a warpgroup holds at most one slot in flight while
+      // it waits for the next: the ring (3 slots) never waits on a slot that its own reader still holds.
+      bool held = false;                         // a slot whose MMAs may still be running
+      uint32_t held_slot = 0;
+      auto release = [&](uint32_t slot_it) {
+        if (lane == 0) mbar_arrive(&empty[slot_it % kRing]);
+      };
+      auto slot_issued = [&](uint32_t slot_it) {
+        wgmma_commit();
+        if (held) {
+          wgmma_wait<1>();
+          release(held_slot);
         }
-        if (part == 0)
-          for (int a = 0; a < d; ++a) emb[(size_t)a * 128 + row] = x[a];
-        if (io.extra) {
-          // background: embedding of the view direction (n_extra = 3 + 6 * frequencies values), same split
-          float dv[3] = {0.f, 0.f, 0.f};
-          if (valid)
-            for (int a = 0; a < 3; ++a) dv[a] = io.extra[(size_t)pt * 3 + a];
-          const int nvp = (P.n_extra - 3) / 2;
-          for (int pi = part; pi < nvp; pi += NPART) {
-            int f = pi / 3, a = pi - f * 3;
-            float sn, cs;
-            sincosf(__fmul_rn(dv[a], (float)(1 << f)), &sn, &cs);
-            ge[(size_t)(3 + 6 * f + a) * 128 + row] = sn;
-            ge[(size_t)(3 + 6 * f + 3 + a) * 128 + row] = cs;
-          }
-          if (part == 0)
-            for (int a = 0; a < 3; ++a) ge[(size_t)a * 128 + row] = dv[a];
-        }
-        __threadfence_block();
-        ep_bar<NEPI>();
-        const int ncol = P.step[0].nk * 64;
-        const int c0 = part * (ncol / NPART), c1 = c0 + ncol / NPART;
-        for (int c = c0; c < c1; c += 8) {
-          float v[8];
+        held = true;
+        held_slot = slot_it;
+      };
+      for (int kc = 0; kc < st.nk; ++kc) {
+        if (kc == 4) {
+          // extra-input K-block (colour layer 0): once the MMAs over K-block 0 have drained it, this row's extra inputs
+          // (16 columns per lane of the quad, zero padded to 64) take its place and accumulate into the same tile
+          wgmma_wait<0>();
+          acc_fence(acc);
+          if (held) release(held_slot);
+          held = false;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = (c + j < E) ? emb[(size_t)(c + j) * 128 + row] : 0.f;
-          store_a8(A32, row, c, v);
-        }
-        arrive_all();
-      }
-      // colour-net extra inputs: foreground [x_c, n] (networks.py:281) live in registers (n arrives at the end of the
-      // reverse sweep); the background view-dir embedding (:275) was parked in `ge` by the prologue
-      float nrm[3] = {0.f, 0.f, 0.f};
-      for (int s = 0; s < P.nsteps; ++s) {
-        const TcStep st = P.step[s];
-        // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
-        const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
-        // reverse-sweep steps: start fetching sigma' of the first chunk before blocking on the accumulator
-        float4 s4[G4];
-        const bool need_sig = (st.epi == EPI_BWD) && st.sig >= 0;
+          for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int g4 = 0; g4 < G4; ++g4) s4[g4] = make_float4(0.f, 0.f, 0.f, 0.f);      // (always initialised: see b4 below)
-        if (need_sig) {
+            for (int c8 = 0; c8 < 16; c8 += 8) {
+              const int e0 = 16 * q + c8;
+              float xv[8];
 #pragma unroll
-          for (int g4 = 0; g4 < G4; ++g4) s4[g4] = ld_stream(&sig[((size_t)st.sig * 64 + ((col_of(0) >> 2) + g4)) * 128 + row]);
-        }
-        if (st.nk == 5) {
-          // colour layer 0: once the MMAs over K-block 0 have drained it, this row's extra inputs (16 columns per
-          // column part, zero padded to 64) take its place as the fifth K-block of the same accumulation
-          mbar_wait(x_free, xf_ph);
-          xf_ph ^= 1;
-          constexpr int XC = 64 / NPART;       // columns of the extra K-block staged by each column part
+              for (int j = 0; j < 8; ++j) xv[j] = 0.f;
+              if (io.extra) {
 #pragma unroll
-          for (int c8 = 0; c8 < XC; c8 += 8) {
-            const int e0 = part * XC + c8;
-            float xv[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) xv[j] = 0.f;
-            if (io.extra) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                if (e0 + j < P.n_extra) xv[j] = ge[(size_t)(e0 + j) * 128 + row];
-            } else if (e0 == 0) {
-              xv[0] = x[0]; xv[1] = x[1]; xv[2] = x[2];
-              xv[3] = nrm[0]; xv[4] = nrm[1]; xv[5] = nrm[2];
+                for (int j = 0; j < 8; ++j)
+                  if (e0 + j < P.n_extra) xv[j] = ge[(size_t)(e0 + j) * 128 + rowt[h]];
+              } else if (e0 == 0) {
+                xv[0] = x[h][0]; xv[1] = x[h][1]; xv[2] = x[h][2];
+                xv[3] = nrm[h][0]; xv[4] = nrm[h][1]; xv[5] = nrm[h][2];
+              }
+              store_a8(A32, rowt[h], e0, xv);
             }
-            store_a8(A32, row, e0, xv);
           }
           fence_async_smem();
-          mbar_arrive(x_ready);
+          wg_sync(bar_id);
+          wgmma_fence();
         }
-        // cycle stamps of one tile (scripts/gpu_trace.py): compiled in only with -DMP_TC_TRACE=1 (scripts/build_variant.sh);
-        // even predicated off they cost ~1.5 % of the epilogue's issue slots
-#if MP_TC_TRACE
-        const bool tr = (io.knobs & 2) && blockIdx.x == 0 && warp == 2 && lane == 0 && tile == (int)(blockIdx.x + gridDim.x);
-#else
-        constexpr bool tr = false;
-#endif
-        unsigned long long* trp = g_trace + (P.nsteps > 12 ? 0 : 1024) + s * 8;
-        if (tr) trp[0] = clock64();
-        mbar_wait(d_full, df_ph);
-        df_ph ^= 1;
-        tc_fence_after();
-        if (tr) trp[1] = clock64();
-        auto reload_features = [&]() {
+        const uint32_t ka = (uint32_t)(kc & 3) * 16384u;
+        // hi slot: A_hi.W_hi + A_lo.W_hi
+        int r = it % kRing;
+        mbar_wait(&full[r], (it / kRing) & 1);
+        uint32_t wb = smem_u32(ring + (size_t)r * kSlotBytes);
 #pragma unroll
-          for (int c8 = 0; c8 < PCOLS / 8; c8 += 4) {
-            uint4 fh[4], fl[4];
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint64_t bd = make_desc(wb + ks * 32);
+          wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), bd, (kc | ks) != 0);
+          if (!one_term) wgmma_f16(acc, make_desc(a_lo + ka + ks * 32), bd, 1);
+        }
+        slot_issued(it++);
+        if (!one_term) {
+          // lo slot: A_hi.W_lo
+          r = it % kRing;
+          mbar_wait(&full[r], (it / kRing) & 1);
+          wb = smem_u32(ring + (size_t)r * kSlotBytes);
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int chunk = (cbeg >> 3) + c8 + u;
-              fh[u] = ld_stream(&fsc[(size_t)chunk * 128 + row]);
-              fl[u] = ld_stream(&fsc[(size_t)(32 + chunk) * 128 + row]);
-            }
+          for (int ks = 0; ks < 4; ++ks) wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), make_desc(wb + ks * 32), 1);
+          slot_issued(it++);
+        }
+      }
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (held) release(held_slot);
+
+      // ---------------- epilogue ----------------
+      auto reload_features = [&]() {
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int chunk = (cbeg >> 3) + c8 + u;
-              const uint32_t o = a_off(row, chunk >> 3, chunk & 7);
-              sts128(A32, o, fh[u]);
-              sts128(A32, 65536 + o, fl[u]);
-              if ((lane & 7) == 0 && !(io.knobs & 4)) {
-                discard_line(&fsc[(size_t)chunk * 128 + row], fh[u].x);
-                discard_line(&fsc[(size_t)(32 + chunk) * 128 + row], fl[u].x);
+        for (int jp = 0; jp < 16; ++jp) {
+          const uint4 fh = ld_stream(&fsc[(size_t)jp * 128 + t]);
+          const uint4 fl = ld_stream(&fsc[(size_t)(16 + jp) * 128 + t]);
+          store_pairs(lane_base, lane_x, jp, fh, fl);
+          if ((lane & 7) == 0 && !keep_lines) {
+            discard_line(&fsc[(size_t)jp * 128 + t], fh.x);
+            discard_line(&fsc[(size_t)(16 + jp) * 128 + t], fl.x);
+          }
+        }
+      };
+      if (st.flags & F_FINAL_GRAD) {
+        // ---- last step of the reverse sweep ----
+        // B0's output columns are permuted at pack time BY AXIS: columns [16 a, 16 a + 16) (a < d_in) hold every
+        // embedding index that depends on x_a -- [x_a, sin(2^0 x_a), cos(2^0 x_a), sin(2^1 x_a), ...]
+        // (embedders.py:8-34) -- so the chain rule
+        //   d sdf / d x_a = sum_k (g_k + skip_k) * d embed_k / d x_a
+        // of one axis lives in column groups 2 a, 2 a + 1, reduced over the quad.  The skip gradient (parked at the
+        // F_SKIP_GRAD step) and the partner sin / cos of each index (parked by the tile prologue) come from scratch.
+        float gax[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+        const int nterm = 1 + 2 * P.multires;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (j < 2 * d) {
+            const int a = j >> 1;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int jj = (8 * j + 2 * q + (e & 1)) & 15;
+              if (jj < nterm) {
+                const int h = e >> 1;
+                // jj = 0: x_a itself; jj = 1 + 2 f: sin(2^f x_a); jj = 2 + 2 f: cos(2^f x_a)
+                const int fq = (jj - 1) >> 1;
+                const bool is_cos = ((jj - 1) & 1) != 0;
+                const int k = (jj == 0) ? a : d + 2 * fq * d + (is_cos ? d : 0) + a;
+                const float pg = ge[(size_t)k * 128 + rowt[h]];
+                const float tot = fmaf(acc[4 * j + e], isc, pg);     // through layer 0 + through the skip connection
+                float w = 1.f;
+                if (jj > 0) {
+                  // partner: cos for a sin entry (+d), sin for a cos entry (-d)
+                  const float pe = emb[(size_t)(is_cos ? k - d : k + d) * 128 + rowt[h]];
+                  // d sin(2^f x) = 2^f cos(2^f x) ; d cos(2^f x) = -2^f sin(2^f x)
+                  w = (float)(1 << fq) * (is_cos ? -pe : pe);
+                }
+                gax[h][a] = fmaf(w, tot, gax[h][a]);
               }
             }
           }
-          arrive_all();
-        };
-        if (PIPE && (st.flags & F_FINAL_GRAD) && s + 1 < P.nsteps) {
-          // all MMAs of the reverse sweep are done, A is free: the features return for the colour net right away and
-          // its first layer's MMAs run under the rest of this step (the accumulators alternate)
-          reload_features();
-          if (tr) g_trace[512] = clock64();
         }
-        const uint32_t t_row = t_row0 + (PIPE ? ebuf * 256u : 0u);
-        ebuf ^= 1;
-        // steps whose operand for the next step is complete chunk by chunk (no tail rewrites A)
-        const bool chunk_handover = PIPE && s + 1 < P.nsteps && !(st.flags & (F_RGB_OUT | F_FINAL_GRAD));
-        float dot0 = 0.f, dot1 = 0.f, dot2 = 0.f;        // sdf / rgb partial dots
-        float va[CW];
-        // the accumulator registers are dead once a chunk has been split to fp16: the next chunk's TMEM load is
-        // started there, so its latency hides behind this chunk's stores and hand-over
-        auto issue_next = [&](const int ci) {
-          if (ci + 1 < NCH) tmem_issue<CW>(t_row + (uint32_t)col_of(ci + 1), va);
-        };
-        auto process_chunk = [&](auto ktag, float* v, const int ci) {
-          constexpr int KIND = decltype(ktag)::value;
-          const int c = col_of(ci);
-          // the bias of this chunk is fetched under the TMEM load
-          // (loaded unconditionally where the kind uses it and not declared live otherwise: a conditionally initialised
-          // array makes the compiler keep it in local memory -- 8 local loads / stores per chunk, measured 13.5 k -> 20 k
-          // cycles per forward step)
-          float4 b4[G4];
-          if constexpr (KIND != K_BWD) {
 #pragma unroll
-            for (int g4 = 0; g4 < G4; ++g4) b4[g4] = __ldg((const float4*)(st.bias + c + 4 * g4));
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int a = 0; a < 4; ++a) gax[h][a] = quad_sum(gax[h][a]);
+          // normal = normalize(g . J^-1) (multiply.py:661), normalised again with eps 1e-6 (:606)
+          const float gx0 = gax[h][0], gx1 = d > 1 ? gax[h][1] : 0.f, gx2 = d > 2 ? gax[h][2] : 0.f;
+          if (q == 0 && io.grad_out && valid[h]) {
+            io.grad_out[3 * (size_t)pt[h]] = gx0;
+            io.grad_out[3 * (size_t)pt[h] + 1] = gx1;
+            io.grad_out[3 * (size_t)pt[h] + 2] = gx2;
           }
-          tmem_wait<CW>(v);
-          if constexpr (KIND == K_SP_PLAIN || KIND == K_SP_SAVE || KIND == K_SP_SEED) {
+          float n0 = 0.f, n1 = 0.f, n2 = 0.f;
+          if (io.jinv && valid[h]) {
+            const float4* J4 = (const float4*)(io.jinv + 12 * (size_t)pt[h]);
+            const float4 ja = __ldg(J4), jb = __ldg(J4 + 1), jc = __ldg(J4 + 2);
+            float v0 = gx0 * ja.x + gx1 * ja.w + gx2 * jb.z;
+            float v1 = gx0 * ja.y + gx1 * jb.x + gx2 * jb.w;
+            float v2 = gx0 * ja.z + gx1 * jb.y + gx2 * jc.x;
+            float nr = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);     // multiply.py:661
+            const float inr = 1.f / nr;
+            v0 *= inr; v1 *= inr; v2 *= inr;
+            float n2r = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-6f);     // multiply.py:606
+            const float in2 = 1.f / n2r;
+            n0 = v0 * in2; n1 = v1 * in2; n2 = v2 * in2;
+            if (q == 0 && io.nrm_out) {
+              io.nrm_out[3 * (size_t)slot[h]] = n0;
+              io.nrm_out[3 * (size_t)slot[h] + 1] = n1;
+              io.nrm_out[3 * (size_t)slot[h] + 2] = n2;
+            }
+          }
+          nrm[h][0] = n0;
+          nrm[h][1] = n1;
+          nrm[h][2] = n2;
+        }
+        // the MMAs of the reverse sweep are done with A: the features return as the colour net's input
+        if (s + 1 < P.nsteps) reload_features();
+        continue;
+      }
+
+      auto run_epi = [&](auto ktag) {
+        constexpr int KIND = decltype(ktag)::value;
+        float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};     // sdf / rgb partial dots of the two rows
+#pragma unroll
+        for (int jp = 0; jp < 16; ++jp) {
+          float* v = acc + 8 * jp;
+          float yv[8];                       // K_SP_SEED: h7 (the stashed features); A receives the seed
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int j = 2 * jp + jj;
+            const int c = 8 * j + 2 * q;     // columns c, c + 1 of u[0], u[1] (row 0) and u[2], u[3] (row 1)
+            float* u = v + 4 * jj;
+            float b[2] = {0.f, 0.f};
+            if constexpr (KIND != K_BWD) {
+              const float2 b2 = __ldg((const float2*)(st.bias + c));
+              b[0] = b2.x;
+              b[1] = b2.y;
+            }
             if constexpr (KIND == K_SP_SEED) {
               // last SDF layer of the fused chain: sigma'_7 is consumed right here -- the reverse sweep starts from
               // A = W8[0,:] * sigma'_7 (d sdf / d z7), h7 only feeds the sdf dot and the feature stash
-              float seed[CW];
+              const float2 w2 = __ldg((const float2*)(P.w8row + c));
+              const float w[2] = {w2.x, w2.y};
 #pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                float4 w4 = __ldg((const float4*)(P.w8row + c + 4 * g4));
+              for (int e = 0; e < 4; ++e) {
+                float y, dd;
+                softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), y, dd);
+                dot[e >> 1][0] = fmaf(y, w[e & 1], dot[e >> 1][0]);
+                yv[4 * jj + e] = y;
+                u[e] = dd * w[e & 1];
+              }
+            } else if constexpr (KIND == K_SP_SAVE || KIND == K_SP_PLAIN) {
+              if constexpr (KIND == K_SP_SAVE) {
                 float dd[4];
-                softplus_fast_grad(fmaf(v[4 * g4 + 0], isc, b4[g4].x), v[4 * g4 + 0], dd[0]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 1], isc, b4[g4].y), v[4 * g4 + 1], dd[1]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 2], isc, b4[g4].z), v[4 * g4 + 2], dd[2]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 3], isc, b4[g4].w), v[4 * g4 + 3], dd[3]);
-                seed[4 * g4 + 0] = dd[0] * w4.x;
-                seed[4 * g4 + 1] = dd[1] * w4.y;
-                seed[4 * g4 + 2] = dd[2] * w4.z;
-                seed[4 * g4 + 3] = dd[3] * w4.w;
-                dot0 = fmaf(v[4 * g4 + 0], w4.x, dot0);
-                dot0 = fmaf(v[4 * g4 + 1], w4.y, dot0);
-                dot0 = fmaf(v[4 * g4 + 2], w4.z, dot0);
-                dot0 = fmaf(v[4 * g4 + 3], w4.w, dot0);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), u[e], dd[e]);
+                st_stream(&sig[(((size_t)st.sig * kConsumers + g) * 32 + j) * 128 + t], make_float4(dd[0], dd[1], dd[2], dd[3]));
+              } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) u[e] = softplus_fast(fmaf(u[e], isc, b[e & 1]));
               }
-              uint4 fh[CW / 8], fl[CW / 8];
+              if ((st.flags & F_INJECT_EMB) && c + 1 >= P.inj_col) {
 #pragma unroll
-              for (int j = 0; j < CW; j += 8) split8(v + j, fh[j >> 3], fl[j >> 3]);
-              issue_next(ci);
+                for (int e = 0; e < 4; ++e)
+                  if (c + (e & 1) >= P.inj_col) u[e] = emb[(size_t)(c + (e & 1) - P.inj_col) * 128 + rowt[e >> 1]];
+              }
+              if (st.flags & F_SDF_DOT) {
+                const float2 w2 = __ldg((const float2*)(P.w8row + c));
+                dot[0][0] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][0]));
+                dot[1][0] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][0]));
+              }
+            } else if constexpr (KIND == K_FEAT) {
 #pragma unroll
-              for (int j = 0; j < CW; j += 8) {
-                if (st.flags & F_STASH_FEAT) {
-                  int chunk = (c + j) >> 3;
-                  st_stream(&fsc[(size_t)chunk * 128 + row], fh[j >> 3]);
-                  st_stream(&fsc[(size_t)(32 + chunk) * 128 + row], fl[j >> 3]);
+              for (int e = 0; e < 4; ++e) u[e] = fmaf(u[e], isc, b[e & 1]);
+              if ((st.flags & F_FEAT_OUT) && io.feat_out) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                  if (valid[h]) *(float2*)(io.feat_out + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
+              }
+            } else if constexpr (KIND == K_BWD) {
+              float4 s4 = make_float4(1.f, 1.f, 1.f, 1.f);
+              const float4* sp = &sig[(((size_t)(st.sig < 0 ? 0 : st.sig) * kConsumers + g) * 32 + j) * 128 + t];
+              if (st.sig >= 0) s4 = ld_stream(sp);
+              const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
+              if ((st.flags & F_SKIP_GRAD) && c + 1 >= P.inj_col) {
+                // columns >= inj_col are d/d embed through the skip connection: park them, zero them in A
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float gval = u[e] * isc;
+                  const int col = c + (e & 1);
+                  if (col >= P.inj_col) {
+                    ge[(size_t)(col - P.inj_col) * 128 + rowt[e >> 1]] = gval;
+                    u[e] = 0.f;
+                  } else {
+                    u[e] = gval * sv[e];
+                  }
                 }
-                store_a8(A32, row, c + j, seed + j);
+              } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) u[e] *= isc * sv[e];
               }
-              return;
-            }
-            if constexpr (KIND == K_SP_SAVE) {
+              // this group's sigma' line is dead: drop it from L2
+              if (st.sig >= 0 && (lane & 7) == 0 && !keep_lines) discard_line(sp, s4.x);
+            } else {   // K_RELU
 #pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                float dd[4];
-                softplus_fast_grad(fmaf(v[4 * g4 + 0], isc, b4[g4].x), v[4 * g4 + 0], dd[0]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 1], isc, b4[g4].y), v[4 * g4 + 1], dd[1]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 2], isc, b4[g4].z), v[4 * g4 + 2], dd[2]);
-                softplus_fast_grad(fmaf(v[4 * g4 + 3], isc, b4[g4].w), v[4 * g4 + 3], dd[3]);
-                st_stream(&sig[((size_t)st.sig * 64 + ((c >> 2) + g4)) * 128 + row], make_float4(dd[0], dd[1], dd[2], dd[3]));
-              }
-            } else {
+              for (int e = 0; e < 4; ++e) u[e] = fmaxf(fmaf(u[e], isc, b[e & 1]), 0.f);
+              if (st.flags & F_RGB_OUT) {
 #pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                v[4 * g4 + 0] = softplus_fast(fmaf(v[4 * g4 + 0], isc, b4[g4].x));
-                v[4 * g4 + 1] = softplus_fast(fmaf(v[4 * g4 + 1], isc, b4[g4].y));
-                v[4 * g4 + 2] = softplus_fast(fmaf(v[4 * g4 + 2], isc, b4[g4].z));
-                v[4 * g4 + 3] = softplus_fast(fmaf(v[4 * g4 + 3], isc, b4[g4].w));
-              }
-            }
-            if ((st.flags & F_INJECT_EMB) && c + CW > P.inj_col) {
-#pragma unroll
-              for (int j = 0; j < CW; ++j)
-                if (c + j >= P.inj_col) v[j] = emb[(size_t)(c + j - P.inj_col) * 128 + row];
-            }
-            if (st.flags & F_SDF_DOT) {
-#pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                float4 w4 = __ldg((const float4*)(P.w8row + c + 4 * g4));
-                dot0 = fmaf(v[4 * g4 + 0], w4.x, dot0);
-                dot0 = fmaf(v[4 * g4 + 1], w4.y, dot0);
-                dot0 = fmaf(v[4 * g4 + 2], w4.z, dot0);
-                dot0 = fmaf(v[4 * g4 + 3], w4.w, dot0);
-              }
-            }
-          } else if constexpr (KIND == K_FEAT) {
-#pragma unroll
-            for (int g4 = 0; g4 < G4; ++g4) {
-              const float4 b = b4[g4];
-              v[4 * g4 + 0] = fmaf(v[4 * g4 + 0], isc, b.x);
-              v[4 * g4 + 1] = fmaf(v[4 * g4 + 1], isc, b.y);
-              v[4 * g4 + 2] = fmaf(v[4 * g4 + 2], isc, b.z);
-              v[4 * g4 + 3] = fmaf(v[4 * g4 + 3], isc, b.w);
-            }
-            if ((st.flags & F_FEAT_OUT) && io.feat_out && valid) {
-#pragma unroll
-              for (int j = 0; j < CW; j += 4)
-                *(float4*)(io.feat_out + (size_t)pt * 256 + c + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            }
-          } else if constexpr (KIND == K_BWD) {
-            if ((st.flags & F_SKIP_GRAD) && c + CW > P.inj_col) {
-              // columns >= inj_col are d/d embed through the skip connection: park them, zero them in A
-              const float* s4f = reinterpret_cast<const float*>(s4);
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                float gval = v[j] * isc;
-                if (c + j >= P.inj_col) {
-                  ge[(size_t)(c + j - P.inj_col) * 128 + row] = gval;
-                  v[j] = 0.f;
-                } else {
-                  v[j] = gval * s4f[j];
+                for (int k = 0; k < 3; ++k) {
+                  const float2 w2 = __ldg((const float2*)(P.Wrgb + 256 * k + c));
+                  dot[0][k] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][k]));
+                  dot[1][k] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][k]));
                 }
-              }
-            } else {
-#pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                v[4 * g4 + 0] *= isc * s4[g4].x;
-                v[4 * g4 + 1] *= isc * s4[g4].y;
-                v[4 * g4 + 2] *= isc * s4[g4].z;
-                v[4 * g4 + 3] *= isc * s4[g4].w;
-              }
-            }
-            if (need_sig && (lane & 7) == 0 && !(io.knobs & 4)) {   // this chunk's sigma' lines are dead: drop them from L2
-#pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4)
-                discard_line(&sig[((size_t)st.sig * 64 + ((c >> 2) + g4)) * 128 + row], v[4 * g4]);
-            }
-            if (need_sig && ci + 1 < NCH) {   // next chunk's sigma' streams in behind the stores below
-#pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4)
-                s4[g4] = ld_stream(&sig[((size_t)st.sig * 64 + ((col_of(ci + 1) >> 2) + g4)) * 128 + row]);
-            }
-          } else {   // EPI_RELU
-#pragma unroll
-            for (int g4 = 0; g4 < G4; ++g4) {
-              const float4 b = b4[g4];
-              v[4 * g4 + 0] = fmaf(v[4 * g4 + 0], isc, b.x);
-              v[4 * g4 + 1] = fmaf(v[4 * g4 + 1], isc, b.y);
-              v[4 * g4 + 2] = fmaf(v[4 * g4 + 2], isc, b.z);
-              v[4 * g4 + 3] = fmaf(v[4 * g4 + 3], isc, b.w);
-            }
-#pragma unroll
-            for (int j = 0; j < CW; ++j) v[j] = fmaxf(v[j], 0.f);
-            if (st.flags & F_RGB_OUT) {
-#pragma unroll
-              for (int g4 = 0; g4 < G4; ++g4) {
-                float4 w0 = __ldg((const float4*)(P.Wrgb + c + 4 * g4));
-                float4 w1 = __ldg((const float4*)(P.Wrgb + 256 + c + 4 * g4));
-                float4 w2 = __ldg((const float4*)(P.Wrgb + 512 + c + 4 * g4));
-                dot0 = fmaf(v[4 * g4 + 0], w0.x, fmaf(v[4 * g4 + 1], w0.y, fmaf(v[4 * g4 + 2], w0.z, fmaf(v[4 * g4 + 3], w0.w, dot0))));
-                dot1 = fmaf(v[4 * g4 + 0], w1.x, fmaf(v[4 * g4 + 1], w1.y, fmaf(v[4 * g4 + 2], w1.z, fmaf(v[4 * g4 + 3], w1.w, dot1))));
-                dot2 = fmaf(v[4 * g4 + 0], w2.x, fmaf(v[4 * g4 + 1], w2.y, fmaf(v[4 * g4 + 2], w2.z, fmaf(v[4 * g4 + 3], w2.w, dot2))));
               }
             }
           }
-          // activations of this chunk -> A (fp16 hi/lo, swizzled) unless this is the last layer
-          // (F_FINAL_GRAD steps never get here; F_RGB_OUT exists only on ReLU steps; F_STASH_FEAT only on the seed step,
-          // which returned above -- testing them here cost seven predicated-off instructions per chunk)
+          if constexpr (KIND == K_SP_SEED) {
+            if (st.flags & F_STASH_FEAT) {
+              uint4 fh, fl;
+              split8(yv, fh, fl);
+              st_stream(&fsc[(size_t)jp * 128 + t], fh);
+              st_stream(&fsc[(size_t)(16 + jp) * 128 + t], fl);
+            }
+          }
+          // activations of these 16 columns -> A (fp16 hi/lo, swizzled) unless this is the last layer
           bool to_a = true;
           if constexpr (KIND == K_RELU) to_a = !(st.flags & F_RGB_OUT);
-          if (to_a) {
-            uint4 hi[CW / 8], lo[CW / 8];
+          if (to_a) store_acc16(lane_base, lane_x, jp, v);
+        }
+        // ---- step-specific tails: per-row dots reduced over the quad ----
+        if (st.flags & F_SDF_DOT) {
 #pragma unroll
-            for (int j = 0; j < CW; j += 8) split8(v + j, hi[j >> 3], lo[j >> 3]);
-            issue_next(ci);
-#pragma unroll
-            for (int j = 0; j < CW; j += 8) {
-#if MP_AOFF
-              // (PIPE) chunk ci is K-block ci; the 16-byte slot inside the row depends only on the column part
-              const uint32_t o = (uint32_t)ci * 16384u + (j ? aoff1 : aoff0);
-#else
-              const uint32_t o = a_off(row, (c + j) >> 6, ((c + j) >> 3) & 7);
-#endif
-              sts128(A32, o, hi[j >> 3]);
-              sts128(A32, 65536 + o, lo[j >> 3]);
-            }
-          } else {
-            issue_next(ci);
+          for (int h = 0; h < 2; ++h) {
+            const float sdot = quad_sum(dot[h][0]);
+            if (q == 0 && valid[h] && io.sdf_out) io.sdf_out[slot[h]] = __ldg(P.b8) + sdot;
           }
-        };
-        if (st.flags & F_FINAL_GRAD) {
-          // ---- last step of the reverse sweep: its own straight-line code (everything it needs lives only here, so the
-          // hot chunk loops of the other steps do not carry its registers) ----
-          // B0's output columns are permuted at pack time BY AXIS: column part a (a < d_in) holds, in its 16 columns of
-          // K-block 0, every embedding index that depends on x_a -- [x_a, sin(2^0 x_a), cos(2^0 x_a), sin(2^1 x_a), ...]
-          // (embedders.py:8-34) -- so the chain rule
-          //   d sdf / d x_a = sum_k (g_k + skip_k) * d embed_k / d x_a
-          // of one axis runs inside one thread's registers.  The skip gradient (parked at the F_SKIP_GRAD step) and the
-          // partner sin / cos of each index (parked by the tile prologue) come from scratch: independent loads issued
-          // together under the TMEM load.
-          float gax = 0.f;                                 // d sdf / d x_part (column parts 0..d-1)
-          if (part < d) {
-            tmem_issue<CW>(t_row + (uint32_t)col_of(0), va);
-            float pg[14], pe[14];
+        }
+        if constexpr (KIND == K_RELU) {
+          if (st.flags & F_RGB_OUT) {
 #pragma unroll
-            for (int j = 0; j < 14; ++j) {
-              // j = 0: x_a itself; j = 1 + 2 f: sin(2^f x_a); j = 2 + 2 f: cos(2^f x_a)
-              const int fq = (j - 1) >> 1;
-              const int k = (j == 0) ? part : d + 2 * fq * d + ((j - 1) & 1) * d + part;
-              const bool ok = j < 1 + 2 * P.multires;
-              pg[j] = ok ? ge[(size_t)k * 128 + row] : 0.f;
-              // partner: cos for a sin entry (+d), sin for a cos entry (-d)
-              pe[j] = (ok && j > 0) ? emb[(size_t)(((j - 1) & 1) ? k - d : k + d) * 128 + row] : 0.f;
-            }
-            tmem_wait<CW>(va);
+            for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int j = 0; j < 14; ++j) {
-              const float tot = fmaf(va[j], isc, pg[j]);           // through layer 0 + through the skip connection
-              const int fq = (j - 1) >> 1;
-              // d x / d x = 1 ; d sin(2^f x) = 2^f cos(2^f x) ; d cos(2^f x) = -2^f sin(2^f x)
-              const float w = (j == 0) ? 1.f : (float)(1 << fq) * (((j - 1) & 1) ? -pe[j] : pe[j]);
-              gax = fmaf(w, tot, gax);
-            }
-          }
-          tc_fence_before();
-          if (tr) g_trace[513] = clock64();
-          // axes 1..d-1 travel to column part 0 through shared memory (one float per row); it derives
-          // normal = normalize(g . J^-1) (multiply.py:661), normalised again with eps 1e-6 (:606), writes the outputs and
-          // is the part that stages the colour net's extra inputs [x_c, n].  Parts 1.. go on without waiting.
-          // (Round 1 exchanged every term through global scratch behind two 512-thread barriers: 30 k cycles per tile.)
-          float n0 = 0.f, n1 = 0.f, n2 = 0.f;
-          if (part != 0) {
-            if (part < d) {
-              xs[(part - 1) * 128 + row] = gax;
-              asm volatile("bar.arrive 4, %0;" ::"r"(128 * d) : "memory");
-            }
-          } else {
-            // the inverse Jacobian of this row's point (cold: written by the deformer kernel) travels under the barrier
-            float4 ja = make_float4(0.f, 0.f, 0.f, 0.f), jb = ja, jc = ja;
-            if (io.jinv && valid) {
-              const float4* J4 = (const float4*)(io.jinv + 12 * (size_t)pt);
-              ja = __ldg(J4);      // J[0..3]
-              jb = __ldg(J4 + 1);  // J[4..7]
-              jc = __ldg(J4 + 2);  // J[8..11]
-            }
-            asm volatile("bar.sync 4, %0;" ::"r"(128 * d) : "memory");
-            const float gx0 = gax, gx1 = d > 1 ? xs[row] : 0.f, gx2 = d > 2 ? xs[128 + row] : 0.f;
-            if (io.grad_out && valid) {
-              io.grad_out[3 * (size_t)pt] = gx0;
-              io.grad_out[3 * (size_t)pt + 1] = gx1;
-              io.grad_out[3 * (size_t)pt + 2] = gx2;
-            }
-            if (io.jinv && valid) {
-              float v0 = gx0 * ja.x + gx1 * ja.w + gx2 * jb.z;
-              float v1 = gx0 * ja.y + gx1 * jb.x + gx2 * jb.w;
-              float v2 = gx0 * ja.z + gx1 * jb.y + gx2 * jc.x;
-              float nr = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);     // multiply.py:661
-              const float inr = 1.f / nr;
-              v0 *= inr; v1 *= inr; v2 *= inr;
-              float n2r = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-6f);     // multiply.py:606
-              const float in2 = 1.f / n2r;
-              n0 = v0 * in2; n1 = v1 * in2; n2 = v2 * in2;
-              if (io.nrm_out) {
-                io.nrm_out[3 * (size_t)slot] = n0;
-                io.nrm_out[3 * (size_t)slot + 1] = n1;
-                io.nrm_out[3 * (size_t)slot + 2] = n2;
+              for (int k = 0; k < 3; ++k) {
+                const float z = __ldg(P.brgb + k) + quad_sum(dot[h][k]);
+                if (q == 0 && valid[h] && io.rgb_out) io.rgb_out[3 * (size_t)slot[h] + k] = 1.f / (1.f + __expf(-z));
               }
             }
           }
-          nrm[0] = n0;
-          nrm[1] = n1;
-          nrm[2] = n2;
-          if (tr) g_trace[517] = clock64();
-          // hand-over: the features already went back into A (reload_features above); nothing else to arrive on
-          if (tr) trp[6] = clock64();
-          continue;
         }
-        // (a second register buffer for the TMEM reads was measured slower: +20 % kernel time from spills / code size)
-        auto run_chunks = [&](auto ktag) {
-          tmem_issue<CW>(t_row + (uint32_t)col_of(0), va);
-#pragma unroll 1
-          for (int ci = 0; ci < NCH; ++ci) {
-            process_chunk(ktag, va, ci);
-            if (tr) trp[2 + ci] = clock64();
-            if (chunk_handover) {
-              // K-block ci of the next layer's operand is complete in this thread
-              fence_async_smem();
-              tc_fence_before();
-              mbar_arrive(&a_ready[ci]);
-            }
-          }
-        };
-        if (st.epi == EPI_SOFTPLUS) {
-          if ((st.flags & (F_SAVE_SIG | F_SEED_BWD)) == (F_SAVE_SIG | F_SEED_BWD))
-            run_chunks(KTag<K_SP_SEED>{});
-          else if (st.flags & F_SAVE_SIG)
-            run_chunks(KTag<K_SP_SAVE>{});
-          else
-            run_chunks(KTag<K_SP_PLAIN>{});
-        } else if (st.epi == EPI_FEAT) {
-          run_chunks(KTag<K_FEAT>{});
-        } else if (st.epi == EPI_BWD) {
-          run_chunks(KTag<K_BWD>{});
-        } else {
-          run_chunks(KTag<K_RELU>{});
-        }
-        tc_fence_before();
-        // ---- step-specific tails ----
-        if (st.flags & F_SDF_DOT) {
-          misc[row * 32 + part] = dot0;
-          __threadfence_block();
-          ep_bar<NEPI>();
-          if (part == 0 && valid && io.sdf_out) {
-            float sacc = __ldg(P.b8);
-#pragma unroll
-            for (int pp = 0; pp < NPART; ++pp) sacc += misc[row * 32 + pp];
-            io.sdf_out[slot] = sacc;
-          }
-          // (no second barrier: these scratch slots are next written a whole tile -- many barriers -- later)
-        }
-        if (st.flags & F_SKIP_GRAD) __threadfence_block();
-        if (st.flags & F_RGB_OUT) {
-          // last step of the tile: the MMAs are done with A, its K-block 3 serves as the exchange buffer for the
-          // partial dots (the next write there is a whole layer step -- and several barriers -- away)
-          float* xch = reinterpret_cast<float*>(A + 3 * 16384);
-          xch[(part * 3 + 0) * 128 + row] = dot0;
-          xch[(part * 3 + 1) * 128 + row] = dot1;
-          xch[(part * 3 + 2) * 128 + row] = dot2;
-          ep_bar<NEPI>();
-          if (part == 0 && valid && io.rgb_out) {
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-              float z = __ldg(P.brgb + k);
-#pragma unroll
-              for (int pp = 0; pp < NPART; ++pp) z += xch[(pp * 3 + k) * 128 + row];
-              io.rgb_out[3 * (size_t)slot + k] = 1.f / (1.f + __expf(-z));
-            }
-          }
-        }
-        // hand A (and the drained accumulator) to the MMA warp for the next step of this tile;
-        // the last step's hand-over is the next tile's prologue arrival
-        if (s + 1 < P.nsteps && !chunk_handover) {
-          if (!(st.flags & F_FINAL_GRAD))
-            arrive_all();
-          else if (!PIPE)
-            reload_features();     // single accumulator: only after this step has drained it
-        }
-        if (tr) trp[6] = clock64();
+      };
+      if (st.epi == EPI_SOFTPLUS) {
+        if ((st.flags & (F_SAVE_SIG | F_SEED_BWD)) == (F_SAVE_SIG | F_SEED_BWD))
+          run_epi(KTag<K_SP_SEED>{});
+        else if (st.flags & F_SAVE_SIG)
+          run_epi(KTag<K_SP_SAVE>{});
+        else
+          run_epi(KTag<K_SP_PLAIN>{});
+      } else if (st.epi == EPI_FEAT) {
+        run_epi(KTag<K_FEAT>{});
+      } else if (st.epi == EPI_BWD) {
+        run_epi(KTag<K_BWD>{});
+      } else {
+        run_epi(KTag<K_RELU>{});
       }
+      // the skip gradient parked in `ge` is read by other lanes of the quad at the final-gradient step
+      if (st.flags & F_SKIP_GRAD) __threadfence_block();
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem0), "n"(TCOLS) : "memory");
   }
 }
 
@@ -1370,7 +1134,7 @@ int tc_trace_read(unsigned long long* out, int n) {
 
 size_t tc_workspace_bytes(int N) { return (size_t)sm_count() * kScratchPerCta + 4096; }
 
-// optional per-launch timing of the tcgen05 kernel (bench.py roofline): CUDA events on the
+// optional per-launch timing of the tensor-core kernel (bench.py roofline): CUDA events on the
 // launching stream + an async copy of the device-side point count into pinned memory
 struct ProfEntry {
   cudaEvent_t e0, e1;
@@ -1424,7 +1188,7 @@ int prof_read(double* ms, long long* launches, double* points, int reset) {
   return 0;
 }
 
-// Precision mode of the tcgen05 engine (mp_set_precision): which of the three split-precision product terms each layer
+// Precision mode of the tensor-core engine (mp_set_precision): which of the three split-precision product terms each layer
 // step issues.  The weight blob always holds the hi and lo slots; a single-term step just skips the lo slots.
 //   0  parity (default): every step A_hi.W_hi + A_lo.W_hi + A_hi.W_lo  -- RGB / SDF within 1e-4 of the fp32 reference
 //   1  colour layers single-term (A_hi.W_hi): SDF / normals unchanged, RGB error ~2e-5 (still inside the gate)
@@ -1433,22 +1197,15 @@ int prof_read(double* ms, long long* launches, double* points, int reset) {
 std::atomic<int> g_precision{0};
 
 // The tensor core adds each MMA's products into the fp32 accumulator with round-toward-zero: every one of the
-// n = 4 nk terms accumulations of a layer step (K = 16 per tcgen05.mma) drops on average half an ulp of the running sum,
+// n = 4 nk terms accumulations of a layer step (K = 16 per wgmma) drops on average half an ulp of the running sum,
 // always toward zero.  Unlike round-to-nearest noise this loss is coherent -- every pre-activation shrinks by the same
-// relative amount, layer after layer -- and it is what kept the engine's SDF at 4e-6 and its gradients at 6e-6 from
-// the fp64 value of the same weights while the fp32 SIMT engine sits at 3e-7.  First-order model: a running sum that
-// grows linearly to its final value z loses  sum_i ulp(z i/n)/2 ~= (n/2) * E[ulp(z)/|z|]/2 * |z|, with
-// E[ulp/|z|] = 2^-23 / (2 ln 2) for a log-uniform mantissa: 2.15e-8 |z| per accumulation, 1.03e-6 |z| for the 48
-// accumulations of a 256-wide three-term layer.  The epilogue multiplies the accumulator by (1 + n * kRzPerMma), which
-// is free (it is folded into the 2^-s rescale).  The constant is the model's 2.15e-8 calibrated by one factor measured on
-// the device (scripts/gpu_normal_diag.py, 4096 points around the surface and 4096 near the canonical origin, against
-// the fp64 evaluation of the same weights; MP_TC_RZ_SCALE sweeps it):
-//   factor   SDF L-inf   d sdf/dx L-inf (mean)    rendered normals, 48-ray sample of the benchmark batch
-//   0        3.7e-6      6.0e-6 (4.0e-6)          4.8e-4   (one sample at |grad| ~ 1e-4 off by 0.07)
-//   0.8      5.8e-7      1.3e-6 (4.3e-7)          3.0e-6   <- kRzPerMma
-//   1.0      1.2e-6      2.1e-6 (1.1e-6)          3.7e-6
-//   1.2      1.6e-6      2.8e-6 (1.7e-6)          6.9e-6
-// (fp32 SIMT engine: 3.1e-7 / 7.1e-7 (1.9e-7) / 2.9e-6.)
+// relative amount, layer after layer -- and uncompensated it dominates the error of the rendered normals where
+// |grad sdf| is small.  First-order model: a running sum that grows linearly to its final value z loses
+// sum_i ulp(z i/n)/2 ~= (n/2) * E[ulp(z)/|z|]/2 * |z|, with E[ulp/|z|] = 2^-23 / (2 ln 2) for a log-uniform mantissa:
+// 2.15e-8 |z| per accumulation, 1.03e-6 |z| for the 48 accumulations of a 256-wide three-term layer.  The epilogue
+// multiplies the accumulator by (1 + n * kRzPerMma), which is free (it is folded into the 2^-s rescale).  The constant
+// is 0.8 times the model's 2.15e-8; MP_TC_RZ_SCALE multiplies it (0 switches it off) and scripts/gpu_normal_diag.py
+// measures the per-sample SDF / gradient / normal error against the fp64 evaluation of the same weights.
 constexpr float kRzPerMma = 1.72e-8f;
 
 static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cudaStream_t st, int kind) {
@@ -1470,7 +1227,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
   int maxtiles = (io.cap + 127) / 128;
   if (grid > maxtiles) grid = maxtiles;
   if (grid < 1) return 0;
-  MP_REQUIRE(ws && ws_bytes >= (size_t)grid * kScratchPerCta, "tcgen05 engine: workspace too small (%zu < %zu)",
+  MP_REQUIRE(ws && ws_bytes >= (size_t)grid * kScratchPerCta, "tensor-core engine: workspace too small (%zu < %zu)",
              ws_bytes, (size_t)grid * kScratchPerCta);
   io.scratch = (char*)ws;
   io.scratch_per_cta = kScratchPerCta;
@@ -1494,7 +1251,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     MP_CHECK_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> g(attr_mu);
     if (dev < 0 || dev >= 64 || !((attr_done >> dev) & 1ull)) {
-      MP_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+      MP_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
       if (dev >= 0 && dev < 64) attr_done |= 1ull << dev;
     }
   }
@@ -1514,7 +1271,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     }
     MP_CHECK_CUDA(cudaEventRecord(pe.e0, st));
   }
-  tc_chain_kernel<16, true><<<grid, 64 + 32 * 16, kSmemBytes, st>>>(P, io);
+  tc_chain_kernel<<<grid, kThreads, kSmemBytes, st>>>(P, io);
   MP_LAUNCH_CHECK();
   if (prof) {
     MP_CHECK_CUDA(cudaEventRecord(pe.e1, st));
@@ -1525,7 +1282,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
 
 int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
                 float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  MP_REQUIRE(f.tc, "tcgen05 engine: field not packed");
+  MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
   TcBlob* tb = (TcBlob*)f.tc;
   TcIO io;
   memset(&io, 0, sizeof(io));
@@ -1540,7 +1297,7 @@ int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, cons
 int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
                   const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
                   float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  MP_REQUIRE(f.tc, "tcgen05 engine: field not packed");
+  MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
   TcBlob* tb = (TcBlob*)f.tc;
   TcIO io;
   memset(&io, 0, sizeof(io));
@@ -1555,15 +1312,15 @@ int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, co
   io.grad_out = grad_out;
   io.feat_out = feat_out;
   if (!Jinv_list && !grad_out) return tc_launch(tb->fwd_prog, io, ws, ws_bytes, st, 1);
-  MP_REQUIRE(tb->has_full, "tcgen05 engine: this field has no fused shading program");
+  MP_REQUIRE(tb->has_full, "tensor-core engine: this field has no fused shading program");
   return tc_launch(tb->full_prog, io, ws, ws_bytes, st, 2);
 }
 
 int tc_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
           size_t ws_bytes, cudaStream_t st) {
-  MP_REQUIRE(f.tc, "tcgen05 engine: field not packed");
+  MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
   TcBlob* tb = (TcBlob*)f.tc;
-  MP_REQUIRE(tb->has_full && f.ren_mode == 1, "tcgen05 engine: not a background field");
+  MP_REQUIRE(tb->has_full && f.ren_mode == 1, "tensor-core engine: not a background field");
   TcIO io;
   memset(&io, 0, sizeof(io));
   io.x = pts;

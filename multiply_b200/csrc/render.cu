@@ -220,7 +220,7 @@ static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
 extern "C" {
 
 int mp_set_engine(int engine) {
-  MP_REQUIRE(engine == 0 || engine == 1, "mp_set_engine: engine must be 0 (simt fp32) or 1 (tcgen05)");
+  MP_REQUIRE(engine == 0 || engine == 1, "mp_set_engine: engine must be 0 (simt fp32) or 1 (tensor cores)");
   mp::g_engine = engine;
   return 0;
 }
@@ -273,7 +273,7 @@ int mp_render_forward(mp_net_t* f, const float* points, const float* normals, co
                       void* workspace, size_t workspace_bytes, void* stream) {
   MP_REQUIRE(f && points && normals && feat && rgb, "mp_render_forward: null argument");
   if (N <= 0) return 0;
-  // the standalone colour operator always runs on the fp32 SIMT kernels (the fused tcgen05 chain
+  // the standalone colour operator always runs on the fp32 SIMT kernels (the fused tensor-core chain
   // consumes features straight from shared memory and has no (points, normals, feat) entry)
   return mp::simt_render(f->f, points, normals, feat, N, rgb, workspace, workspace_bytes, (cudaStream_t)stream);
 }

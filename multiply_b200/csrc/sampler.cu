@@ -4,7 +4,7 @@
 //     ErrorBoundSampler.get_z_vals       :66-220
 //     ErrorBoundSampler.get_error_bound  :222-230
 //
-// B200 design: one warp per ray, the ray's sorted sample list (<= max_total_iters * E values)
+// Design: one warp per ray, the ray's sorted sample list (<= max_total_iters * E values)
 // staged in shared memory; prefix sums are warp scans over per-lane contiguous chunks; the
 // resampled points are merged (stable two-way merge by rank) instead of re-sorted.  The
 // batch-global convergence test `beta.max() > beta0` (:137) is an atomicOr into a per-trip

@@ -15,12 +15,12 @@ def _dev(t, device):
 
 
 def set_engine(name):
-    """'tc' = tcgen05 split-fp16 tensor-core engine (default), 'simt' = fp32 validation engine."""
+    """'tc' = wgmma split-fp16 tensor-core engine (default), 'simt' = fp32 validation engine."""
     L.check(L.lib().mp_set_engine({"simt": 0, "tc": 1}[name]), "mp_set_engine")
 
 
 def set_precision(mode):
-    """tcgen05 engine precision: 'parity' (default, three split terms), 'colour1' (single-term colour layers),
+    """Tensor-core engine precision: 'parity' (default, three split terms), 'colour1' (single-term colour layers),
     'throughput' (single fp16 term everywhere; outside the 1e-4 gate)."""
     L.check(L.lib().mp_set_precision({"parity": 0, "colour1": 1, "throughput": 2}[mode]), "mp_set_precision")
 

@@ -6,7 +6,7 @@ exact (fp64 matmul of the rounded operands), result rounded to fp32.  Compares S
 normal and RGB of one foreground field against (a) the fp64 evaluation of the same network ("truth")
 and (b) the fp32 torch evaluation (what the reference / oracle computes).
 
-    python scripts/numerics_study.py            # prints a table, writes profiles/r2_numerics.json
+    python scripts/numerics_study.py            # prints a table, writes profiles/numerics.json
 """
 import json
 import os
@@ -148,7 +148,7 @@ def main():
         report("bf16 " + mode, chain(person, cfg, x, mode, dt=torch.bfloat16))
     os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
     json.dump(dict(points=4096, truth="fp64 evaluation of the same weights", rows=rows),
-              open(os.path.join(ROOT, "profiles", "r2_numerics.json"), "w"), indent=1)
+              open(os.path.join(ROOT, "profiles", "numerics.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -17,7 +17,7 @@ def _g(golden_dir, name):
 
 ENGINES = ["simt", "tc"]
 # Network-level tolerance (absolute, outputs are O(1)): the fp32 SIMT engine agrees with the CPU
-# reference to rounding; the tcgen05 engine (fp16 hi/lo operands, fp32 accumulation inside the tensor
+# reference to rounding; the tensor-core engine (fp16 hi/lo operands, fp32 accumulation inside the tensor
 # core, whose round-toward-zero is compensated in the epilogue, mlp_tc.cu:kRzPerMma) to ~2e-6 — both far
 # inside the 1e-4 gate of north_star.
 TOL_NET = {"simt": 1e-5, "tc": 2e-5}

@@ -1,7 +1,7 @@
 """Person-sharded rendering (multiply_b200/parallel.py: PersonShardedRenderer) against the fused single-GPU forward.
 In one process (world 1) the per-person pass, mp_composite, mp_background and mp_final_compose are driven separately
 through the C ABI; the frame must equal mp_render_rays bit for bit.  The 2-rank exchange is covered on CPU
-(tests/test_parallel_gloo.py) and on two GPUs by scripts/gpu_person_shard.sh."""
+(tests/test_parallel_gloo.py) and on two GPUs by scripts/person_shard_check.py."""
 import pytest
 import torch
 
