@@ -307,6 +307,45 @@ int mp_background(mp_net_t* bg_field, const float* ray_dirs, const float* cam_lo
                   float* bg_rgb /*[R,3]*/, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * canonical mesh: kaolin.metrics.trianglemesh.point_to_mesh_distance and kaolin.ops.mesh.check_sign as used by
+ * Multiply.check_off_in_surface_points_cano_mesh (multiply.py:153-167) and MultiplyModel.get_interpenetration_loss
+ * (multiply_model.py:532).  A uniform grid of face references over the mesh's bounds; one handle per mesh, built
+ * once (model build, multiply.py:118-121, and each mesh swap, multiply_model.py:504-506).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct mp_mesh mp_mesh_t;
+#define MP_MESH_PLAN_SCRATCH_BYTES 1024
+typedef struct {
+  int V, F;
+  double lo[3];            /* grid origin (mesh bounds minus the margin) */
+  double h;                /* cubic cell size */
+  int dim[3];              /* cells per axis */
+  long long n_refs;        /* (cell, face) references */
+  size_t storage_bytes;    /* device storage mp_mesh_create needs */
+} mp_mesh_plan_t;
+/* verts [V,3] fp32, faces [F,3] int64 (device).  Sizes the grid over the bounds padded by `margin` and counts the
+ * references each face's bounding box makes; scratch: MP_MESH_PLAN_SCRATCH_BYTES of device memory.  Synchronises
+ * `stream` once (to read the sizes back). */
+int mp_mesh_plan(const float* verts, int V, const int64_t* faces, int F, float margin, void* scratch,
+                 mp_mesh_plan_t* plan_host, void* stream);
+/* Builds the grid (count, scan, fill on the device) into caller storage of plan->storage_bytes; verts / faces must be
+ * the arrays given to mp_mesh_plan.  They are copied: the caller may release them once the stream has passed. */
+int mp_mesh_create(const mp_mesh_plan_t* plan_host, const float* verts, const int64_t* faces, void* storage,
+                   size_t storage_bytes, mp_mesh_t** out, void* stream);
+void mp_mesh_free(mp_mesh_t* mesh);
+/* kaolin point_to_mesh_distance (multiply.py:155): pts [N,3] -> dist2 [N] squared distance to the nearest face,
+ * face_idx [N] its index (lowest on ties), dist_type [N] where on it: 0 interior, 1/2/3 vertex 0/1/2, 4/5/6 edge
+ * 01/12/20.  face_idx / dist_type may be NULL. */
+int mp_mesh_distance(const mp_mesh_t* mesh, const float* pts, int N, float* dist2, int64_t* face_idx, int* dist_type,
+                     void* stream);
+/* kaolin check_sign (multiply.py:158, multiply_model.py:532): inside [N] = 1 iff the ray p + t (0,0,1), t > 0, crosses
+ * the mesh an odd number of times (fp64 watertight crossing test).  Meaningful for watertight meshes only. */
+int mp_mesh_check_sign(const mp_mesh_t* mesh, const float* pts, int N, uint8_t* inside, void* stream);
+/* check_off_in_surface_points_cano_mesh (multiply.py:153-167): x_c [rows*N_samples,3] (row-major by ray) -> off [rows]
+ * = min over the row's samples of the signed distance > thr, in [rows] = that minimum <= 0 (uint8). */
+int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int N_samples, float thr, uint8_t* off,
+                          uint8_t* in, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * the fused entry used by Multiply.forward (multiply.py:174-598, eval branch)
  * ---------------------------------------------------------------------------------------- */
 /* Training-mode forward VALUES (multiply.py:174-598 with self.training, shipped loss weights, current_epoch >= 250):
@@ -317,6 +356,14 @@ typedef struct {
   const mp_sampler_rng_t* rng[MP_MAX_PERSONS]; /* host structs of device pointers, one per person */
   float* z_eik[MP_MAX_PERSONS];                /* [R_p] z_samples_eik out, or NULL */
   const float* t_rand_bg;                      /* [R,32] torch.rand of the background's UniformSampler, or NULL */
+  /* current_epoch < 250 (multiply.py:313-316, :549-560): when cano_mesh[k] is set, the canonical points of rendered
+   * person k's main pass go through mp_mesh_surface_flags' kernel, and the per-person flags are merged into
+   * index_off_surface [R] (AND over persons; rays a person does not hit count as off) and index_in_surface [R] (OR).
+   * All NULL: no flags (epoch >= 250). */
+  const mp_mesh_t* cano_mesh[MP_MAX_PERSONS];
+  float surface_threshold;                     /* 0.05 (multiply.py:88) */
+  uint8_t* index_off_surface;                  /* [R] out, required when a mesh is set */
+  uint8_t* index_in_surface;                   /* [R] out, required when a mesh is set */
 } mp_train_t;
 
 typedef struct {

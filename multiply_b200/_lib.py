@@ -58,7 +58,17 @@ class PersonSamples(C.Structure):
 
 class Train(C.Structure):
     _fields_ = [("rng", C.POINTER(SamplerRng) * MP_MAX_PERSONS), ("z_eik", C.c_void_p * MP_MAX_PERSONS),
-                ("t_rand_bg", C.c_void_p)]
+                ("t_rand_bg", C.c_void_p),
+                ("cano_mesh", C.c_void_p * MP_MAX_PERSONS), ("surface_threshold", C.c_float),
+                ("index_off_surface", C.c_void_p), ("index_in_surface", C.c_void_p)]
+
+
+MP_MESH_PLAN_SCRATCH_BYTES = 1024
+
+
+class MeshPlan(C.Structure):
+    _fields_ = [("V", C.c_int), ("F", C.c_int), ("lo", C.c_double * 3), ("h", C.c_double), ("dim", C.c_int * 3),
+                ("n_refs", C.c_longlong), ("storage_bytes", C.c_size_t)]
 
 
 class Scene(C.Structure):
@@ -133,6 +143,12 @@ SIGNATURES = {
     "mp_final_compose": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP]),
     "mp_background_workspace_bytes": (_SZ, [_I]),
     "mp_background": (_I, [_VP, _VP, _VP, _I, _F, _VP, _VP, _SZ, _VP]),
+    "mp_mesh_plan": (_I, [_VP, _I, _VP, _I, _F, _VP, C.POINTER(MeshPlan), _VP]),
+    "mp_mesh_create": (_I, [C.POINTER(MeshPlan), _VP, _VP, _VP, _SZ, C.POINTER(_VP), _VP]),
+    "mp_mesh_free": (None, [_VP]),
+    "mp_mesh_distance": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP]),
+    "mp_mesh_check_sign": (_I, [_VP, _VP, _I, _VP, _VP]),
+    "mp_mesh_surface_flags": (_I, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP]),
     "mp_render_workspace_bytes": (_SZ, [C.POINTER(Scene), _I]),
     "mp_render_rays": (_I, [C.POINTER(Scene), _VP, _VP, _VP, _I, C.POINTER(RenderOut), _VP, _SZ, _VP]),
 }

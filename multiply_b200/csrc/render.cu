@@ -45,6 +45,13 @@ int launch_final_compose(const float* fg, const float* bgT, const float* bg, int
 int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
                       void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand = nullptr);
 size_t bg_ws_bytes(int R);
+// mesh.cu
+struct Mesh;
+const Mesh& mesh_of(const mp_mesh_t* h);
+int launch_surface_flags(const Mesh& m, const float* xc, const int* slot, const int* count_dev, int cap, int n,
+                         float thr, uint8_t* off, uint8_t* in, cudaStream_t st);
+int launch_merge_flags(const int64_t* idx, int rows, const int* rows_dev, const uint8_t* off_p, const uint8_t* in_p,
+                       uint8_t* off, uint8_t* in, cudaStream_t st);
 
 static size_t engine_ws_bytes(int N) {
   size_t a = simt_workspace_bytes(N), b = tc_workspace_bytes(N);
@@ -170,6 +177,7 @@ struct PersonBufs {
   float *dirs, *cam, *z, *sdf, *rgb, *nrm, *xc_list, *jinv;
   int *slot_list, *count, *row_of_ray;
   uint8_t* outl;
+  uint8_t *off, *in;     // per-row surface flags (training with a canonical mesh only)
 };
 
 struct RenderWs {
@@ -207,6 +215,9 @@ static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
     b.count = a.take<int>(1);
     b.row_of_ray = a.take<int>(R);
     b.outl = a.take<uint8_t>((size_t)Rp * n);
+    const bool flags = sc.train && sc.train->cano_mesh[p];
+    b.off = flags ? a.take<uint8_t>(Rp) : nullptr;
+    b.in = flags ? a.take<uint8_t>(Rp) : nullptr;
     sub = max(sub, sampler_ws_bytes(c, Rp));
     sub = max(sub, engine_ws_bytes(Rp * n));
   }
@@ -378,6 +389,12 @@ static int render_person(const mp_scene_t* scene, int p, int R, const RenderWs& 
   if (pre_shade) MP_CHECK_CUDA(cudaEventRecord(pre_shade, st));
   MP_TRY(field_shade_list(field, b.xc_list, b.slot_list, b.count, Rp * n, b.jinv, b.sdf, b.rgb, b.nrm, nullptr,
                           nullptr, w.sub[p], w.sub_bytes, st));
+  if (tr && tr->cano_mesh[p]) {     // check_off_in_surface_points_cano_mesh on the main pass's points (:313-316)
+    MP_CHECK_CUDA(cudaMemsetAsync(b.off, 1, Rp, st));
+    MP_CHECK_CUDA(cudaMemsetAsync(b.in, 0, Rp, st));
+    MP_TRY(launch_surface_flags(mesh_of(tr->cano_mesh[p]), b.xc_list, b.slot_list, b.count, Rp * n, n,
+                                tr->surface_threshold, b.off, b.in, st));
+  }
   if (!prune && !tr) {     // (multiply.py:142-143 is eval-only)
     force_outlier_sdf_kernel<<<div_up(Rp * n, 256), 256, 0, st>>>(b.outl, Rp * n, b.sdf);
     MP_LAUNCH_CHECK();
@@ -409,6 +426,13 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
   MP_REQUIRE(scene->P >= 1 && scene->P <= MP_MAX_PERSONS, "mp_render_rays: P out of range");
   MP_REQUIRE(R > 0, "mp_render_rays: R must be positive");
   MP_REQUIRE(out->rgb_values, "mp_render_rays: rgb_values output is required");
+  const mp_train_t* tr = scene->train;
+  int n_mesh = 0;
+  for (int p = 0; tr && p < scene->P; ++p) n_mesh += tr->cano_mesh[p] ? 1 : 0;
+  MP_REQUIRE(n_mesh == 0 || n_mesh == scene->P, "mp_render_rays: canonical meshes are set for %d of %d persons", n_mesh,
+             scene->P);
+  MP_REQUIRE(n_mesh == 0 || (tr->index_off_surface && tr->index_in_surface),
+             "mp_render_rays: surface flags need index_off_surface and index_in_surface outputs");
   const cudaStream_t caller = (cudaStream_t)stream;
   const mp_sampler_cfg_t& c = scene->sampler;
   const int n = c.N_samples + c.N_samples_extra + 1;     // multiply.py:290-292
@@ -502,6 +526,13 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
   float* bgT = out->bg_T ? out->bg_T : w.bgT;
   MP_TRY(launch_composite(cp, R, n, beta, w.fg, normal, acc, accp, bgT, caller));     // multiply.py:427-480
   MP_TRY(launch_final_compose(w.fg, bgT, bg, R, out->rgb_values, out->fg_rgb_values, caller));   // :544-545, :590
+  if (n_mesh) {     // multiply.py:549-560
+    MP_CHECK_CUDA(cudaMemsetAsync(tr->index_off_surface, 1, R, caller));
+    MP_CHECK_CUDA(cudaMemsetAsync(tr->index_in_surface, 0, R, caller));
+    for (int p = 0; p < scene->P; ++p)
+      MP_TRY(launch_merge_flags(scene->hit_index[p], scene->hit_count[p], scene->hit_count_dev[p], w.pb[p].off,
+                                w.pb[p].in, tr->index_off_surface, tr->index_in_surface, caller));
+  }
   return 0;
 }
 }

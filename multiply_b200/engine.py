@@ -216,6 +216,80 @@ class Body:
             pass
 
 
+class CanonicalMesh:
+    """A triangle mesh on the device with its grid of face references (mp_mesh_plan / mp_mesh_create): the canonical
+    mesh of one person (multiply.py:118-121, replaced by multiply_model.py:504-506), queried by kaolin's
+    point_to_mesh_distance / check_sign (multiply.py:155,158) and the per-ray surface flags (:153-167).  Building it
+    reads the grid size back once (one synchronisation); the queries do not synchronise."""
+
+    def __init__(self, verts, faces, margin=0.01, device="cuda"):
+        lib = L.lib()
+        self.device = torch.device(device)
+        with torch.cuda.device(self.device):
+            v = _dev(verts.reshape(-1, 3), self.device)
+            f = torch.as_tensor(faces).detach().to(device=self.device, dtype=torch.int64).reshape(-1, 3).contiguous()
+            self.V, self.F = v.shape[0], f.shape[0]
+            scratch = torch.empty(L.MP_MESH_PLAN_SCRATCH_BYTES, dtype=torch.uint8, device=self.device)
+            plan = L.MeshPlan()
+            L.check(lib.mp_mesh_plan(v.data_ptr(), self.V, f.data_ptr(), self.F, float(margin), scratch.data_ptr(),
+                                     C.byref(plan), L.stream_ptr()), "mp_mesh_plan")
+            self.plan = plan
+            self.storage = torch.empty(plan.storage_bytes, dtype=torch.uint8, device=self.device)
+            h = C.c_void_p()
+            L.check(lib.mp_mesh_create(C.byref(plan), v.data_ptr(), f.data_ptr(), self.storage.data_ptr(),
+                                       plan.storage_bytes, C.byref(h), L.stream_ptr()), "mp_mesh_create")
+            self._src = (v, f)        # read by the build kernels enqueued above
+            self.handle = h
+
+    @property
+    def grid_dims(self):
+        return tuple(self.plan.dim)
+
+    def distance(self, pts):
+        """pts [N,3] -> (dist2 [N] fp32 squared distance, face_idx [N] int64, dist_type [N] int32), kaolin's
+        convention: 0 face interior, 1/2/3 vertex 0/1/2, 4/5/6 edge 01/12/20; ties go to the lowest face index."""
+        with torch.cuda.device(self.device):
+            p = _dev(pts.reshape(-1, 3), self.device)
+            N = p.shape[0]
+            d2 = torch.empty(N, device=self.device)
+            fi = torch.empty(N, dtype=torch.int64, device=self.device)
+            dt = torch.empty(N, dtype=torch.int32, device=self.device)
+            L.check(L.lib().mp_mesh_distance(self.handle, p.data_ptr(), N, d2.data_ptr(), fi.data_ptr(), dt.data_ptr(),
+                                             L.stream_ptr()), "mp_mesh_distance")
+            return d2, fi, dt
+
+    def check_sign(self, pts):
+        """pts [N,3] -> inside [N] bool: odd number of crossings of the ray p + t (0,0,1), t > 0."""
+        with torch.cuda.device(self.device):
+            p = _dev(pts.reshape(-1, 3), self.device)
+            N = p.shape[0]
+            ins = torch.empty(N, dtype=torch.uint8, device=self.device)
+            L.check(L.lib().mp_mesh_check_sign(self.handle, p.data_ptr(), N, ins.data_ptr(), L.stream_ptr()),
+                    "mp_mesh_check_sign")
+            return ins.bool()
+
+    def surface_flags(self, x_c, N_samples, threshold=0.05):
+        """check_off_in_surface_points_cano_mesh (multiply.py:153-167): x_c [rows*N_samples,3] ->
+        (index_off_surface [rows], index_in_surface [rows]) bool."""
+        with torch.cuda.device(self.device):
+            x = _dev(x_c.reshape(-1, 3), self.device)
+            rows = x.shape[0] // int(N_samples)
+            assert rows * int(N_samples) == x.shape[0], "x_c must hold rows * N_samples points"
+            off = torch.empty(rows, dtype=torch.uint8, device=self.device)
+            ins = torch.empty(rows, dtype=torch.uint8, device=self.device)
+            L.check(L.lib().mp_mesh_surface_flags(self.handle, x.data_ptr(), rows, int(N_samples), float(threshold),
+                                                  off.data_ptr(), ins.data_ptr(), L.stream_ptr()),
+                    "mp_mesh_surface_flags")
+            return off.bool(), ins.bool()
+
+    def __del__(self):
+        try:
+            if getattr(self, "handle", None):
+                L.lib().mp_mesh_free(self.handle)
+        except Exception:
+            pass
+
+
 def sampler_cfg(cfg, beta_param, beta_min=1e-4):
     c = L.SamplerCfg()
     c.scene_bounding_sphere = cfg["scene_bounding_sphere"]
@@ -290,7 +364,9 @@ class Renderer:
         out: optional dict of preallocated contiguous output tensors (e.g. ``parallel.PixelBuffer.views``);
         train: training-mode VALUES (mp_train_t): dict(rng=[per rendered person the tabled draws of
         ``ErrorBoundSampler.draw_training_rng``], t_rand_bg=[R,32] or None) — stochastic sampling, no outlier clamp,
-        jittered background depths; adds ``z_eik_{k}`` [R_k] per person.  No gradients.
+        jittered background depths; adds ``z_eik_{k}`` [R_k] per person.  With ``meshes=[CanonicalMesh per rendered
+        person]`` (current_epoch < 250, multiply.py:313-316) and ``threshold`` (default 0.05) it also returns
+        ``index_off_surface`` / ``index_in_surface`` [R] bool, merged over persons as multiply.py:549-560.  No gradients.
         Returns the eval output dict of Multiply.forward (multiply.py:589-598)."""
         with torch.cuda.device(self.device):
             return self._render(inputs, hit_lists, debug, persons, check, out, train)
@@ -329,6 +405,7 @@ class Renderer:
         sc.bg_field = self.bg.handle if self.bg is not None else None
         keep_train = []
         z_eik = {}
+        flags = {}
         if train is not None:
             assert not dev_counts, "training mode needs host-side hit counts"
             tr = L.Train()
@@ -343,6 +420,17 @@ class Renderer:
                 tb = _dev(tb, dev)
                 keep_train.append(tb)
                 tr.t_rand_bg = tb.data_ptr()
+            meshes = train.get("meshes")
+            if meshes is not None:
+                assert len(meshes) == Pn and all(m is not None for m in meshes), "one canonical mesh per rendered person"
+                for k, m in enumerate(meshes):
+                    tr.cano_mesh[k] = m.handle
+                keep_train.append(list(meshes))
+                tr.surface_threshold = float(train.get("threshold", 0.05))
+                flags = {"index_off_surface": torch.empty(R, dtype=torch.uint8, device=dev),
+                         "index_in_surface": torch.empty(R, dtype=torch.uint8, device=dev)}
+                tr.index_off_surface = flags["index_off_surface"].data_ptr()
+                tr.index_in_surface = flags["index_in_surface"].data_ptr()
             keep_train.append(tr)
             sc.train = C.pointer(tr)
         need = lib.mp_render_workspace_bytes(C.byref(sc), R)
@@ -386,6 +474,8 @@ class Renderer:
         self._keep = (uv, pose, K, hits, keep_train)
         for k, v in z_eik.items():
             dbg[f"z_eik_{k}"] = v
+        for k, v in flags.items():
+            res[k] = v.bool()
         if check:
             self.check_status()
         res.update(dbg)

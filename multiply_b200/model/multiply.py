@@ -45,6 +45,17 @@ class Multiply(nn.Module):
         self.deformer_list = [SMPLDeformer(smpl_verts=s.verts_c, smpl_weights=s.weights, scale=getattr(s, "scale", 1.0))
                               for s in self.smpl_server_list]
         self.sdf_bounding_sphere = 3.0                                   # multiply.py:85
+        self.threshold = 0.05                                            # multiply.py:88
+        # canonical meshes (multiply.py:118-121): the server's triangles over its canonical vertices (mesh_verts_c when
+        # the server keeps the mesh's vertices apart from verts_c, as scene.SyntheticSMPLServer does); None = no mesh
+        self.mesh_v_cano_list, self.mesh_f_cano_list = [], []
+        for srv in self.smpl_server_list:
+            f = getattr(srv, "faces", None)
+            v = getattr(srv, "mesh_verts_c", None)
+            v = srv.verts_c if v is None else v
+            self.mesh_v_cano_list.append(v.reshape(-1, 3) if f is not None else None)
+            self.mesh_f_cano_list.append(torch.as_tensor(f).to(torch.int64) if f is not None else None)
+        self._cano_meshes = {}
         d = _get(opt, "density")
         self.density = LaplaceDensity(**(dict(d) if not isinstance(d, dict) else d))
         self.bg_density = AbsDensity()
@@ -99,6 +110,31 @@ class Multiply(nn.Module):
         if self._renderer is not None:
             for b in self._renderer.bodies:
                 b.set_root_finder(*self._root_finder)
+
+    def set_canonical_mesh(self, person_id, verts, faces):
+        """Replaces person ``person_id``'s canonical mesh (verts [V,3], faces [F,3]), as multiply_model.py:504-506 does
+        with the marching-cubes mesh every 20 epochs.  Its grid is rebuilt on the next use."""
+        self.mesh_v_cano_list[person_id] = verts.detach().reshape(-1, 3)
+        self.mesh_f_cano_list[person_id] = torch.as_tensor(faces).detach().to(torch.int64).reshape(-1, 3)
+        self._cano_meshes.pop(person_id, None)
+
+    def _canonical_mesh(self, person_id, device):
+        if self.mesh_f_cano_list[person_id] is None:
+            raise ValueError("person %d has no canonical mesh: the SMPL server provides no faces; call "
+                             "Multiply.set_canonical_mesh(person_id, verts, faces) before training at current_epoch < 250"
+                             % person_id)
+        m = self._cano_meshes.get(person_id)
+        if m is None or m.device != torch.device(device):
+            m = engine.CanonicalMesh(self.mesh_v_cano_list[person_id], self.mesh_f_cano_list[person_id], device=device)
+            self._cano_meshes[person_id] = m
+        return m
+
+    def check_off_in_surface_points_cano_mesh(self, x_cano, N_samples, person_id, threshold=0.05):
+        """multiply.py:153-167: canonical points x_cano [rows*N_samples,3] against person ``person_id``'s canonical
+        mesh -> (index_off_surface [rows], index_in_surface [rows]) bool: the row's minimum signed distance (negative
+        inside, kaolin's check_sign) > threshold, resp. <= 0."""
+        dev = x_cano.device if x_cano.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        return self._canonical_mesh(person_id, dev).surface_flags(x_cano, N_samples, threshold)
 
     def _person_dict(self, p, smpl_out, cond=None):
         srv = self.smpl_server_list[p]
@@ -264,17 +300,15 @@ class Multiply(nn.Module):
     # ---- Multiply.forward, training branch: VALUES only ------------------------------------------
     def _forward_train_values(self, input, id=-1, cond_zero_shit=False):
         """The values of the training branch of Multiply.forward (multiply.py:174-598 with self.training) for the shipped
-        loss weights (smpl_surface_weight = zero_pose_weight = 0, confs/model/*.yaml:77-88) at current_epoch >= 250 (the
-        earlier epochs need kaolin's point-to-mesh test, :152-166, absent offline): stochastic sampling with the
+        loss weights (smpl_surface_weight = zero_pose_weight = 0, confs/model/*.yaml:77-88): stochastic sampling with the
         reference's own random stream (the same torch.manual_seed gives the same sample depths), no outlier clamp (:142 is
         eval-only), eikonal samples and their SDF gradients (:320-331), temporal loss (:242-243), jittered background
         depths (:482).  NO autograd graph is built: the tensors are detached values — the backward pass is the open half of
         SURVEY.md 8f-1 (DESIGN.md 7).  One scalar read per person keeps the random stream in step with the reference's
-        (its trip count decides how much randperm consumes)."""
+        (its trip count decides how much randperm consumes).  At current_epoch < 250 the canonical points of the main
+        pass are also tested against each person's canonical mesh (:313-316, check_off_in_surface_points_cano_mesh) and
+        index_off_surface / index_in_surface [R] bool are the merged flags of :549-560; at >= 250 they are None."""
         epoch = int(input["current_epoch"])
-        if epoch < 250:
-            raise NotImplementedError("current_epoch < 250 needs kaolin's point-to-mesh test for index_off_surface "
-                                      "(multiply.py:152-166, :313-316), absent offline")
         dev = input["uv"].device
         smpl_params, smpl_pose = input["smpl_params"], input["smpl_pose"]
         scale = smpl_params[:, :, 0]
@@ -295,6 +329,7 @@ class Multiply(nn.Module):
         if first:
             self._ensure_renderer(dev, [self._person_dict(i, outs[i], smpl_pose[:, i, 3:] / np.pi) for i in range(P)])
         r = self._ensure_renderer(dev)
+        meshes = [self._canonical_mesh(i, dev) for i in person_list] if epoch < 250 else None
         for k, i in enumerate(person_list):
             cond = smpl_pose[:, i, 3:] * 0. if zero_cond else smpl_pose[:, i, 3:] / np.pi
             pd = dict(verts_p=outs[i]["smpl_verts"].reshape(-1, 3), tfs=outs[i]["smpl_tfs"].reshape(24, 4, 4), cond=cond)
@@ -332,14 +367,16 @@ class Multiply(nn.Module):
             frame = self.frame_latent_encoder(input["idx"])
         if r.bg is not None:
             r.bg.set_cond(frame.detach())
-        out = r.render(input, hits, persons=person_list, train=dict(rng=rngs, t_rand_bg=t_rand_bg))
+        out = r.render(input, hits, persons=person_list,
+                       train=dict(rng=rngs, t_rand_bg=t_rand_bg, meshes=meshes, threshold=self.threshold))
         temporal = torch.zeros(1, device=dev)
         if epoch > 250:                                                    # multiply.py:242-243
             temporal = torch.mean(torch.square(input["smpl_pose_last"] - input["smpl_pose"])).reshape(1).detach()
         z1 = torch.zeros(1, device=dev)
         res = {"rgb_values": out["rgb_values"], "normal_values": out["normal_values"], "acc_map": out["acc_map"],
                "acc_person_list": out["acc_person_list"], "grad_theta": torch.cat(grad_theta, 0)[None],
-               "index_outside": input.get("index_outside"), "index_off_surface": None, "index_in_surface": None,
+               "index_outside": input.get("index_outside"), "index_off_surface": out.get("index_off_surface"),
+               "index_in_surface": out.get("index_in_surface"),
                "interpenetration_loss": z1, "temporal_loss": temporal, "smpl_surface_loss": z1.clone(),
                "zero_pose_loss": z1.clone(), "epoch": input["current_epoch"], "cam_loc": cam,
                "t_list": [], "fg_rgb_values_each_person_list": [], "hitted_mask_idx": [], "mean_hitted_vertex_list": []}

@@ -45,6 +45,8 @@ class SMPLServer(torch.nn.Module):
         self.tfs_c_inv = ti                          # smpl.py:47
         self.weights = a["lbs_weights"][None]
         self.scale = 1.0
+        # the pkl's triangles over verts_c (multiply.py:118-121), when the model dict carries them (optional `faces`)
+        self.faces = torch.as_tensor(model["faces"]).to(torch.int64) if model.get("faces") is not None else None
 
     def forward(self, scale, transl, thetas, betas, absolute=False):
         """smpl.py:50-95: scale [1], transl [1,3], thetas [1,72], betas [1,10] -> dict."""

@@ -75,14 +75,34 @@ def _rigid_transform(rot, joints):
     return G - corr
 
 
-def make_body(seed, V=6890):
-    """Capsule body: rest verts [V,3], skinning weights [V,24] (row-sum 1)."""
-    rng = np.random.RandomState(seed)
+def _capsules():
+    """The body's capsules in the rest pose: end points a [25,3], b [25,3], radii [25]."""
     # bones: (parent joint -> joint) for j>=1, plus a head blob at joint 15 and a pelvis blob at 0
     seg_a = [_J[PARENTS[j]] for j in range(1, 24)] + [_J[15], _J[0]]
     seg_b = [_J[j] for j in range(1, 24)] + [_J[15] + np.array([0, 0.12, 0.0]), _J[0] + np.array([0, 0.02, 0])]
     seg_r = [_RADIUS[j] for j in range(1, 24)] + [0.10, 0.13]
-    seg_a, seg_b, seg_r = np.array(seg_a), np.array(seg_b), np.array(seg_r)
+    return np.array(seg_a), np.array(seg_b), np.array(seg_r)
+
+
+def _skin_weights(verts):
+    """Normalised Gaussian of the distance to the bone segment of each joint: [N,24]."""
+    W = np.zeros((verts.shape[0], 24))
+    for j in range(24):
+        a = _J[PARENTS[j]] if j > 0 else _J[0]
+        b = _J[j] if j > 0 else _J[0] + np.array([0, 0.05, 0])
+        ab = b - a
+        t = np.clip(((verts - a) @ ab) / (ab @ ab + 1e-12), 0, 1)
+        d = np.linalg.norm(verts - (a + t[:, None] * ab), axis=1)
+        W[:, j] = np.exp(-(d / 0.06) ** 2)
+    W[W < 1e-4 * W.max(1, keepdims=True)] = 0
+    W /= W.sum(1, keepdims=True)
+    return W
+
+
+def make_body(seed, V=6890):
+    """Capsule body: rest verts [V,3], skinning weights [V,24] (row-sum 1)."""
+    rng = np.random.RandomState(seed)
+    seg_a, seg_b, seg_r = _capsules()
     length = np.linalg.norm(seg_b - seg_a, axis=1)
     area = 2 * math.pi * seg_r * (length + 2 * seg_r)
     counts = np.floor(area / area.sum() * V).astype(int)
@@ -102,18 +122,108 @@ def make_body(seed, V=6890):
         p = a[None] + (tc + over)[:, None] * ax[None] + rad[:, None] * dirs
         verts.append(p)
     verts = np.concatenate(verts, 0)[:V]
-    # weights: normalised Gaussian of distance to the bone segment of each joint
-    W = np.zeros((V, 24))
-    for j in range(24):
-        a = _J[PARENTS[j]] if j > 0 else _J[0]
-        b = _J[j] if j > 0 else _J[0] + np.array([0, 0.05, 0])
+    return verts, _skin_weights(verts)
+
+
+def _canonical_A():
+    """Bone transforms of the canonical pose (hips +-pi/6 about z, lib/model/smpl.py:38-39)."""
+    theta_c = np.zeros((24, 3))
+    theta_c[1, 2] = math.pi / 6
+    theta_c[2, 2] = -math.pi / 6
+    return _rigid_transform(_rodrigues(theta_c), _J)
+
+
+# Freudenthal split of a cube (corner bit 1 = +x, 2 = +y, 4 = +z) into 6 tetrahedra around the 0-7 diagonal; the same
+# split in every cube, so the tetrahedra of neighbouring cubes share faces exactly
+_TETS = np.array([[0, 1, 3, 7], [0, 1, 5, 7], [0, 2, 3, 7], [0, 2, 6, 7], [0, 4, 5, 7], [0, 4, 6, 7]])
+
+
+def make_body_mesh(body_seed=100, step=0.033):
+    """Triangle mesh of the capsule union of ``make_body`` in the canonical pose: (verts [V,3] fp32, faces [F,3] int64).
+
+    Marching tetrahedra of the union's signed distance on a lattice of spacing ``step``: one vertex per lattice edge
+    the surface crosses (shared by every tetrahedron around that edge), triangles oriented so that their normal points
+    from the inside corners of their tetrahedron to the outside ones.  The result is watertight (every edge in exactly
+    two faces, in opposite directions), consistently oriented (positive volume) and non-convex.  The canonical capsules
+    are the rest-pose ones with their end points moved by the canonical pose's skinning (the weights of make_body).
+    ``body_seed`` only shifts the lattice by a sub-step offset (no lattice point lies on the surface); the default step
+    gives a face count of the order of SMPL's 13 776, step 0.005 about 3 x 10^5.  Deterministic."""
+    seg_a, seg_b, seg_r = _capsules()
+    A_c = _canonical_A()
+    seg_a = lbs_np(seg_a, _skin_weights(seg_a), A_c)
+    seg_b = lbs_np(seg_b, _skin_weights(seg_b), A_c)
+    off = step * (0.25 + 0.5 * ((body_seed * 0.6180339887498949) % 1.0)) * np.array([1.0, 0.7548776662, 0.5698402910])
+    pad = 3 * step
+    lo = np.minimum(seg_a, seg_b).min(0) - seg_r.max() - pad - off
+    hi = np.maximum(seg_a, seg_b).max(0) + seg_r.max() + pad
+    n = np.ceil((hi - lo) / step).astype(int) + 1
+    axes = [lo[k] + step * np.arange(n[k]) for k in range(3)]
+    sdf = np.full(tuple(n), np.inf)
+    for a, b, r in zip(seg_a, seg_b, seg_r):     # each capsule inside its own box (+ 2 steps): exact near every surface
+        blo = np.maximum(np.floor((np.minimum(a, b) - r - 2 * step - lo) / step).astype(int), 0)
+        bhi = np.minimum(np.ceil((np.maximum(a, b) + r + 2 * step - lo) / step).astype(int) + 1, n)
+        X, Y, Z = np.meshgrid(*[axes[k][blo[k]:bhi[k]] for k in range(3)], indexing="ij")
+        P = np.stack([X, Y, Z], -1)
         ab = b - a
-        t = np.clip(((verts - a) @ ab) / (ab @ ab + 1e-12), 0, 1)
-        d = np.linalg.norm(verts - (a + t[:, None] * ab), axis=1)
-        W[:, j] = np.exp(-(d / 0.06) ** 2)
-    W[W < 1e-4 * W.max(1, keepdims=True)] = 0
-    W /= W.sum(1, keepdims=True)
-    return verts, W
+        t = np.clip(((P - a) @ ab) / (ab @ ab + 1e-12), 0.0, 1.0)
+        d = np.linalg.norm(P - (a + t[..., None] * ab), axis=-1) - r
+        sl = tuple(slice(blo[k], bhi[k]) for k in range(3))
+        sdf[sl] = np.minimum(sdf[sl], d)
+    sdf[sdf == 0.0] = 1e-12
+    # cubes with a sign change
+    inside = sdf < 0
+    corners = [(i & 1, (i >> 1) & 1, (i >> 2) & 1) for i in range(8)]
+    cnt = sum(inside[dx:n[0] - 1 + dx, dy:n[1] - 1 + dy, dz:n[2] - 1 + dz].astype(np.int8) for dx, dy, dz in corners)
+    cx, cy, cz = np.nonzero((cnt > 0) & (cnt < 8))
+    gid = lambda x, y, z: (x * n[1] + y) * n[2] + z
+    cid = np.stack([gid(cx + dx, cy + dy, cz + dz) for dx, dy, dz in corners], 1)      # [C,8]
+    tv = cid[:, _TETS].reshape(-1, 4)                                                  # [T,4] lattice ids
+    flat = sdf.reshape(-1)
+    ts = flat[tv]
+    tin = ts < 0
+    k = tin.sum(1)
+    keep = (k > 0) & (k < 4)
+    tv, ts, tin, k = tv[keep], ts[keep], tin[keep], k[keep]
+    order = np.argsort(~tin, axis=1, kind="stable")               # inside corners first
+    tv = np.take_along_axis(tv, order, 1)
+    tris = []
+    for kk, pairs in ((1, [[(0, 1), (0, 2), (0, 3)]]), (3, [[(0, 3), (1, 3), (2, 3)]]),
+                      (2, [[(0, 2), (0, 3), (1, 3)], [(0, 2), (1, 3), (1, 2)]])):
+        sel = tv[k == kk]
+        for tri in pairs:
+            e = np.stack([np.sort(np.stack([sel[:, i], sel[:, j]], 1), 1) for i, j in tri], 1)     # [n,3,2]
+            tris.append((e, sel, kk))
+    edges = np.concatenate([e.reshape(-1, 2) for e, _, _ in tris], 0)
+    uniq, inv = np.unique(edges, axis=0, return_inverse=True)
+    inv = inv.reshape(-1)
+
+    def pos(ids):
+        x = ids // (n[1] * n[2])
+        y = (ids // n[2]) % n[1]
+        z = ids % n[2]
+        return np.stack([axes[0][x], axes[1][y], axes[2][z]], -1)
+    pa, pb = pos(uniq[:, 0]), pos(uniq[:, 1])
+    sa, sb = flat[uniq[:, 0]], flat[uniq[:, 1]]
+    verts = pa + (sa / (sa - sb))[:, None] * (pb - pa)
+    faces, o = [], 0
+    for e, sel, kk in tris:
+        m = e.shape[0]
+        f = inv[o:o + 3 * m].reshape(m, 3)
+        o += 3 * m
+        # orient: normal from the inside corners of the tetrahedron towards its outside corners
+        pc = pos(sel)
+        din = pc[:, :kk].mean(1)
+        dout = pc[:, kk:].mean(1)
+        v = verts[f]
+        nrm = np.cross(v[:, 1] - v[:, 0], v[:, 2] - v[:, 0])
+        flip = (nrm * (dout - din)).sum(1) < 0
+        f[flip] = f[flip][:, [0, 2, 1]]
+        faces.append(f)
+    faces = np.concatenate(faces, 0)
+    # canonical order: faces sorted by their vertex ids (independent of numpy's traversal)
+    faces = faces[np.lexsort(faces.T[::-1])]
+    return (torch.from_numpy(np.ascontiguousarray(verts.astype(np.float32))),
+            torch.from_numpy(np.ascontiguousarray(faces.astype(np.int64))))
 
 
 def lbs_np(verts, W, A):
@@ -380,6 +490,9 @@ class SyntheticSMPLServer:
         self.verts_c = f32(lbs_np(verts_t, W, self._A_c))[None]
         self.weights = f32(W)[None]
         self.scale = 1.0
+        # canonical triangle mesh of the same capsules (the SMPL pkl's `f` over verts_c in the reference,
+        # multiply.py:118-121); its own vertices, since verts_c here is a point cloud
+        self.mesh_verts_c, self.faces = make_body_mesh(100 + person_index)
 
     def canonical_output(self):
         return self(torch.ones(1), torch.zeros(1, 3), torch.zeros(1, 72), torch.zeros(1, 10))
@@ -454,6 +567,8 @@ def make_smpl_scene(P=2, S=64, seed=42, device="cuda", frame_index=3, pose_std=0
     from .model.smpl import SMPLServer
     from .model.multiply import Multiply
     servers = [SMPLServer(model=make_smpl_model(300 + p, body_seed=100 + p), device=device) for p in range(P)]
+    for p, srv in enumerate(servers):          # canonical mesh of the capsules (SyntheticSMPLServer)
+        srv.mesh_verts_c, srv.faces = make_body_mesh(100 + p)
     smpl_inputs = smpl_scene_inputs(P, frame_index, pose_std, scale)
     smpl_params, smpl_pose, smpl_trans = smpl_inputs["smpl_params"], smpl_inputs["smpl_pose"], smpl_inputs["smpl_trans"]
     nets, rest = smpl_scene_networks(P, S, seed)
