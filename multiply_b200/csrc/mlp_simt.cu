@@ -430,9 +430,11 @@ int simt_bg(const Field& f, const float* pts, const float* dirs, int N, float* s
     MP_REQUIRE(simt_take(a, n, b, false), "simt_bg: workspace too small (%zu needed)", a.off);
     float* h7;
     MP_TRY(simt_trunk(f, pts + 4 * (size_t)s, n, nullptr, b, false, &h7, st));
-    scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nullptr, nullptr,
-                                                            sdf + s);
-    MP_LAUNCH_CHECK();
+    if (sdf) {     // may be NULL (mp_bg_nets_forward)
+      scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nullptr, nullptr,
+                                                              sdf + s);
+      MP_LAUNCH_CHECK();
+    }
     const int X = f.ren_extra, ldc = X + 256;
     view_embed_kernel<<<div_up(n, 128), 128, 0, st>>>(dirs + 3 * (size_t)s, f.multires_view, n, b.cin, ldc);
     MP_LAUNCH_CHECK();

@@ -1313,6 +1313,15 @@ int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, co
   io.feat_out = feat_out;
   if (!Jinv_list && !grad_out) return tc_launch(tb->fwd_prog, io, ws, ws_bytes, st, 1);
   MP_REQUIRE(tb->has_full, "tensor-core engine: this field has no fused shading program");
+  if (feat_out) {
+    // the fused program folds L8's feature rows into the colour layer and never materialises the features: the
+    // forward program writes them (operator API only; the render passes no feature output)
+    TcIO fio = io;
+    fio.jinv = nullptr;
+    fio.sdf_out = fio.rgb_out = fio.nrm_out = fio.grad_out = nullptr;
+    MP_TRY(tc_launch(tb->fwd_prog, fio, ws, ws_bytes, st, 1));
+    io.feat_out = nullptr;
+  }
   return tc_launch(tb->full_prog, io, ws, ws_bytes, st, 2);
 }
 

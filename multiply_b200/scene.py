@@ -347,7 +347,8 @@ def init_render_bg(gen):
     return sd
 
 
-def make_scene(P=2, S=64, seed=42, beta=0.1):
+def make_scene(P=2, S=64, seed=42, beta=0.1, weights="geometric"):
+    """weights: 'geometric' (the networks' initialisation) or 'trained' (perturb_networks(scene, seed) of it)."""
     gen = torch.Generator().manual_seed(seed)
     persons = []
     for p in range(P):
@@ -359,7 +360,154 @@ def make_scene(P=2, S=64, seed=42, beta=0.1):
                  bg_implicit=init_implicit_bg(gen), bg_render=init_render_bg(gen),
                  frame_code=torch.randn(1, 32, generator=torch.Generator().manual_seed(7)),
                  beta_param=beta)
+    if weights == "trained":
+        return perturb_networks(scene, seed)
+    assert weights == "geometric", weights
     return scene
+
+
+# ------------------------------------------------------------------------------------
+# trained-like parameters
+# ------------------------------------------------------------------------------------
+# The geometric init zeroes or trivialises exactly what the MLP kernels treat specially: the Fourier columns of lin0 /
+# lin4 are zero (no sin / cos term reaches the SDF or its gradient), weight_g = ||v||_row (the weight-norm fold is the
+# identity) and the hidden biases are zero.  A trained checkpoint has none of this; perturb_networks makes parameters
+# that look like one while the SDF stays a smooth surface around the body.
+
+FOURIER_AMP = 0.2         # Fourier column noise of lin0 / lin4, relative to the xyz columns' std, times 2^-frequency
+REL_NOISE = 0.1           # weight noise of every other layer, relative to the layer's weight std
+HIDDEN_BIAS_STD = 0.05    # biases of lin0..lin7 (zero in the geometric init)
+
+
+def _embed_freq(k, d=3):
+    """Frequency index f of embedding column k ([x, sin(2^0 x), cos(2^0 x), sin(2^1 x), ...], embedders.py:8-34); -1
+    for x itself."""
+    return -1 if k < d else (k - d) // (2 * d)
+
+
+def _noise(shape, std, gen):
+    return torch.randn(*shape, generator=gen, dtype=torch.float64) * std
+
+
+def _store_weight(sd, name, w, gen):
+    """Effective weight w stored as a weight-norm pair whose g / ||v||_row = u ~ U(0.5, 2): v = w / u, g = ||v|| u."""
+    u = 0.5 + 1.5 * torch.rand(w.shape[0], 1, generator=gen, dtype=torch.float64)
+    v = w / u
+    sd[f"{name}.weight_v"] = v.float()
+    sd[f"{name}.weight_g"] = (v.norm(dim=1, keepdim=True) * u).float()
+
+
+def _effective(sd, name):
+    if f"{name}.weight_v" in sd:
+        v = sd[f"{name}.weight_v"].double()
+        return sd[f"{name}.weight_g"].double() * v / v.norm(dim=1, keepdim=True)
+    return sd[f"{name}.weight"].double()
+
+
+def _sdf64(sd, x, cond, multires=6):
+    """fp64 SDF of a foreground ImplicitNet state dict at x [N,3] (networks.py:126-208); used to keep the surface in
+    place when the parameters are perturbed."""
+    emb = [x] + [f(x * 2.0 ** i) for i in range(multires) for f in (torch.sin, torch.cos)]
+    emb = torch.cat(emb, -1)
+    h = torch.cat([emb, cond.double().expand(x.shape[0], -1)], -1)
+    for l in range(9):
+        if l == 4:
+            h = torch.cat([h, emb], -1) / math.sqrt(2)
+        h = torch.nn.functional.linear(h, _effective(sd, f"lin{l}"), sd[f"lin{l}.bias"].double())
+        if l < 8:
+            h = torch.nn.functional.softplus(h, beta=100)
+    return h[:, 0]
+
+
+def _perturb_implicit_fg(sd, gen, d=3, multires=6, anchor=None):
+    """anchor = (x [N,3], cond): lin8's sdf bias is shifted so that the median SDF at x is the unperturbed one's."""
+    d0 = d * (1 + 2 * multires)
+    out = {}
+    for l in range(9):
+        w = _effective(sd, f"lin{l}")
+        b = sd[f"lin{l}.bias"].double().clone()
+        if l in (0, 4):
+            # columns of the input embedding: in lin0 the first d0, in lin4 (the skip input [h3, embed]) the last d0
+            off = 0 if l == 0 else w.shape[1] - d0
+            s_xyz = float(w[:, off:off + d].std())
+            w[:, off:off + d] += _noise((w.shape[0], d), REL_NOISE * s_xyz, gen)
+            for k in range(d, d0):
+                w[:, off + k] = _noise((w.shape[0],), FOURIER_AMP * s_xyz * 2.0 ** -_embed_freq(k, d), gen)
+            if l == 0:        # the pose-cond columns
+                w[:, d0:] += _noise((w.shape[0], w.shape[1] - d0), REL_NOISE * float(w[:, d0:].std()), gen)
+            else:             # the hidden part of lin4
+                w[:, :off] += _noise((w.shape[0], off), REL_NOISE * float(w[:, :off].std()), gen)
+        elif l == 8:
+            # the geometric init gives every output row the same mean weight: spread the feature rows
+            w[0] += _noise((w.shape[1],), 0.2 * float(w[0].mean()), gen)
+            w[1:] += _noise((w.shape[0] - 1, w.shape[1]), float(w[1:].mean()), gen)
+            b[1:] += _noise((b.shape[0] - 1,), 0.1, gen)
+        else:
+            w += _noise(w.shape, REL_NOISE * float(w.std()), gen)
+        if l < 8:
+            b += _noise(b.shape, HIDDEN_BIAS_STD, gen)
+        _store_weight(out, f"lin{l}", w, gen)
+        out[f"lin{l}.bias"] = b.float()
+    if anchor is not None:
+        # softplus is convex: noise on the pre-activations raises every hidden mean and with it the SDF; then scale the
+        # SDF row so that the median |grad sdf| near the surface is 1, as the eikonal loss of a training run makes it
+        x, cond = anchor
+        shift = (_sdf64(out, x, cond) - _sdf64(sd, x, cond)).median()
+        out["lin8.bias"][0] -= float(shift)
+        x = x.clone().requires_grad_(True)
+        y = _sdf64(out, x, cond)
+        g = torch.autograd.grad(y.sum(), x)[0].norm(dim=1)
+        c = 1.0 / float(g[y.detach().abs() < 0.05].median())
+        out["lin8.weight_g"][0] *= c
+        out["lin8.bias"][0] *= c
+    return out
+
+
+def _perturb_render_fg(sd, gen):
+    out = {}
+    n = len([k for k in sd if k.startswith("lin") and k.endswith(".bias") and "pose" not in k])
+    for l in range(n):
+        w = _effective(sd, f"lin{l}")
+        w += _noise(w.shape, REL_NOISE * float(w.std()), gen)
+        _store_weight(out, f"lin{l}", w, gen)
+        out[f"lin{l}.bias"] = sd[f"lin{l}.bias"].clone()
+    w = sd["lin_pose.weight"].double()
+    out["lin_pose.weight"] = (w + _noise(w.shape, 0.5 * float(w.std()), gen)).float()
+    b = sd["lin_pose.bias"].double()
+    out["lin_pose.bias"] = (b + _noise(b.shape, 0.5 * float(b.std()), gen)).float()
+    return out
+
+
+def _perturb_plain(sd, gen):
+    """Networks without weight norm (background): relative noise on every weight."""
+    out = {}
+    for k, v in sd.items():
+        if k.endswith(".weight"):
+            w = v.double()
+            out[k] = (w + _noise(w.shape, REL_NOISE * float(w.std()), gen)).float()
+        else:
+            out[k] = v.clone()
+    return out
+
+
+def perturb_networks(scene, seed=0):
+    """A copy of ``scene`` whose networks carry trained-like parameters, deterministic in ``seed``:
+      - every weight gets noise, the zero Fourier columns of the foreground lin0 / lin4 included (their noise falls as
+        2^-frequency, so the SDF stays smooth while sin / cos carry a good share of its gradient);
+      - every weight-norm layer stores g = ||v||_row * U(0.5, 2) (the effective weight is the perturbed one);
+      - lin0..lin7 of the foreground ImplicitNet get non-zero biases, the feature part of lin8's bias is perturbed;
+      - the RenderingNet's lin_pose is perturbed as well;
+      - lin8's SDF row is shifted and scaled so that the median SDF at the canonical body vertices is the unperturbed
+        one's and the median |grad sdf| near the surface is 1.
+    Bodies, cameras and the sampler configuration are shared with ``scene``."""
+    gen = torch.Generator().manual_seed(10007 + seed)
+    persons = []
+    for person in scene["persons"]:
+        anchor = (person["verts_c"].double(), person["cond"])
+        persons.append(dict(person, implicit=_perturb_implicit_fg(person["implicit"], gen, anchor=anchor),
+                            render=_perturb_render_fg(person["render"], gen)))
+    return dict(scene, persons=persons, bg_implicit=_perturb_plain(scene["bg_implicit"], gen),
+                bg_render=_perturb_plain(scene["bg_render"], gen))
 
 
 # ------------------------------------------------------------------------------------

@@ -251,6 +251,27 @@ def main():
     grid_case(ref)
     train_sampler_case(ref)
     train_forward_case(ref)
+    trained_case(ref)
+
+
+def trained_case(ref):
+    """ImplicitNet forward (sdf, features), its autograd grad sdf and RenderingNet RGB of the unmodified reference
+    modules at the trained-like parameters of scene.perturb_networks (non-zero Fourier columns, g != ||v||_row, hidden
+    biases), on points over the canonical box and near the body."""
+    sc = S.make_scene(P=2, S=64, seed=42, weights="trained")
+    m = build_ref_model(ref, sc)
+    p0 = sc["persons"][0]
+    g = torch.Generator().manual_seed(11)
+    vc = p0["verts_c"]
+    x = torch.cat([(torch.rand(128, 3, generator=g) - 0.5) * 2.0,
+                   vc[torch.randint(0, vc.shape[0], (128,), generator=g)] + 0.03 * torch.randn(128, 3, generator=g)])
+    xg = x.clone().requires_grad_(True)
+    out = m.foreground_implicit_network_list[0](xg, {"smpl": p0["cond"]}, person_id=0)[0]
+    grad = torch.autograd.grad(out[:, 0].sum(), xg)[0]
+    nrm = torch.nn.functional.normalize(grad, dim=1)
+    with torch.no_grad():
+        rgb = m.foreground_rendering_network_list[0](x, nrm, None, p0["cond"], out[:, 1:].detach(), person_id=0)
+    save("implicit_fg_trained", x=x, out=out, grad=grad, normals=nrm, rgb=rgb)
 
 
 def train_sampler_case(ref):
@@ -476,5 +497,7 @@ if __name__ == "__main__":
             train_sampler_case(_ref)
         if "forward_train" in sys.argv[2:]:
             train_forward_case(_ref)
+        if "implicit_fg_trained" in sys.argv[2:]:
+            trained_case(_ref)
     else:
         main()

@@ -184,3 +184,25 @@ def test_forward_training_mode(golden_dir):
     for k, tol in (("rgb_values", 1e-5), ("acc_map", 1e-5), ("normal_values", 5e-4), ("acc_person_list", 1e-5)):
         d = np.abs(out[k].numpy() - g[k])
         assert np.median(d) < 1e-5 and d.max() < tol, (k, float(d.max()))
+
+
+def test_implicit_fg_trained(golden_dir):
+    """oracle/port.py in float64 against the reference modules at trained-like parameters (scene.perturb_networks):
+    anchors the fp64 oracle of tests/test_gpu_networks.py -- weight-norm semantics (g != ||v||_row), the embedding
+    order for d = 3 (non-zero Fourier columns), the skip layer and the hidden biases -- to the reference."""
+    g = _g(golden_dir, "implicit_fg_trained")
+    p0 = S.make_scene(P=2, S=64, seed=42, weights="trained")["persons"][0]
+    imp = {k: v.double() for k, v in p0["implicit"].items()}
+    ren = {k: v.double() for k, v in p0["render"].items()}
+    cond = p0["cond"].double()
+    x = torch.from_numpy(g["x"]).double().requires_grad_(True)
+    y = port.implicit_forward(imp, x, cond, 6)
+    gr = torch.autograd.grad(y[:, 0].sum(), x)[0]
+    # the fixture is the reference in float32: the bounds are its rounding (measured 2.6e-6 / 1.3e-6 / 9e-8); a port
+    # that ignored weight_g would be off by 3
+    assert np.abs(y.detach().numpy() - g["out"]).max() < 5e-6
+    assert np.abs(gr.numpy() - g["grad"]).max() < 5e-6
+    with torch.no_grad():
+        rgb = port.rendering_forward(ren, "pose_no_view", x.detach(), torch.from_numpy(g["normals"]).double(), None, cond,
+                                     torch.from_numpy(g["out"][:, 1:]).double())
+    assert np.abs(rgb.numpy() - g["rgb"]).max() < 1e-6
