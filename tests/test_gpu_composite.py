@@ -1,0 +1,320 @@
+"""GPU: the multi-person compositor (csrc/composite.cu: mp_composite, mp_final_compose) against a float64 restatement of
+multiply.py:427-480 at person-count, sample-count, block and tie edges.
+
+The kernel merges the P per-person lists of a ray by rank (binary searches: count_le for earlier persons, count_lt for
+later ones, so equal t_end values keep (person, sample) order), scans sigma * delta in chunks per lane and takes bg_T
+from the exclusive prefix of the ray's last merged sample.  Whole renders only ever tie on the shared `far` where
+sigma ~ 0, so the tie order and the prefix there are checked here on synthetic inputs where they matter: identical z
+rows of two persons on one ray, zero-length intervals inside one list, and the shared far with a negative sdf on the
+last sample.  Sizes: P = 1 .. 8 (MP_MAX_PERSONS), n around the warp (1, 31, 32, 33, 193, 385) and the largest n whose
+12 P n bytes of shared memory per warp fit the kernel's 200 KB cap at P = 8; R = 1 and around the rays-per-block edge."""
+import os
+import sys
+
+import numpy as np
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+SENTINEL = -1234.5
+SMEM_CAP = 200 * 1024                   # launch_composite: dynamic shared memory of one block
+N_MAX_P8 = SMEM_CAP // (12 * 8)         # 2133: the largest n with 12 * P * n <= 200 KB at P = 8
+# fp64 comparison gate of every output (fg_rgb, normal, acc, acc_person, bg_T); the measured worst values are quoted in
+# the docstring of test_composite_vs_fp64
+TOL = 1e-5
+MEASURED = {}
+
+
+# ---------------------------------------------------------------------------------------------
+# float64 (or float32) restatement of multiply.py:427-480
+# ---------------------------------------------------------------------------------------------
+
+def composite_ref(persons, R, n, beta, dtype=np.float64, reverse=False):
+    """Flatten every person's samples, sort by (ray, t_end, person, sample) -- (ray, t_end, -person, -sample) with
+    `reverse` --, Laplace sigma (density.py:20-25), exclusive per-ray prefix of sigma * delta, w = T * alpha, and
+    bg_T = T at the start of the ray's last merged sample (1 for rays no person hits).
+    persons: list of dict(idx [R_p] int64, z [R_p, n+1], sdf [R_p, n], rgb / nrm [R_p, n, 3]).
+    Returns fg_rgb [R,3], normal [R,3], acc [R], acc_person [R,P], bg_T [R] in `dtype`."""
+    P = len(persons)
+    cols = {k: [] for k in ("ray", "pid", "smp", "ts", "te", "sdf", "rgb", "nrm")}
+    for p, d in enumerate(persons):
+        Rp = d["idx"].shape[0]
+        cols["ray"].append(np.repeat(np.asarray(d["idx"], np.int64), n))
+        cols["pid"].append(np.full(Rp * n, p))
+        cols["smp"].append(np.tile(np.arange(n), Rp))
+        cols["ts"].append(d["z"][:, :-1].reshape(-1))
+        cols["te"].append(d["z"][:, 1:].reshape(-1))
+        cols["sdf"].append(d["sdf"].reshape(-1))
+        cols["rgb"].append(d["rgb"].reshape(-1, 3))
+        cols["nrm"].append(d["nrm"].reshape(-1, 3))
+    c = {k: np.concatenate(v) for k, v in cols.items()}
+    sg = -1 if reverse else 1
+    o = np.lexsort((sg * c["smp"], sg * c["pid"], c["te"], c["ray"]))
+    c = {k: v[o] for k, v in c.items()}
+    # sigma and the exponentials with torch's operations in the order of oracle/port.py (in float32, 1 - exp and the
+    # 0.5 + 0.5 * expm1 of a positive sdf cancel, so another library's expm1 would move them by an ulp of 0.5 / beta)
+    td = torch.float64 if dtype == np.float64 else torch.float32
+    ts, te, sdf = (torch.from_numpy(c[k].astype(dtype)) for k in ("ts", "te", "sdf"))
+    b = torch.tensor(beta, dtype=td)
+    sigma = (1 / b) * (0.5 + 0.5 * sdf.sign() * torch.expm1(-sdf.abs() / b))
+    sd_t = sigma * (te - ts)
+    sd = sd_t.numpy()
+    ray = c["ray"]
+    starts = np.flatnonzero(np.r_[True, ray[1:] != ray[:-1]]) if ray.size else np.zeros(0, np.int64)
+    ends = np.r_[starts[1:], ray.size]
+    excl = np.zeros_like(sd)
+    for s, e in zip(starts, ends):             # per-ray sequential exclusive scan (nerfacc's definition)
+        excl[s + 1:e] = np.cumsum(sd[s:e - 1], dtype=dtype)
+    T = torch.exp(-torch.from_numpy(excl)).numpy()
+    w = (torch.from_numpy(T) * (1 - torch.exp(-sd_t))).numpy()
+    fg, nrm = np.zeros((R, 3), dtype), np.zeros((R, 3), dtype)
+    acc, accp = np.zeros(R, dtype), np.zeros((R, P), dtype)
+    np.add.at(fg, ray, w[:, None] * c["rgb"].astype(dtype))
+    np.add.at(nrm, ray, w[:, None] * c["nrm"].astype(dtype))
+    np.add.at(acc, ray, w)
+    np.add.at(accp, (ray, c["pid"]), w)
+    bgT = np.ones(R, dtype)
+    if ray.size:
+        bgT[ray[ends - 1]] = T[ends - 1]
+    return fg, nrm, acc, accp, bgT
+
+
+# ---------------------------------------------------------------------------------------------
+# synthetic inputs
+# ---------------------------------------------------------------------------------------------
+
+def make_inputs(seed, P, R, n, substitute=False, ties=True):
+    """Per-person hit lists and sample rows.  Ray 0 is hit by every person, ray 1 by none, ray 2 by person 0 only, the
+    rest by random subsets; with `substitute` the last person's list is the single ray 0 (multiply.py:262-263).  Rows
+    are sorted z with a per-ray `far` shared by all persons as the last column; sdf spreads over [-1, 1] with exact
+    zeros.  With `ties`: persons 0 and 1 share one z row on ray 0 (and on every third ray both hit), some rows carry
+    zero-length intervals, and half of the rays end with a negative sdf on the last sample."""
+    rng = np.random.RandomState(seed)
+    H = rng.random_sample((P, R)) < 0.6
+    H[:, 0] = True
+    if R > 1:
+        H[:, 1] = False
+    if R > 2:
+        H[:, 2] = False
+        H[0, 2] = True
+    if substitute and P > 1:
+        H[P - 1] = False
+        H[P - 1, 0] = True
+    far = rng.uniform(3.0, 4.0, R).astype(np.float32)
+    neg_last = rng.random_sample(R) < 0.5
+    persons = []
+    for p in range(P):
+        idx = np.flatnonzero(H[p]).astype(np.int64)
+        Rp = idx.size
+        near = rng.uniform(0.5, 1.5, Rp)
+        u = np.sort(rng.random_sample((Rp, n - 1)), 1) if n > 1 else np.zeros((Rp, 0))
+        z = np.concatenate([near[:, None], near[:, None] + u * (far[idx] - near)[:, None], far[idx][:, None]], 1)
+        z = z.astype(np.float32)
+        z[:, -1] = far[idx]
+        zm = 0.5 * (z[:, :-1] + z[:, 1:])
+        surf = rng.uniform(0.8, 3.5, (Rp, 1))
+        k = rng.uniform(1.0, 20.0, (Rp, 1))
+        sdf = np.clip((surf - zm) * k + rng.normal(0, 0.05, zm.shape), -1, 1)
+        noisy = rng.random_sample(Rp) < 0.3
+        sdf[noisy] = rng.uniform(-1, 1, (int(noisy.sum()), n))
+        sdf[rng.random_sample(sdf.shape) < 0.05] = 0.0
+        sdf = sdf.astype(np.float32)
+        if ties:
+            if n > 2:        # zero-length intervals: z[i + 1] = z[i] on some rows
+                rows = rng.random_sample(Rp) < 0.3
+                cols = rng.randint(1, n - 1, int(rows.sum()))
+                z[np.flatnonzero(rows), cols + 1] = z[np.flatnonzero(rows), cols]
+            last_neg = neg_last[idx]
+            sdf[last_neg, -1] = -np.abs(sdf[last_neg, -1]) - np.float32(0.25)
+        persons.append(dict(idx=idx, z=np.ascontiguousarray(z), sdf=np.ascontiguousarray(sdf),
+                            rgb=rng.random_sample((Rp, n, 3)).astype(np.float32),
+                            nrm=rng.uniform(-1, 1, (Rp, n, 3)).astype(np.float32)))
+    if ties and P > 1:      # persons 0 and 1: identical z rows (and a negative-sdf stretch) on shared rays
+        a, b = persons[0], persons[1]
+        shared = np.intersect1d(a["idx"], b["idx"])
+        shared = shared[(shared % 3) == 0]
+        ra, rb = np.searchsorted(a["idx"], shared), np.searchsorted(b["idx"], shared)
+        b["z"][rb] = a["z"][ra]
+        b["sdf"][rb, : max(1, n // 2)] = -0.05
+        a["sdf"][ra, : max(1, n // 2)] = -0.02
+    return persons
+
+
+def subset(persons, rays):
+    """The same samples composited for the rays `rays` only (sorted), renumbered 0 .. len(rays) - 1."""
+    out = []
+    for d in persons:
+        keep = np.isin(d["idx"], rays)
+        out.append(dict(idx=np.searchsorted(rays, d["idx"][keep]).astype(np.int64),
+                        **{k: np.ascontiguousarray(d[k][keep]) for k in ("z", "sdf", "rgb", "nrm")}))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------
+# the C ABI with sentinel-padded outputs (as tests/test_gpu_networks.py)
+# ---------------------------------------------------------------------------------------------
+
+def _out(N, width):
+    return torch.full(((N + 128) * width,), SENTINEL, device="cuda")
+
+
+def _take(buf, N, width, what):
+    tail = buf[N * width:]
+    assert bool((tail == SENTINEL).all()), "%s: %d values written past R = %d" % (what, int((tail != SENTINEL).sum()), N)
+    return buf[:N * width].reshape(N, width).cpu().numpy() if width > 1 else buf[:N].cpu().numpy()
+
+
+def wpc_of(P, n):
+    """Rays per block of launch_composite."""
+    return max(1, min(8, SMEM_CAP // (12 * P * n)))
+
+
+def call_composite(persons, R, n, beta, P_arg=None, ws_delta=0):
+    """(status, outputs or the untouched-check of the raw buffers)."""
+    from multiply_b200 import _lib as L
+    lib = L.lib()
+    P = len(persons)
+    arr = (L.PersonSamples * max(P, 1))()
+    keep = []
+    for p, d in enumerate(persons):
+        dev = {k: torch.from_numpy(d[k]).cuda() if d["idx"].size else torch.zeros(1, device="cuda")
+               for k in ("z", "sdf", "rgb", "nrm")}
+        dev["idx"] = torch.from_numpy(d["idx"]).cuda() if d["idx"].size else torch.zeros(1, dtype=torch.int64,
+                                                                                         device="cuda")
+        keep.append(dev)
+        arr[p].n_rows = int(d["idx"].size)
+        arr[p].ray_index = dev["idx"].data_ptr()
+        arr[p].z_vals = dev["z"].data_ptr()
+        arr[p].sdf = dev["sdf"].data_ptr()
+        arr[p].rgb = dev["rgb"].data_ptr()
+        arr[p].normal = dev["nrm"].data_ptr()
+    bufs = dict(fg=_out(R, 3), nrm=_out(R, 3), acc=_out(R, 1), accp=_out(R, P), bgT=_out(R, 1))
+    ws_bytes = lib.mp_composite_workspace_bytes(R, P) + ws_delta
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device="cuda")
+    rc = lib.mp_composite(arr, P if P_arg is None else P_arg, R, n, float(beta), bufs["fg"].data_ptr(),
+                          bufs["nrm"].data_ptr(), bufs["acc"].data_ptr(), bufs["accp"].data_ptr(), bufs["bgT"].data_ptr(),
+                          ws.data_ptr(), ws_bytes, L.stream_ptr())
+    torch.cuda.synchronize()
+    if rc != 0:
+        return rc, bufs
+    return rc, (_take(bufs["fg"], R, 3, "fg_rgb"), _take(bufs["nrm"], R, 3, "normal"), _take(bufs["acc"], R, 1, "acc"),
+                _take(bufs["accp"], R, P, "acc_person").reshape(R, P), _take(bufs["bgT"], R, 1, "bg_T"))
+
+
+NAMES = ("fg_rgb", "normal", "acc", "acc_person", "bg_T")
+
+
+def _errs(got, want):
+    return {k: float(np.abs(np.asarray(g, np.float64) - w).max()) if g.size else 0.0
+            for k, g, w in zip(NAMES, got, want)}
+
+
+# (P, n, beta): every P in 1..8, every n of the docstring, both betas; beta = 1e-4 makes T underflow after one sample
+CASES = [(1, 1, 0.1), (1, 32, 1e-4), (1, 385, 0.1), (2, 31, 0.1), (2, 33, 1e-4), (3, 193, 0.1), (3, 1, 1e-4),
+         (4, 32, 0.1), (4, 385, 1e-4), (5, 33, 0.1), (6, 193, 1e-4), (7, 31, 0.1), (7, 385, 0.1), (8, 1, 0.1),
+         (8, 33, 1e-4), (8, 193, 0.1), (8, N_MAX_P8, 0.1), (8, N_MAX_P8, 1e-4)]
+
+
+@pytest.mark.parametrize("P,n,beta", CASES, ids=["P%d-n%d-b%g" % c for c in CASES])
+def test_composite_vs_fp64(P, n, beta):
+    """Every output against the fp64 restatement, at R = 1 and around the rays-per-block edge; nothing written past R;
+    and a subset of the rays composited alone (hit lists remapped) gives bit-identical results for those rays.
+
+    Measured on one H100 80GB HBM3 at a 400 W power limit: worst error over all cases and outputs 3.1e-6 (P = 7,
+    n = 385, beta = 0.1); the fp32 sigma of a positive sdf (0.5 + 0.5 * expm1 cancels) and the fp32 prefix sums over up
+    to 17 064 samples per ray account for it."""
+    wpc = wpc_of(P, n)
+    Rs = sorted({1, max(1, wpc - 1), wpc, wpc + 1, 2 * wpc + 1, 3 * wpc + 5})
+    for R in Rs:
+        persons = make_inputs(1000 * P + n + R, P, R, n, substitute=(R % 2 == 1))
+        rc, got = call_composite(persons, R, n, beta)
+        assert rc == 0
+        want = composite_ref(persons, R, n, np.float32(beta))
+        e = _errs(got, want)
+        key = (P, n, beta, R)
+        MEASURED[key] = max(e.values())
+        print("COMPOSITE P=%d n=%d beta=%g R=%d wpc=%d errors %s" % (P, n, beta, R, wpc,
+                                                                   " ".join("%s=%.2e" % kv for kv in e.items())))
+        assert max(e.values()) < TOL, e
+        if R >= 3:
+            rays = np.arange(0, R, 2)
+            rc, part = call_composite(subset(persons, rays), rays.size, n, beta)
+            assert rc == 0
+            for k, a, b in zip(NAMES, part, got):
+                assert np.array_equal(a.view(np.uint32), b[rays].view(np.uint32)), k
+
+
+def test_tie_order():
+    """Equal t_end values merge in (person, sample) order.  A case where that order and the reversed one differ by
+    more than 1e-3 in the weights or bg_T: the kernel matches the first and not the second."""
+    P, n, R, beta = 3, 33, wpc_of(3, 33) + 1, 0.1
+    persons = make_inputs(7, P, R, n)
+    for p, d in enumerate(persons):        # ray 0 (every person hits it): nearly empty up to a dense last sample
+        row = int(np.searchsorted(d["idx"], 0))
+        d["sdf"][row] = 1.0
+        d["sdf"][row, -1] = -0.1 - 0.3 * p
+    fwd = composite_ref(persons, R, n, np.float32(beta))
+    rev = composite_ref(persons, R, n, np.float32(beta), reverse=True)
+    gap = max(float(np.abs(a - b).max()) for a, b in zip(fwd, rev))
+    assert gap > 1e-3
+    rc, got = call_composite(persons, R, n, beta)
+    assert rc == 0
+    assert max(_errs(got, fwd).values()) < TOL
+    assert max(_errs(got, rev).values()) > 1e-3 - TOL
+    # in particular on bg_T, where the shared far with a negative sdf decides which sample is last
+    assert float(np.abs(fwd[4] - rev[4]).max()) > 1e-3
+    assert float(np.abs(got[4] - fwd[4]).max()) < TOL
+
+
+def test_rejected_calls_leave_outputs_untouched():
+    """An over-cap P * n, a P outside [1, 8] and a short workspace each return a negative status with the expected
+    mp_last_error() text, and no output is written (the checks run on the host before any kernel writes)."""
+    from multiply_b200 import _lib as L
+    lib = L.lib()
+
+    def untouched(bufs):
+        return all(bool((b == SENTINEL).all()) for b in bufs.values())
+
+    persons = make_inputs(3, 8, 5, N_MAX_P8 + 1, ties=False)
+    rc, bufs = call_composite(persons, 5, N_MAX_P8 + 1, 0.1)
+    assert rc < 0 and "too large for shared memory" in lib.mp_last_error().decode() and untouched(bufs)
+    persons = make_inputs(4, 2, 5, 8)
+    for bad_P in (0, 9):
+        rc, bufs = call_composite(persons, 5, 8, 0.1, P_arg=bad_P)
+        assert rc < 0 and "bad person list" in lib.mp_last_error().decode() and untouched(bufs)
+    rc, bufs = call_composite(persons, 5, 8, 0.1, ws_delta=-1)
+    assert rc < 0 and "workspace too small" in lib.mp_last_error().decode() and untouched(bufs)
+    # the largest n that fits still runs
+    persons = make_inputs(5, 8, 2, N_MAX_P8, ties=False)
+    rc, _ = call_composite(persons, 2, N_MAX_P8, 0.1)
+    assert rc == 0
+
+
+@pytest.mark.parametrize("with_bg,with_fg_out", [(True, True), (False, True), (True, False), (False, False)])
+def test_final_compose(with_bg, with_fg_out):
+    """rgb = fg + bg_T * bg (bg NULL: white) and fg_rgb_values = fg + bg_T (may be NULL), bit for bit as fp32."""
+    from multiply_b200 import _lib as L
+    R = 1029
+    rng = np.random.RandomState(11)
+    fg = rng.random_sample((R, 3)).astype(np.float32)
+    bgT = rng.random_sample(R).astype(np.float32)
+    bgT[::7] = 1.0
+    bgT[::11] = 0.0
+    bg = rng.random_sample((R, 3)).astype(np.float32)
+    d_fg, d_T, d_bg = (torch.from_numpy(a).cuda() for a in (fg, bgT, bg))
+    rgb = _out(R, 3)
+    fgo = _out(R, 3) if with_fg_out else None
+    L.check(L.lib().mp_final_compose(d_fg.data_ptr(), d_T.data_ptr(), d_bg.data_ptr() if with_bg else None, R,
+                                     rgb.data_ptr(), L.ptr(fgo), L.stream_ptr()), "mp_final_compose")
+    torch.cuda.synchronize()
+    b = bg if with_bg else np.ones_like(bg)
+    want = (fg + (bgT[:, None] * b).astype(np.float32)).astype(np.float32)
+    assert np.array_equal(_take(rgb, R, 3, "rgb").view(np.uint32), want.view(np.uint32))
+    if with_fg_out:
+        want_fg = (fg + bgT[:, None]).astype(np.float32)
+        assert np.array_equal(_take(fgo, R, 3, "fg_rgb_values").view(np.uint32), want_fg.view(np.uint32))
