@@ -301,6 +301,39 @@ int mp_composite(const mp_person_samples_t* persons_host, int P, int R, int n, f
 int mp_final_compose(const float* fg_rgb /*[R,3]*/, const float* bg_T /*[R]*/, const float* bg_rgb /*[R,3] or NULL*/, int R,
                      float* rgb_values /*[R,3]*/, float* fg_rgb_values /*[R,3] or NULL*/, void* stream);
 
+/* Backward of the compositing stages (multiply.py:427-480, :544-545, :590, :682-696) with torch autograd's kink
+ * conventions: d sigma / d sdf = 0 at sdf == 0 (sign(0) = 0) and d|s|/ds = sign(s).  Every upstream gradient d_* may be
+ * NULL, meaning zero, unless marked required.  Each output slot is written once; deterministic (no float atomics).
+ *
+ * mp_composite_backward: the same inputs as mp_composite plus the upstream gradients d_fg_rgb [R,3], d_normal [R,3],
+ * d_acc [R], d_acc_person [R,P], d_bg_T [R]; writes per person p the sample gradients of its [R_p, n] rows and
+ * d_beta (one device float, required) = dL/dbeta for beta = |beta_param| + beta_min (the chain to beta_param is the
+ * caller's).  Rays no person hits contribute nothing (their bg_T = 1 is a constant). */
+typedef struct {
+  float* d_sdf;             /* [R_p, n] */
+  float* d_rgb;             /* [R_p, n, 3] */
+  float* d_normal;          /* [R_p, n, 3] */
+} mp_person_sample_grads_t;
+
+size_t mp_composite_backward_workspace_bytes(int R, int P);
+int mp_composite_backward(const mp_person_samples_t* persons_host, int P, int R, int n, float beta,
+                          const float* d_fg_rgb, const float* d_normal, const float* d_acc, const float* d_acc_person,
+                          const float* d_bg_T, const mp_person_sample_grads_t* grads_host, float* d_beta,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* bg_volume_rendering + the weighted sum (multiply.py:682-696, :539): bg_sdf [R,32], bg_rgb_samples [R,32,3] in the
+ * flipped depth order the networks see (the bg_sdf / bg_rgb_samples taps of mp_render_out_t); depths from bound_r and
+ * t_rand_bg [R,32] (training) or NULL (eval), the last interval 1e10 long.  d_bg_rgb [R,3] (required) ->
+ * d_bg_sdf [R,32], d_bg_rgb_samples [R,32,3]. */
+int mp_bg_composite_backward(const float* bg_sdf, const float* bg_rgb_samples, int R, float bound_r,
+                             const float* t_rand_bg_or_null, const float* d_bg_rgb, float* d_bg_sdf,
+                             float* d_bg_rgb_samples, void* stream);
+/* backward of mp_final_compose: d_fg_rgb = d_rgb_values + d_fg_rgb_values ; d_bg_T = sum_c (d_rgb_values_c * bg_rgb_c +
+ * d_fg_rgb_values_c) (bg_rgb NULL -> white) ; d_bg_rgb = bg_T * d_rgb_values (may be NULL: not written). */
+int mp_final_compose_backward(const float* bg_T /*[R]*/, const float* bg_rgb_or_null /*[R,3]*/, int R,
+                              const float* d_rgb_values /*[R,3]*/, const float* d_fg_rgb_values_or_null /*[R,3]*/,
+                              float* d_fg_rgb /*[R,3]*/, float* d_bg_T /*[R]*/, float* d_bg_rgb_or_null /*[R,3]*/,
+                              void* stream);
+
 /* background: inverse-sphere samples -> depth2pts_outside (multiply.py:698-726) -> bg nets -> bg_volume_rendering */
 size_t mp_background_workspace_bytes(int R);
 int mp_background(mp_net_t* bg_field, const float* ray_dirs, const float* cam_loc, int R, float bound_r,
@@ -351,7 +384,8 @@ int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int
 /* Training-mode forward VALUES (multiply.py:174-598 with self.training, shipped loss weights, current_epoch >= 250):
  * stochastic sampling per person (mp_sampler_rng_t), no outlier clamp in the SDF callback or the main pass
  * (multiply.py:142 is eval-only), jittered inverse-sphere depths of the background pass (the second
- * inverse_sphere_sampler.get_z_vals call, :482).  Gradients are NOT produced (SURVEY.md 8f-1, DESIGN.md 7). */
+ * inverse_sphere_sampler.get_z_vals call, :482).  The render produces no gradients itself; the backward of its
+ * compositing stages is mp_composite_backward / mp_bg_composite_backward / mp_final_compose_backward on its taps. */
 typedef struct {
   const mp_sampler_rng_t* rng[MP_MAX_PERSONS]; /* host structs of device pointers, one per person */
   float* z_eik[MP_MAX_PERSONS];                /* [R_p] z_samples_eik out, or NULL */
@@ -396,6 +430,12 @@ typedef struct {
   float* bg_T;            /* [R] or NULL */
   int* status;            /* device int or NULL: bit 0 = some ray misses the bounding sphere (the reference prints
                              'BOUNDING SPHERE PROBLEM' and exits, rend_util.py:140-142; its pixels are undefined here) */
+  /* optional background taps (NULL to skip; written only when a background is rendered), the inputs of
+   * mp_bg_composite_backward: bg_rgb [R,3] (bg_rgb_values, multiply.py:539), bg_sdf [R,32] and bg_rgb_samples [R,32,3]
+   * (the background networks' per-sample outputs in the flipped depth order of multiply.py:516) */
+  float* bg_rgb;
+  float* bg_sdf;
+  float* bg_rgb_samples;
 } mp_render_out_t;
 
 size_t mp_render_workspace_bytes(const mp_scene_t* scene, int R);

@@ -84,7 +84,12 @@ class RenderOut(C.Structure):
                 ("acc_map", C.c_void_p), ("acc_person_list", C.c_void_p),
                 ("z_vals", C.c_void_p * MP_MAX_PERSONS), ("sdf", C.c_void_p * MP_MAX_PERSONS),
                 ("rgb", C.c_void_p * MP_MAX_PERSONS), ("normals", C.c_void_p * MP_MAX_PERSONS),
-                ("trips", C.c_void_p), ("bg_T", C.c_void_p), ("status", C.c_void_p)]
+                ("trips", C.c_void_p), ("bg_T", C.c_void_p), ("status", C.c_void_p),
+                ("bg_rgb", C.c_void_p), ("bg_sdf", C.c_void_p), ("bg_rgb_samples", C.c_void_p)]
+
+
+class PersonSampleGrads(C.Structure):
+    _fields_ = [("d_sdf", C.c_void_p), ("d_rgb", C.c_void_p), ("d_normal", C.c_void_p)]
 
 
 # name -> (restype, argtypes) ; mirrors include/multiply_b200.h one to one
@@ -141,6 +146,11 @@ SIGNATURES = {
     "mp_composite_workspace_bytes": (_SZ, [_I, _I]),
     "mp_composite": (_I, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "mp_final_compose": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP]),
+    "mp_composite_backward_workspace_bytes": (_SZ, [_I, _I]),
+    "mp_composite_backward": (_I, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP,
+                                   C.POINTER(PersonSampleGrads), _VP, _VP, _SZ, _VP]),
+    "mp_bg_composite_backward": (_I, [_VP, _VP, _I, _F, _VP, _VP, _VP, _VP, _VP]),
+    "mp_final_compose_backward": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "mp_background_workspace_bytes": (_SZ, [_I]),
     "mp_background": (_I, [_VP, _VP, _VP, _I, _F, _VP, _VP, _SZ, _VP]),
     "mp_mesh_plan": (_I, [_VP, _I, _VP, _I, _F, _VP, C.POINTER(MeshPlan), _VP]),

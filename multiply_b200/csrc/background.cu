@@ -90,6 +90,45 @@ __global__ void bg_composite_kernel(const float* __restrict__ sdf, const float* 
   }
 }
 
+// Backward of bg_composite_kernel, one warp per ray, lane = sample.  With fe_j = dist_j |s_j|, T_j = exp(-sum_{k<j} fe_k),
+// w_j = T_j (1 - exp(-fe_j)) and h_j = <d bg_rgb, rgb_j>:
+//   dL/dfe_j = T_{j+1} h_j - sum_{k>j} w_k h_k ;  dL/ds_j = dL/dfe_j dist_j sign(s_j) ;  dL/drgb_j = w_j d bg_rgb
+// (sign(0) = 0: AbsDensity's autograd kink).  The last interval is 1e10 long, as in the forward.
+__global__ void bg_composite_backward_kernel(const float* __restrict__ sdf, const float* __restrict__ rgb, int R,
+                                             float inv_bound, const float* __restrict__ t_rand,
+                                             const float* __restrict__ d_out, float* __restrict__ d_sdf,
+                                             float* __restrict__ d_rgb) {
+  int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= R) return;
+  size_t i = (size_t)w * 32 + lane;
+  float s = sdf[i];
+  float dens = fabsf(s);
+  float zc = bg_depth(w, 31 - lane, inv_bound, t_rand);
+  float zn = (lane < 31) ? bg_depth(w, 30 - lane, inv_bound, t_rand) : 0.f;
+  float dist = (lane < 31) ? (zc - zn) : 1e10f;
+  float fe = dist * dens;
+  float T = expf(-warp_scan_excl(fe, lane));
+  float ex = expf(-fe);
+  float wgt = (1.f - ex) * T;
+  const float d0 = d_out[3 * (size_t)w], d1 = d_out[3 * (size_t)w + 1], d2 = d_out[3 * (size_t)w + 2];
+  float h = d0 * rgb[3 * i] + d1 * rgb[3 * i + 1] + d2 * rgb[3 * i + 2];
+  // exclusive suffix sum of w h over the lanes above
+  float incl = wgt * h;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    float t = __shfl_down_sync(0xffffffffu, incl, o);
+    if (lane + o < 32) incl += t;
+  }
+  float suf = __shfl_down_sync(0xffffffffu, incl, 1);
+  if (lane == 31) suf = 0.f;
+  float dfe = (T * ex) * h - suf;
+  float sg = (s > 0.f) ? 1.f : ((s < 0.f) ? -1.f : 0.f);
+  d_sdf[i] = dfe * dist * sg;
+  d_rgb[3 * i] = wgt * d0;
+  d_rgb[3 * i + 1] = wgt * d1;
+  d_rgb[3 * i + 2] = wgt * d2;
+}
+
 size_t bg_ws_bytes(int R) {
   size_t N = (size_t)(R > 0 ? R : 1) * 32;
   return align_up(N * 4 * 4, 256) + align_up(N * 3 * 4, 256) * 2 + align_up(N * 4, 256) + field_bg_ws_bytes((int)N) +
@@ -97,7 +136,7 @@ size_t bg_ws_bytes(int R) {
 }
 
 int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
-                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand) {
+                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand, float* tap_sdf, float* tap_rgb) {
   if (R <= 0) return 0;
   Arena a(ws, ws_bytes);
   int N = R * 32;
@@ -112,6 +151,8 @@ int render_background(const Field& f, const float* dirs, const float* cam, int R
   bg_points_kernel<<<div_up(N, 256), 256, 0, st>>>(dirs, cam, R, bound, inv_bound, pts, dexp, t_rand);
   MP_LAUNCH_CHECK();
   MP_TRY(field_bg(f, pts, dexp, N, sdf, rgb, mws, mb, st));
+  if (tap_sdf) MP_CHECK_CUDA(cudaMemcpyAsync(tap_sdf, sdf, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (tap_rgb) MP_CHECK_CUDA(cudaMemcpyAsync(tap_rgb, rgb, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   bg_composite_kernel<<<div_up(N, 256), 256, 0, st>>>(sdf, rgb, R, inv_bound, bg_rgb, t_rand);
   MP_LAUNCH_CHECK();
   return 0;
@@ -126,6 +167,19 @@ int mp_background(mp_net_t* bg_field, const float* ray_dirs, const float* cam_lo
                   void* workspace, size_t workspace_bytes, void* stream) {
   MP_REQUIRE(bg_field && ray_dirs && cam_loc && bg_rgb, "mp_background: null argument");
   return mp::render_background(bg_field->f, ray_dirs, cam_loc, R, bound_r, bg_rgb, workspace, workspace_bytes,
-                               (cudaStream_t)stream, nullptr);
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr);
+}
+
+int mp_bg_composite_backward(const float* bg_sdf, const float* bg_rgb_samples, int R, float bound_r,
+                             const float* t_rand_bg, const float* d_bg_rgb, float* d_bg_sdf, float* d_bg_rgb_samples,
+                             void* stream) {
+  MP_REQUIRE(bg_sdf && bg_rgb_samples && d_bg_rgb && d_bg_sdf && d_bg_rgb_samples,
+             "mp_bg_composite_backward: null argument");
+  if (R <= 0) return 0;
+  float inv_bound = (float)(1.0 / bound_r);
+  mp::bg_composite_backward_kernel<<<mp::div_up(R * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      bg_sdf, bg_rgb_samples, R, inv_bound, t_rand_bg, d_bg_rgb, d_bg_sdf, d_bg_rgb_samples);
+  MP_LAUNCH_CHECK();
+  return 0;
 }
 }

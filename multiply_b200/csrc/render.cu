@@ -43,7 +43,8 @@ int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cu
 int launch_final_compose(const float* fg, const float* bgT, const float* bg, int R, float* rgb, float* fg_out,
                          cudaStream_t st);
 int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
-                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand = nullptr);
+                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand = nullptr,
+                      float* tap_sdf = nullptr, float* tap_rgb = nullptr);
 size_t bg_ws_bytes(int R);
 // mesh.cu
 struct Mesh;
@@ -503,7 +504,13 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
     }
     if (rc == 0)
       rc = render_background(scene->bg_field->f, w.dirs, w.cam, R, c.scene_bounding_sphere, w.bg, w.sub[scene->P],
-                             w.sub_bytes, sb, scene->train ? scene->train->t_rand_bg : nullptr);
+                             w.sub_bytes, sb, scene->train ? scene->train->t_rand_bg : nullptr, out->bg_sdf,
+                             out->bg_rgb_samples);
+    if (rc == 0 && out->bg_rgb &&
+        cudaMemcpyAsync(out->bg_rgb, w.bg, (size_t)R * 3 * sizeof(float), cudaMemcpyDeviceToDevice, sb) != cudaSuccess) {
+      set_error("mp_render_rays: bg_rgb tap copy failed");
+      rc = -2;
+    }
     bg = w.bg;
   }
   if (fork) {

@@ -5,6 +5,8 @@ libmultiply_b200.so (see _lib.py).  No fallback path exists.
 """
 import ctypes as C
 import math
+
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -366,7 +368,13 @@ class Renderer:
         ``ErrorBoundSampler.draw_training_rng``], t_rand_bg=[R,32] or None) — stochastic sampling, no outlier clamp,
         jittered background depths; adds ``z_eik_{k}`` [R_k] per person.  With ``meshes=[CanonicalMesh per rendered
         person]`` (current_epoch < 250, multiply.py:313-316) and ``threshold`` (default 0.05) it also returns
-        ``index_off_surface`` / ``index_in_surface`` [R] bool, merged over persons as multiply.py:549-560.  No gradients.
+        ``index_off_surface`` / ``index_in_surface`` [R] bool, merged over persons as multiply.py:549-560.  With
+        ``beta=<0-d tensor>`` (the LaplaceDensity beta, equal to the fp32 |beta_param| + beta_min the sampler uses) the
+        five pixel outputs are attached to beta's graph through ``RenderComposite``: ``out["samples"]`` is a list of
+        per-person dicts of leaf tensors (sdf [R_k,n], rgb / normal [R_k,n,3], which require grad; plus z_vals [R_k,n+1]
+        and ray_index [R_k]) and, when a background is rendered, ``out["samples_bg"]`` holds its leaves (sdf [R,32],
+        rgb [R,32,3] in the flipped depth order; plus t_rand, the jitter of its depths or None, and bg_rgb [R,3]).  Backward fills their ``.grad``
+        and beta's; the networks, deformer and SMPL inputs stay outside the graph.
         Returns the eval output dict of Multiply.forward (multiply.py:589-598)."""
         with torch.cuda.device(self.device):
             return self._render(inputs, hit_lists, debug, persons, check, out, train)
@@ -406,6 +414,14 @@ class Renderer:
         keep_train = []
         z_eik = {}
         flags = {}
+        beta = train.get("beta") if train is not None else None
+        grad_on = beta is not None
+        if grad_on:
+            assert torch.is_tensor(beta) and beta.numel() == 1, "train['beta'] must be a 0-d tensor"
+            want = np.float32(abs(np.float32(self.beta_param))) + np.float32(self.beta_min)
+            assert np.float32(float(beta.detach())) == want, \
+                "train['beta'] = %r differs from the sampler's beta %r" % (float(beta.detach()), float(want))
+            assert not dev_counts, "render gradients need host-side hit counts"
         if train is not None:
             assert not dev_counts, "training mode needs host-side hit counts"
             tr = L.Train()
@@ -469,6 +485,29 @@ class Renderer:
                 out.sdf[k] = dbg[f"sdf_{k}"].data_ptr()
                 out.rgb[k] = dbg[f"rgb_{k}"].data_ptr()
                 out.normals[k] = dbg[f"normals_{k}"].data_ptr()
+        taps = None
+        if grad_on:        # the compositor's inputs, kept for RenderComposite.backward
+            n = self.n
+            taps = dict(z=[], sdf=[], rgb=[], nrm=[], bg_T=torch.empty(R, device=dev))
+            for k in range(Pn):
+                Rp = hits[k][0].numel()
+                for key, shp in (("z", (Rp, n + 1)), ("sdf", (Rp, n)), ("rgb", (Rp, n, 3)), ("nrm", (Rp, n, 3))):
+                    name = {"z": "z_vals", "sdf": "sdf", "rgb": "rgb", "nrm": "normals"}[key]
+                    t = dbg.get(f"{name}_{k}")
+                    if t is None:
+                        t = torch.empty(*shp, device=dev)
+                        getattr(out, name)[k] = t.data_ptr()
+                    taps[key].append(t)
+            if out.bg_T:
+                taps["bg_T"] = dbg["bg_T"]
+            else:
+                out.bg_T = taps["bg_T"].data_ptr()
+            if self.bg is not None:
+                taps.update(bg_rgb=torch.empty(R, 3, device=dev), bg_sdf=torch.empty(R, 32, device=dev),
+                            bg_rgb_s=torch.empty(R, 32, 3, device=dev))
+                out.bg_rgb = taps["bg_rgb"].data_ptr()
+                out.bg_sdf = taps["bg_sdf"].data_ptr()
+                out.bg_rgb_samples = taps["bg_rgb_s"].data_ptr()
         L.check(lib.mp_render_rays(C.byref(sc), uv.data_ptr(), pose.data_ptr(), K.data_ptr(), R, C.byref(out),
                                    self._ws.data_ptr(), self._ws.numel(), L.stream_ptr()), "mp_render_rays")
         self._keep = (uv, pose, K, hits, keep_train)
@@ -478,8 +517,95 @@ class Renderer:
             res[k] = v.bool()
         if check:
             self.check_status()
+        if grad_on:
+            res.update(self._attach_graph(res, taps, hits, beta, train.get("t_rand_bg"), R, Pn))
         res.update(dbg)
         return res
+
+    def _attach_graph(self, res, taps, hits, beta, t_rand_bg, R, Pn):
+        dev = self.device
+        samples = [dict(sdf=taps["sdf"][k].clone().requires_grad_(True), rgb=taps["rgb"][k].clone().requires_grad_(True),
+                        normal=taps["nrm"][k].clone().requires_grad_(True), z_vals=taps["z"][k], ray_index=hits[k][0])
+                   for k in range(Pn)]
+        leaves = [t for d in samples for t in (d["sdf"], d["rgb"], d["normal"])]
+        extra = {}
+        info = dict(n=self.n, R=R, P=Pn, beta=float(beta.detach()), hits=[h[0] for h in hits], z=taps["z"],
+                    bg_T=taps["bg_T"], bound=float(self.cfg["scene_bounding_sphere"]), device=dev, bg=None)
+        if self.bg is not None:
+            t_rand = None if t_rand_bg is None else _dev(t_rand_bg, dev)
+            bg = dict(sdf=taps["bg_sdf"].clone().requires_grad_(True), rgb=taps["bg_rgb_s"].clone().requires_grad_(True),
+                      t_rand=t_rand, bg_rgb=taps["bg_rgb"])
+            leaves += [bg["sdf"], bg["rgb"]]
+            info["bg"] = dict(rgb=taps["bg_rgb"], t_rand=t_rand)
+            extra["samples_bg"] = bg
+        names = ("rgb_values", "fg_rgb_values", "normal_values", "acc_map", "acc_person_list")
+        outs = RenderComposite.apply(info, tuple(res[k] for k in names), beta, *leaves)
+        extra.update(zip(names, outs))
+        extra["samples"] = samples
+        return extra
+
+
+class RenderComposite(torch.autograd.Function):
+    """The compositing stages of Multiply.forward as one autograd node: inputs beta (0-d) and the per-sample leaves
+    (per rendered person sdf, rgb, normal; then the background's sdf and rgb when one is rendered), outputs rgb_values,
+    fg_rgb_values, normal_values, acc_map, acc_person_list.  The forward returns the pixels the fused render already
+    produced (nothing is recomputed); the backward runs mp_final_compose_backward, mp_composite_backward and
+    mp_bg_composite_backward on the current stream.  d_beta is dL/dbeta of beta itself; the |beta_param| + beta_min
+    chain is ordinary torch on the parameter."""
+
+    @staticmethod
+    def forward(ctx, info, pixels, beta, *leaves):
+        ctx.info = info
+        ctx.beta_shape = beta.shape
+        ctx.save_for_backward(*leaves)
+        return tuple(p.detach() for p in pixels)
+
+    @staticmethod
+    def backward(ctx, d_rgb, d_fgv, d_nrm, d_acc, d_accp):
+        info = ctx.info
+        leaves = ctx.saved_tensors
+        dev, R, P, n = info["device"], info["R"], info["P"], info["n"]
+        lib = L.lib()
+
+        def g(t):
+            return None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous()
+        d_rgb, d_fgv, d_nrm, d_acc, d_accp = (g(t) for t in (d_rgb, d_fgv, d_nrm, d_acc, d_accp))
+        with torch.cuda.device(dev):
+            st = L.stream_ptr()
+            if d_rgb is None:
+                d_rgb = torch.zeros(R, 3, device=dev)
+            bg = info["bg"]
+            d_fg = torch.empty(R, 3, device=dev)
+            d_bgT = torch.empty(R, device=dev)
+            d_bg = torch.empty(R, 3, device=dev) if bg is not None else None
+            L.check(lib.mp_final_compose_backward(info["bg_T"].data_ptr(), L.ptr(bg["rgb"]) if bg else None, R,
+                                                  d_rgb.data_ptr(), L.ptr(d_fgv), d_fg.data_ptr(), d_bgT.data_ptr(),
+                                                  L.ptr(d_bg), st), "mp_final_compose_backward")
+            arr = (L.PersonSamples * P)()
+            gr = (L.PersonSampleGrads * P)()
+            grads = []
+            for k in range(P):
+                sdf, rgb, nrm = leaves[3 * k: 3 * k + 3]
+                arr[k].n_rows = info["hits"][k].numel()
+                arr[k].ray_index = info["hits"][k].data_ptr()
+                arr[k].z_vals = info["z"][k].data_ptr()
+                arr[k].sdf, arr[k].rgb, arr[k].normal = sdf.data_ptr(), rgb.data_ptr(), nrm.data_ptr()
+                gk = (torch.empty_like(sdf), torch.empty_like(rgb), torch.empty_like(nrm))
+                gr[k].d_sdf, gr[k].d_rgb, gr[k].d_normal = (t.data_ptr() for t in gk)
+                grads += gk
+            d_beta = torch.empty(1, device=dev)
+            ws = torch.empty(lib.mp_composite_backward_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
+            L.check(lib.mp_composite_backward(arr, P, R, n, info["beta"], d_fg.data_ptr(), L.ptr(d_nrm), L.ptr(d_acc),
+                                              L.ptr(d_accp), d_bgT.data_ptr(), gr, d_beta.data_ptr(), ws.data_ptr(),
+                                              ws.numel(), st), "mp_composite_backward")
+            if bg is not None:
+                b_sdf, b_rgb = leaves[3 * P], leaves[3 * P + 1]
+                d_bsdf, d_brgb = torch.empty_like(b_sdf), torch.empty_like(b_rgb)
+                L.check(lib.mp_bg_composite_backward(b_sdf.data_ptr(), b_rgb.data_ptr(), R, info["bound"],
+                                                     L.ptr(bg["t_rand"]), d_bg.data_ptr(), d_bsdf.data_ptr(),
+                                                     d_brgb.data_ptr(), st), "mp_bg_composite_backward")
+                grads += [d_bsdf, d_brgb]
+        return (None, None, d_beta.reshape(ctx.beta_shape)) + tuple(grads)
 
 
 def sampler_rng_struct(rng, dev):

@@ -111,6 +111,15 @@ class Multiply(nn.Module):
             for b in self._renderer.bodies:
                 b.set_root_finder(*self._root_finder)
 
+    def set_render_grad(self, on=True):
+        """Not in the reference's interface (the reference always back-propagates; this mirror's training forward returns
+        detached values by default): on = the training forward's pixel outputs are differentiable w.r.t.
+        ``density.beta`` and the per-sample sdf / rgb / normals and background sdf / rgb it exposes as
+        ``res["render_samples"]`` (dict(persons=[dict(sdf, rgb, normal)], bg=dict(sdf, rgb) or None), leaf tensors whose
+        ``.grad`` a network backward consumes).  ``loss.backward()`` then fills ``density.beta.grad``.  Eval mode ignores
+        the switch.  Off (default) = detached values, as before."""
+        self._render_grad = bool(on)
+
     def set_canonical_mesh(self, person_id, verts, faces):
         """Replaces person ``person_id``'s canonical mesh (verts [V,3], faces [F,3]), as multiply_model.py:504-506 does
         with the marching-cubes mesh every 20 epochs.  Its grid is rebuilt on the next use."""
@@ -303,8 +312,9 @@ class Multiply(nn.Module):
         loss weights (smpl_surface_weight = zero_pose_weight = 0, confs/model/*.yaml:77-88): stochastic sampling with the
         reference's own random stream (the same torch.manual_seed gives the same sample depths), no outlier clamp (:142 is
         eval-only), eikonal samples and their SDF gradients (:320-331), temporal loss (:242-243), jittered background
-        depths (:482).  NO autograd graph is built: the tensors are detached values — the backward pass is the open half of
-        SURVEY.md 8f-1 (DESIGN.md 7).  One scalar read per person keeps the random stream in step with the reference's
+        depths (:482).  By default NO autograd graph is built and the tensors are detached values; with
+        ``set_render_grad(True)`` the pixel outputs carry the compositing stages' graph (to density.beta and the
+        per-sample leaves of ``res["render_samples"]``; the networks' backward is still open, DESIGN.md 7).  One scalar read per person keeps the random stream in step with the reference's
         (its trip count decides how much randperm consumes).  At current_epoch < 250 the canonical points of the main
         pass are also tested against each person's canonical mesh (:313-316, check_off_in_surface_points_cano_mesh) and
         index_off_surface / index_in_surface [R] bool are the merged flags of :549-560; at >= 250 they are None."""
@@ -367,8 +377,11 @@ class Multiply(nn.Module):
             frame = self.frame_latent_encoder(input["idx"])
         if r.bg is not None:
             r.bg.set_cond(frame.detach())
-        out = r.render(input, hits, persons=person_list,
-                       train=dict(rng=rngs, t_rand_bg=t_rand_bg, meshes=meshes, threshold=self.threshold))
+        train = dict(rng=rngs, t_rand_bg=t_rand_bg, meshes=meshes, threshold=self.threshold)
+        grad_on = getattr(self, "_render_grad", False)
+        if grad_on:
+            train["beta"] = self.density.get_beta()
+        out = r.render(input, hits, persons=person_list, train=train)
         temporal = torch.zeros(1, device=dev)
         if epoch > 250:                                                    # multiply.py:242-243
             temporal = torch.mean(torch.square(input["smpl_pose_last"] - input["smpl_pose"])).reshape(1).detach()
@@ -380,6 +393,8 @@ class Multiply(nn.Module):
                "interpenetration_loss": z1, "temporal_loss": temporal, "smpl_surface_loss": z1.clone(),
                "zero_pose_loss": z1.clone(), "epoch": input["current_epoch"], "cam_loc": cam,
                "t_list": [], "fg_rgb_values_each_person_list": [], "hitted_mask_idx": [], "mean_hitted_vertex_list": []}
+        if grad_on:
+            res["render_samples"] = dict(persons=out["samples"], bg=out.get("samples_bg"))
         if "sam_mask" in input:
             res["sam_mask"] = input["sam_mask"].squeeze()
         return res

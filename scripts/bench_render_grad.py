@@ -1,0 +1,123 @@
+"""Timings of the compositing backward (csrc/composite.cu: mp_composite_backward, mp_final_compose_backward;
+csrc/background.cu: mp_bg_composite_backward) against the forward compositor mp_composite; prints one JSON line.
+
+    python scripts/bench_render_grad.py [--steps 20]
+
+Two workloads: the training step (2 persons x 512 rays x 97 samples) and BASELINE configs[1] (2 x 4096 x 193).  Every
+ray is hit by both persons (the worst case of the merge); sdf, colours and upstream gradients are seeded random data.
+Milliseconds per call from CUDA events around `steps` back-to-back calls after warm-up; the card's name and power limit
+are read in the same run.  Writes nothing to disk.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+
+def _card():
+    name = torch.cuda.get_device_name()
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10).stdout.strip()
+        limit = float(out)
+    except Exception:
+        limit = None
+    return {"card": name, "power_limit_w": limit}
+
+
+def _time(fn, steps):
+    for _ in range(3):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(steps):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / steps
+
+
+def workload(P, R, n, steps):
+    from multiply_b200 import _lib as L
+    lib = L.lib()
+    g = torch.Generator(device="cuda").manual_seed(R + n)
+    dev = "cuda"
+    arr = (L.PersonSamples * P)()
+    gr = (L.PersonSampleGrads * P)()
+    keep = []
+    for p in range(P):
+        z = torch.sort(torch.rand(R, n + 1, device=dev, generator=g) * 3 + 0.5, 1)[0]
+        t = dict(idx=torch.arange(R, device=dev), z=z.contiguous(),
+                 sdf=(torch.rand(R, n, device=dev, generator=g) - 0.5) * 0.4,
+                 rgb=torch.rand(R, n, 3, device=dev, generator=g), nrm=torch.rand(R, n, 3, device=dev, generator=g),
+                 d_sdf=torch.empty(R, n, device=dev), d_rgb=torch.empty(R, n, 3, device=dev),
+                 d_nrm=torch.empty(R, n, 3, device=dev))
+        keep.append(t)
+        arr[p].n_rows, arr[p].ray_index, arr[p].z_vals = R, t["idx"].data_ptr(), t["z"].data_ptr()
+        arr[p].sdf, arr[p].rgb, arr[p].normal = t["sdf"].data_ptr(), t["rgb"].data_ptr(), t["nrm"].data_ptr()
+        gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = t["d_sdf"].data_ptr(), t["d_rgb"].data_ptr(), t["d_nrm"].data_ptr()
+    o = {k: torch.empty(*s, device=dev) for k, s in (("fg", (R, 3)), ("nrm", (R, 3)), ("acc", (R,)), ("accp", (R, P)),
+                                                     ("bgT", (R,)))}
+    u = {k: torch.randn(*v.shape, device=dev, generator=g) for k, v in o.items()}
+    u["rgb"] = torch.randn(R, 3, device=dev, generator=g)
+    bg_rgb = torch.rand(R, 3, device=dev, generator=g)
+    bg_sdf = (torch.rand(R, 32, device=dev, generator=g) - 0.5) * 4
+    bg_rgb_s = torch.rand(R, 32, 3, device=dev, generator=g)
+    d_bg_sdf, d_bg_rgb_s = torch.empty(R, 32, device=dev), torch.empty(R, 32, 3, device=dev)
+    d_fg, d_bgT, d_bg = torch.empty(R, 3, device=dev), torch.empty(R, device=dev), torch.empty(R, 3, device=dev)
+    d_beta = torch.empty(1, device=dev)
+    ws = torch.empty(lib.mp_composite_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
+    wsb = torch.empty(lib.mp_composite_backward_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
+    st = L.stream_ptr()
+    beta = 0.1
+
+    def fwd():
+        L.check(lib.mp_composite(arr, P, R, n, beta, o["fg"].data_ptr(), o["nrm"].data_ptr(), o["acc"].data_ptr(),
+                                 o["accp"].data_ptr(), o["bgT"].data_ptr(), ws.data_ptr(), ws.numel(), st), "mp_composite")
+
+    def blend_bwd():
+        L.check(lib.mp_final_compose_backward(o["bgT"].data_ptr(), bg_rgb.data_ptr(), R, u["rgb"].data_ptr(),
+                                              u["fg"].data_ptr(), d_fg.data_ptr(), d_bgT.data_ptr(), d_bg.data_ptr(), st),
+                "mp_final_compose_backward")
+
+    def comp_bwd():
+        L.check(lib.mp_composite_backward(arr, P, R, n, beta, d_fg.data_ptr(), u["nrm"].data_ptr(), u["acc"].data_ptr(),
+                                          u["accp"].data_ptr(), d_bgT.data_ptr(), gr, d_beta.data_ptr(), wsb.data_ptr(),
+                                          wsb.numel(), st), "mp_composite_backward")
+
+    def bg_bwd():
+        L.check(lib.mp_bg_composite_backward(bg_sdf.data_ptr(), bg_rgb_s.data_ptr(), R, 3.0, None, d_bg.data_ptr(),
+                                             d_bg_sdf.data_ptr(), d_bg_rgb_s.data_ptr(), st), "mp_bg_composite_backward")
+
+    def all_bwd():
+        blend_bwd()
+        comp_bwd()
+        bg_bwd()
+    return {"persons": P, "rays": R, "samples": n,
+            "ms_composite_forward": _time(fwd, steps), "ms_final_compose_backward": _time(blend_bwd, steps),
+            "ms_composite_backward": _time(comp_bwd, steps), "ms_bg_composite_backward": _time(bg_bwd, steps),
+            "ms_backward_total": _time(all_bwd, steps)}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    a = ap.parse_args()
+    import __graft_entry__  # noqa: F401  (repository root on sys.path)
+    torch.cuda.set_device(0)
+    rec = dict(_card())
+    rec["training_step"] = workload(2, 512, 97, a.steps)
+    rec["configs1"] = workload(2, 4096, 193, a.steps)
+    print(json.dumps(rec))
+
+
+if __name__ == "__main__":
+    main()
