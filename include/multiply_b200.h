@@ -374,7 +374,9 @@ int mp_mesh_distance(const mp_mesh_t* mesh, const float* pts, int N, float* dist
  * the mesh an odd number of times (fp64 watertight crossing test).  Meaningful for watertight meshes only. */
 int mp_mesh_check_sign(const mp_mesh_t* mesh, const float* pts, int N, uint8_t* inside, void* stream);
 /* check_off_in_surface_points_cano_mesh (multiply.py:153-167): x_c [rows*N_samples,3] (row-major by ray) -> off [rows]
- * = min over the row's samples of the signed distance > thr, in [rows] = that minimum <= 0 (uint8). */
+ * = min over the row's samples of the signed distance > thr, in [rows] = that minimum <= 0 (uint8).  The signed
+ * distance is -sqrtf(d2) inside and +sqrtf(d2) outside, compared in fp32.  Any thr is allowed, including thr <= 0 (with
+ * thr < 0 an inside sample at depth d < |thr| keeps off) and +-inf; a NaN thr is an error. */
 int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int N_samples, float thr, uint8_t* off,
                           uint8_t* in, void* stream);
 
@@ -395,7 +397,7 @@ typedef struct {
    * index_off_surface [R] (AND over persons; rays a person does not hit count as off) and index_in_surface [R] (OR).
    * All NULL: no flags (epoch >= 250). */
   const mp_mesh_t* cano_mesh[MP_MAX_PERSONS];
-  float surface_threshold;                     /* 0.05 (multiply.py:88) */
+  float surface_threshold;                     /* 0.05 (multiply.py:88); any value but NaN (mp_mesh_surface_flags) */
   uint8_t* index_off_surface;                  /* [R] out, required when a mesh is set */
   uint8_t* index_in_surface;                   /* [R] out, required when a mesh is set */
 } mp_train_t;

@@ -412,10 +412,13 @@ __global__ void mesh_sign_kernel(Mesh m, const float* __restrict__ pts, int N, u
 
 // Per-ray flags of check_off_in_surface_points_cano_mesh (multiply.py:153-167): with signed distance
 // s = (inside ? -1 : 1) * sqrtf(d2), off[row] = AND_s (s > thr), in[row] = OR_s (s <= 0) (= the reference's min tests).
-// Inside samples clear off and set in.  Outside samples need the distance only up to thr: the capped query is exact
-// below (thr (1 + 1e-6))^2, beyond which sqrtf(float(d2)) > thr.  off / in are initialised to 1 / 0 by the caller and
-// only ever written 0 / 1, so the result does not depend on the order of the points.  Point i is sample slot[i] of
-// row slot[i] / n (slot == NULL: slot = i); the number of points is *count_dev when given.
+// Inside samples set in; with thr >= 0 they also clear off (s <= 0 <= thr).  Otherwise the sample needs its distance
+// only up to |thr|: the capped query is exact below cap2 = max((thr (1 + 1e-6))^2, 2^-120), beyond which
+// sqrtf(float(d2)) > |thr| (the floor keeps float(d2) a normal float, so it cannot round to 0).  Past the cap an outside
+// sample keeps off (s > |thr| >= thr) and an inside one clears it (s < -|thr| = thr).  thr must not be NaN (the entry
+// points reject it).  off / in are initialised to 1 / 0 by the caller and only ever written 0 / 1, so the result does
+// not depend on the order of the points.  Point i is sample slot[i] of row slot[i] / n (slot == NULL: slot = i); the
+// number of points is *count_dev when given.
 __global__ void mesh_flags_kernel(Mesh m, const float* __restrict__ xc, const int* __restrict__ slot,
                                   const int* __restrict__ count_dev, int cap, int n, float thr, double cap2,
                                   uint8_t* __restrict__ off, uint8_t* __restrict__ in) {
@@ -424,24 +427,32 @@ __global__ void mesh_flags_kernel(Mesh m, const float* __restrict__ xc, const in
   if (i >= N) return;
   const int row = (slot ? slot[i] : i) / n;
   const D3 p = {(double)xc[3 * (size_t)i], (double)xc[3 * (size_t)i + 1], (double)xc[3 * (size_t)i + 2]};
-  if (mesh_inside(m, p)) {
-    off[row] = 0;
+  const bool inside = mesh_inside(m, p);
+  if (inside) {
     in[row] = 1;
-    return;
+    if (thr >= 0.f) {
+      off[row] = 0;
+      return;
+    }
   }
   double best;
   int f, t;
-  if (!mesh_nearest(m, p, cap2, best, f, t)) return;     // nothing within thr: this sample keeps off
+  if (!mesh_nearest(m, p, cap2, best, f, t)) {     // farther than |thr|
+    if (inside) off[row] = 0;
+    return;
+  }
   const float d = sqrtf((float)best);
-  if (!(d > thr)) off[row] = 0;
-  if (d <= 0.f) in[row] = 1;
+  const float s = inside ? -d : d;
+  if (!(s > thr)) off[row] = 0;
+  if (s <= 0.f) in[row] = 1;
 }
 
 int launch_surface_flags(const Mesh& m, const float* xc, const int* slot, const int* count_dev, int cap, int n,
                          float thr, uint8_t* off, uint8_t* in, cudaStream_t st) {
   if (cap <= 0) return 0;
   const double c = (double)thr * (1.0 + 1e-6);
-  mesh_flags_kernel<<<div_up(cap, 128), 128, 0, st>>>(m, xc, slot, count_dev, cap, n, thr, c * c, off, in);
+  const double cap2 = fmax(c * c, 0x1p-120);
+  mesh_flags_kernel<<<div_up(cap, 128), 128, 0, st>>>(m, xc, slot, count_dev, cap, n, thr, cap2, off, in);
   MP_LAUNCH_CHECK();
   return 0;
 }
@@ -576,6 +587,7 @@ int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int
                           uint8_t* in, void* stream) {
   MP_REQUIRE(mesh && x_c && off && in, "mp_mesh_surface_flags: null argument");
   MP_REQUIRE(N_samples >= 1 && rows >= 0, "mp_mesh_surface_flags: bad sizes");
+  MP_REQUIRE(!isnan(thr), "mp_mesh_surface_flags: thr is NaN");
   if (rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   MP_CHECK_CUDA(cudaMemsetAsync(off, 1, rows, st));

@@ -434,6 +434,7 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
              scene->P);
   MP_REQUIRE(n_mesh == 0 || (tr->index_off_surface && tr->index_in_surface),
              "mp_render_rays: surface flags need index_off_surface and index_in_surface outputs");
+  MP_REQUIRE(n_mesh == 0 || !isnan(tr->surface_threshold), "mp_render_rays: surface_threshold is NaN");
   const cudaStream_t caller = (cudaStream_t)stream;
   const mp_sampler_cfg_t& c = scene->sampler;
   const int n = c.N_samples + c.N_samples_extra + 1;     // multiply.py:290-292

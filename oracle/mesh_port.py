@@ -79,6 +79,9 @@ def point_to_mesh_distance(points, face_vertices, chunk_pairs=1 << 22, return_se
     for s in range(0, N, step):
         p = x[s:s + step, None]
         d, t = _closest_point_triangle(p, a, b, c)
+        # a (near-)degenerate face can reach the face-interior case with va + vb + vc == 0 and get a NaN distance: it
+        # has no distance and is skipped, as mesh.cu's comparisons skip it (its edges are other faces' edges)
+        d = torch.where(torch.isnan(d), torch.full_like(d, float("inf")), d)
         m = d.min(1)[0]
         i = (d == m[:, None]).int().argmax(1)          # lowest index among exact ties
         d2[s:s + step], idx[s:s + step] = m, i

@@ -173,10 +173,10 @@ def test_forward_training_early_epoch_mirror(golden_dir):
         assert np.median(d) < 1e-5 and d.max() < tol, (k, float(d.max()))
 
 
-def _render_train(r, inp, hits, rngs, t_rand_bg, meshes, persons=None):
+def _render_train(r, inp, hits, rngs, t_rand_bg, meshes, persons=None, thr=0.05):
     tr = dict(rng=rngs, t_rand_bg=t_rand_bg)
     if meshes is not None:
-        tr.update(meshes=meshes, threshold=0.05)
+        tr.update(meshes=meshes, threshold=thr)
     out = r.render(inp, hits, debug=True, persons=persons, train=tr)
     torch.cuda.synchronize()
     return out
@@ -201,9 +201,10 @@ def _fused_setup(R=256, empty_person1=False):
     return sc, r, inp, hits, meshes, rngs, torch.rand(R, 32)
 
 
-def _flags_from_taps(sc, r, inp, hits, meshes, out, plist):
+def _flags_from_taps(sc, r, inp, hits, meshes, out, plist, thr=0.05, xc_out=None):
     """The flags recomputed with mp_mesh_surface_flags from the main pass's canonical points (z taps -> samples ->
-    mp_deform_inverse), merged on the host as multiply.py:549-560."""
+    mp_deform_inverse), merged on the host as multiply.py:549-560.  xc_out (a list) receives each person's (rows,
+    canonical points)."""
     from multiply_b200.model import rend_util
     dirs, cam = rend_util.get_camera_params(inp["uv"].cuda(), inp["pose"].cuda(), inp["intrinsics"].cuda())
     dirs = dirs[0]
@@ -218,7 +219,9 @@ def _flags_from_taps(sc, r, inp, hits, meshes, out, plist):
         z = out[f"z_vals_{k}"][:, :n]
         pts = (cam[h][:, None] + z[..., None] * dirs[h][:, None]).reshape(-1, 3)
         xc, _ = r.bodies[p].deform_inverse(pts, exact_far=True)
-        o, i = meshes[k].surface_flags(xc, n)
+        o, i = meshes[k].surface_flags(xc, n, thr)
+        if xc_out is not None:
+            xc_out.append((h, xc))
         off[h, k] = o
         inn[h, k] = i
     return off.all(1), inn.any(1)
