@@ -108,9 +108,6 @@ int mp_set_streams(int on);
  * on the recorded events and returns summed milliseconds, launch counts and processed points (host arrays of 4). */
 int mp_profile_enable(int on);
 int mp_profile_read(double* ms_host, long long* launches_host, double* points_host, int reset);
-/* Diagnostics: copies out the device buffer of per-tile cycle stamps (up to 4096 values).  The wgmma kernel records no
- * stamps, so it reads back zeros; the entry point is kept so that callers built against this header keep linking. */
-int mp_tc_trace_read(unsigned long long* out, int n);
 
 /* ImplicitNet.forward (networks.py:126-208): x [N,d_in] -> out [N,257] (sdf | feature).
  * sdf / feat may be NULL.  Replaces `self.foreground_implicit_network_list[p](x_c, cond)`. */

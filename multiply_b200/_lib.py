@@ -110,7 +110,6 @@ SIGNATURES = {
     "mp_get_precision": (_I, []),
     "mp_profile_enable": (_I, [_I]),
     "mp_set_streams": (_I, [_I]),
-    "mp_tc_trace_read": (_I, [C.POINTER(C.c_ulonglong), _I]),
     "mp_profile_read": (_I, [C.POINTER(C.c_double), C.POINTER(C.c_longlong), C.POINTER(C.c_double), _I]),
     "mp_implicit_forward": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),
     "mp_implicit_forward_grad": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, _VP]),

@@ -8,10 +8,6 @@
 
 namespace mp {
 
-int field_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-             size_t ws_bytes, cudaStream_t st);   // render.cu (engine dispatch)
-size_t field_bg_ws_bytes(int N);
-
 __device__ __forceinline__ float bg_linspace32(int i) {
   float step = 1.0f / 31.0f;
   return (i < 16) ? fmaf(step, (float)i, 0.f) : fmaf(-step, (float)(31 - i), 1.0f);
@@ -131,7 +127,7 @@ __global__ void bg_composite_backward_kernel(const float* __restrict__ sdf, cons
 
 size_t bg_ws_bytes(int R) {
   size_t N = (size_t)(R > 0 ? R : 1) * 32;
-  return align_up(N * 4 * 4, 256) + align_up(N * 3 * 4, 256) * 2 + align_up(N * 4, 256) + field_bg_ws_bytes((int)N) +
+  return align_up(N * 4 * 4, 256) + align_up(N * 3 * 4, 256) * 2 + align_up(N * 4, 256) + field_ws_bytes((int)N) +
          4096;
 }
 
@@ -144,7 +140,7 @@ int render_background(const Field& f, const float* dirs, const float* cam, int R
   float* dexp = a.take<float>((size_t)N * 3);
   float* rgb = a.take<float>((size_t)N * 3);
   float* sdf = a.take<float>(N);
-  size_t mb = field_bg_ws_bytes(N);
+  size_t mb = field_ws_bytes(N);
   void* mws = a.take<char>(mb);
   MP_REQUIRE(a.ok, "background: workspace too small (%zu needed, %zu given)", a.off, ws_bytes);
   float inv_bound = (float)(1.0 / bound);

@@ -145,7 +145,9 @@ struct Field {
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
 static inline int clamp_wpc(size_t v) { return v < 1 ? 1 : (v > 8 ? 8 : (int)v); }
 
-// engines (mlp_simt.cu, mlp_tc.cu)
+// ---- cross-file launchers: every internal function or type one .cu file uses from another --------
+
+// fp32 SIMT engine (mlp_simt.cu)
 size_t simt_workspace_bytes(int N);
 int simt_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
                   float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
@@ -156,15 +158,79 @@ int simt_bg(const Field& f, const float* pts, const float* dirs, int N, float* s
             size_t ws_bytes, cudaStream_t st);
 int simt_render(const Field& f, const float* pts, const float* nrm, const float* feat, int N, float* rgb, void* ws,
                 size_t ws_bytes, cudaStream_t st);
-extern std::atomic<int> g_engine;
 
-// cross-file launchers
+// tensor-core engine (mlp_tc.cu)
+size_t tc_workspace_bytes(int N);
+int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
+                float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
+                  const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
+                  float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int tc_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
+          size_t ws_bytes, cudaStream_t st);
+int tc_pack(Field& f, Arena& a, cudaStream_t st);
+size_t tc_pack_bytes();
+void tc_free(Field& f);
+int prof_enable(int on);
+int prof_read(double* ms, long long* launches, double* points, int reset);
+extern std::atomic<int> g_precision;
+
+// engine dispatch (render.cu): g_engine 1 = tensor cores, 0 = SIMT; field_ws_bytes covers either engine
+extern std::atomic<int> g_engine;
+size_t field_ws_bytes(int N);
+int field_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
+                   float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int field_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
+                     const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
+                     float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int field_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
+             size_t ws_bytes, cudaStream_t st);
+
+// deformer (deform.cu)
 int launch_deform_rays(const Body& b, const float* dirs, const float* cam, const float* z, int z_stride,
                        const int* zpos, int zpos_stride, int n_per_ray, int R, int prune, float* sdf_out,
                        int sdf_stride, float* xc_list, int* slot_list, int* count, uint8_t* outlier_out,
                        const int* active, cudaStream_t st, const int* R_dev = nullptr);
 int launch_forward_jac(const Body& b, const float* x_c, int N, const int* n_dev, float* x_d, float* Jinv,
                        int jstride, cudaStream_t st);
+
+// error-bound ray sampler (sampler.cu)
+int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field, const float* dirs,
+                const float* cam, int R, float* z_final, float* z_bg, int* trips_out, void* ws, size_t ws_bytes,
+                cudaStream_t st, const int* R_dev = nullptr, const mp_sampler_rng_t* rng = nullptr,
+                float* z_eik = nullptr);
+size_t sampler_ws_bytes(const mp_sampler_cfg_t& c, int R);
+
+// multi-person compositor (composite.cu)
+struct CompositePersons {
+  int P;
+  int n_rows[MP_MAX_PERSONS];
+  const int* row_of_ray[MP_MAX_PERSONS];   // [R] -> row in the person's hit list or -1
+  const float* z[MP_MAX_PERSONS];          // [R_p, n+1]
+  const float* sdf[MP_MAX_PERSONS];        // [R_p, n]
+  const float* rgb[MP_MAX_PERSONS];        // [R_p, n, 3]
+  const float* nrm[MP_MAX_PERSONS];        // [R_p, n, 3]
+};
+int launch_composite(const CompositePersons& cp, int R, int n, float beta, float* fg_rgb, float* normal, float* acc,
+                     float* acc_person, float* bg_T, cudaStream_t st);
+int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cudaStream_t st,
+                      const int* n_dev = nullptr);
+int launch_final_compose(const float* fg, const float* bgT, const float* bg, int R, float* rgb, float* fg_out,
+                         cudaStream_t st);
+
+// background (background.cu)
+int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
+                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand = nullptr,
+                      float* tap_sdf = nullptr, float* tap_rgb = nullptr);
+size_t bg_ws_bytes(int R);
+
+// canonical meshes (mesh.cu)
+struct Mesh;
+const Mesh& mesh_of(const mp_mesh_t* h);
+int launch_surface_flags(const Mesh& m, const float* xc, const int* slot, const int* count_dev, int cap, int n,
+                         float thr, uint8_t* off, uint8_t* in, cudaStream_t st);
+int launch_merge_flags(const int64_t* idx, int rows, const int* rows_dev, const uint8_t* off_p, const uint8_t* in_p,
+                       uint8_t* off, uint8_t* in, cudaStream_t st);
 
 }  // namespace mp
 
@@ -204,6 +270,24 @@ __device__ __forceinline__ float warp_scan_excl(float v, int lane) {
   float incl = warp_scan_incl(v, lane);
   float up = __shfl_up_sync(0xffffffffu, incl, 1);
   return lane == 0 ? 0.f : up;
+}
+
+// binary searches of v in the ascending a[0, n): upper_bound = #elements <= v, lower_bound = #elements < v
+__device__ __forceinline__ int upper_bound(const float* a, int n, float v) {   // first i with a[i] > v
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    int mid = (lo + hi) >> 1;
+    if (a[mid] > v) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+__device__ __forceinline__ int lower_bound(const float* a, int n, float v) {   // first i with a[i] >= v
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    int mid = (lo + hi) >> 1;
+    if (a[mid] >= v) hi = mid; else lo = mid + 1;
+  }
+  return lo;
 }
 
 // LaplaceDensity.density_func (lib/model/density.py:20-25):

@@ -12,16 +12,6 @@
 
 namespace mp {
 
-struct CompositePersons {
-  int P;
-  int n_rows[MP_MAX_PERSONS];
-  const int* row_of_ray[MP_MAX_PERSONS];   // [R] -> row in the person's hit list or -1
-  const float* z[MP_MAX_PERSONS];          // [R_p, n+1]
-  const float* sdf[MP_MAX_PERSONS];        // [R_p, n]
-  const float* rgb[MP_MAX_PERSONS];        // [R_p, n, 3]
-  const float* nrm[MP_MAX_PERSONS];        // [R_p, n, 3]
-};
-
 __global__ void fill_int_kernel(int* p, int n, int v) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -31,23 +21,6 @@ __global__ void row_of_ray_kernel(const int64_t* __restrict__ idx, int n_rows, i
   if (n_dev) n_rows = min(n_rows, *n_dev);
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_rows) row_of_ray[idx[i]] = i;
-}
-
-__device__ __forceinline__ int count_le(const float* a, int n, float v) {   // #elements <= v
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    int mid = (lo + hi) >> 1;
-    if (a[mid] > v) hi = mid; else lo = mid + 1;
-  }
-  return lo;
-}
-__device__ __forceinline__ int count_lt(const float* a, int n, float v) {   // #elements < v
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    int mid = (lo + hi) >> 1;
-    if (a[mid] >= v) hi = mid; else lo = mid + 1;
-  }
-  return lo;
 }
 
 // Rank of every sample of the ray in the merged (t_end, person, sample) order; scatters sigma * delta into ssd[rank]
@@ -70,7 +43,7 @@ __device__ __forceinline__ void merge_ranks(const CompositePersons& cp, const in
       int r = i;
       for (int q = 0; q < P; ++q) {
         if (q == p || row[q] < 0) continue;
-        r += (q < p) ? count_le(ste + q * n, n, te) : count_lt(ste + q * n, n, te);
+        r += (q < p) ? upper_bound(ste + q * n, n, te) : lower_bound(ste + q * n, n, te);
       }
       float ts = z[i];
       float sigma = laplace_density(s[i], beta);       // multiply.py:450

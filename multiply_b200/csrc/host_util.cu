@@ -29,7 +29,7 @@ int sm_count() {
 
 extern "C" {
 
-int mp_version(void) { return 100; }
+int mp_version(void) { return 101; }
 
 const char* mp_last_error(void) { return mp::g_err; }
 

@@ -8,10 +8,6 @@
 
 namespace mp {
 
-int tc_pack(Field& f, Arena& a, cudaStream_t st);   // mlp_tc.cu
-size_t tc_pack_bytes();
-void tc_free(Field& f);
-
 // W_nat[o][i] = (g ? g[o] * v[o][i] / ||v[o]|| : v[o][i]) * scale ; one warp per output row
 __global__ void fold_kernel(const float* __restrict__ v, const float* __restrict__ g, int out, int in, float scale,
                             float* __restrict__ W) {
@@ -232,6 +228,7 @@ int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, in
     rc = -3;
   }
   if (rc) {
+    tc_free(f);
     delete h;
     return rc;
   }

@@ -309,6 +309,27 @@ int simt_sdf_list(const Field& f, const float* xc_list, const int* slot_list, co
 
 __global__ void sub_count_kernel(const int* c, int s, int* out) { *out = c ? max(0, *c - s) : 0x7fffffff; }
 
+// RenderingNet layers on the colour input cin [n, ldc] (networks.py:290-312): ReLU layers ping-ponging between c0 and
+// c1, the sigmoid head into a [n,4]-strided buffer, then rgb repacked 3-strided to its slot (dense when slot is null)
+static int simt_colour(const Field& f, const float* cin, int ldc, int n, const int* n_dev, float* c0, float* c1,
+                       const int* slot, float* rgb_out, cudaStream_t st) {
+  MP_TRY(dense(cin, ldc, nullptr, 0, f.ren_Wt[0], f.ren_out[0], f.ren_b0_eff, c0, 256, nullptr, n, n_dev, ldc,
+               f.ren_out[0], ACT_RELU, st));
+  for (int l = 1; l < f.n_ren - 1; ++l) {
+    MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[l], f.ren_out[l], f.ren_b[l], c1, 256, nullptr, n, n_dev, f.ren_in[l],
+                 f.ren_out[l], ACT_RELU, st));
+    float* t = c0;
+    c0 = c1;
+    c1 = t;
+  }
+  const int L = f.n_ren - 1;
+  MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[L], f.ren_out[L], f.ren_b[L], c1, 4, nullptr, n, n_dev, f.ren_in[L], 3,
+               ACT_SIGMOID, st));
+  scatter_rgb4_kernel<<<div_up(n, 256), 256, 0, st>>>(c1, n, n_dev, slot, rgb_out);
+  MP_LAUNCH_CHECK();
+  return 0;
+}
+
 // full foreground shading of a compact list: sdf (scatter), normals (scatter), rgb (scatter)
 // grad_out (optional, [cap,3] dense) receives d sdf / d x_c ; feat_out (optional, dense [cap,256]).
 int simt_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
@@ -373,24 +394,8 @@ int simt_shade_list(const Field& f, const float* xc_list, const int* slot_list, 
     MP_LAUNCH_CHECK();
     copy_cols_kernel<<<div_up(n * 256, 256), 256, 0, st>>>(featp, 256, 0, 256, n, nrem, b.cin, ldc, 6);
     MP_LAUNCH_CHECK();
-    float* c0 = b.H0;
-    float* c1 = b.H1;
-    MP_TRY(dense(b.cin, ldc, nullptr, 0, f.ren_Wt[0], f.ren_out[0], f.ren_b0_eff, c0, 256, nullptr, n, nrem, ldc,
-                 f.ren_out[0], ACT_RELU, st));
-    for (int l = 1; l < f.n_ren - 1; ++l) {
-      MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[l], f.ren_out[l], f.ren_b[l], c1, 256, nullptr, n, nrem,
-                   f.ren_in[l], f.ren_out[l], ACT_RELU, st));
-      float* t = c0;
-      c0 = c1;
-      c1 = t;
-    }
-    int L = f.n_ren - 1;
-    MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[L], f.ren_out[L], f.ren_b[L], c1, 4, nullptr, n, nrem, f.ren_in[L], 3,
-                 ACT_SIGMOID, st));
-    // c1 is [n,4]-strided rgb; repack to 3-strided via scatter
-    scatter_rgb4_kernel<<<div_up(n, 256), 256, 0, st>>>(c1, n, nrem, slot_list ? slot_list + s : nullptr,
-                                                        slot_list ? rgb_out : rgb_out + 3 * (size_t)s);
-    MP_LAUNCH_CHECK();
+    MP_TRY(simt_colour(f, b.cin, ldc, n, nrem, b.H0, b.H1, slot_list ? slot_list + s : nullptr,
+                       slot_list ? rgb_out : rgb_out + 3 * (size_t)s, st));
     scatter3_kernel<<<div_up(n, 256), 256, 0, st>>>(b.ntmp, n, nrem, slot_list ? slot_list + s : nullptr,
                                                     slot_list ? normal_out : normal_out + 3 * (size_t)s);
     MP_LAUNCH_CHECK();
@@ -441,22 +446,7 @@ int simt_bg(const Field& f, const float* pts, const float* dirs, int N, float* s
     // features straight into the colour input block
     MP_TRY(dense(h7, 256, nullptr, 0, f.imp_Wt[8] + 1, kHidden + 1, f.imp_b[8] + 1, b.cin + X, ldc, nullptr, n,
                  nullptr, kHidden, kHidden, ACT_NONE, st));
-    float* c0 = (h7 == b.H0) ? b.H1 : b.H0;
-    float* c1 = h7;
-    MP_TRY(dense(b.cin, ldc, nullptr, 0, f.ren_Wt[0], f.ren_out[0], f.ren_b0_eff, c0, 256, nullptr, n, nullptr, ldc,
-                 f.ren_out[0], ACT_RELU, st));
-    for (int l = 1; l < f.n_ren - 1; ++l) {
-      MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[l], f.ren_out[l], f.ren_b[l], c1, 256, nullptr, n, nullptr,
-                   f.ren_in[l], f.ren_out[l], ACT_RELU, st));
-      float* t = c0;
-      c0 = c1;
-      c1 = t;
-    }
-    int L = f.n_ren - 1;
-    MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[L], f.ren_out[L], f.ren_b[L], c1, 4, nullptr, n, nullptr,
-                 f.ren_in[L], 3, ACT_SIGMOID, st));
-    scatter_rgb4_kernel<<<div_up(n, 256), 256, 0, st>>>(c1, n, nullptr, nullptr, rgb + 3 * (size_t)s);
-    MP_LAUNCH_CHECK();
+    MP_TRY(simt_colour(f, b.cin, ldc, n, nullptr, (h7 == b.H0) ? b.H1 : b.H0, h7, nullptr, rgb + 3 * (size_t)s, st));
   }
   return 0;
 }
@@ -488,22 +478,7 @@ int simt_render(const Field& f, const float* pts, const float* nrm, const float*
     colour_input_kernel<<<div_up(n * ldc, 256), 256, 0, st>>>(pts + 3 * (size_t)s, nrm + 3 * (size_t)s,
                                                              feat + 256 * (size_t)s, n, b.cin, ldc);
     MP_LAUNCH_CHECK();
-    float* c0 = b.H0;
-    float* c1 = b.H1;
-    MP_TRY(dense(b.cin, ldc, nullptr, 0, f.ren_Wt[0], f.ren_out[0], f.ren_b0_eff, c0, 256, nullptr, n, nullptr, ldc,
-                 f.ren_out[0], ACT_RELU, st));
-    for (int l = 1; l < f.n_ren - 1; ++l) {
-      MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[l], f.ren_out[l], f.ren_b[l], c1, 256, nullptr, n, nullptr,
-                   f.ren_in[l], f.ren_out[l], ACT_RELU, st));
-      float* t = c0;
-      c0 = c1;
-      c1 = t;
-    }
-    int L = f.n_ren - 1;
-    MP_TRY(dense(c0, 256, nullptr, 0, f.ren_Wt[L], f.ren_out[L], f.ren_b[L], c1, 4, nullptr, n, nullptr,
-                 f.ren_in[L], 3, ACT_SIGMOID, st));
-    scatter_rgb4_kernel<<<div_up(n, 256), 256, 0, st>>>(c1, n, nullptr, nullptr, rgb + 3 * (size_t)s);
-    MP_LAUNCH_CHECK();
+    MP_TRY(simt_colour(f, b.cin, ldc, n, nullptr, b.H0, b.H1, nullptr, rgb + 3 * (size_t)s, st));
   }
   return 0;
 }

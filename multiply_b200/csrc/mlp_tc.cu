@@ -92,7 +92,6 @@ struct TcIO {
   float* nrm_out;        // [slots,3]
   float* grad_out;       // [cap,3] dense or nullptr
   float* feat_out;       // [cap,256] dense or nullptr
-  int knobs;             // diagnostics (MP_TC_KNOBS bit mask): bit 2 = keep the dead scratch lines (no discard.global.L2)
   float rz;              // relative truncation loss of ONE tensor-core accumulation (see kRzPerMma)
   char* scratch;         // per-CTA scratch
   size_t scratch_per_cta;
@@ -336,9 +335,6 @@ struct KTag {
   static constexpr int value = K;
 };
 
-// kept for the mp_tc_trace_read ABI (cycle stamps of an instrumented build)
-__device__ unsigned long long g_trace[4096];
-
 __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
                                                                const __grid_constant__ TcIO io) {
   extern __shared__ uint8_t smem_raw[];
@@ -407,7 +403,6 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   float* ge = (float*)(scr + kSigBytes + kFeatBytes);          // [96][128]
   float* emb = (float*)(scr + kSigBytes + kFeatBytes + kGeBytes);   // [96][128]
   const int d = P.d_in, E = P.E;
-  const bool keep_lines = (io.knobs & 4) != 0;
 
   float acc[128];
 #pragma unroll
@@ -577,7 +572,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
           const uint4 fh = ld_stream(&fsc[(size_t)jp * 128 + t]);
           const uint4 fl = ld_stream(&fsc[(size_t)(16 + jp) * 128 + t]);
           store_pairs(lane_base, lane_x, jp, fh, fl);
-          if ((lane & 7) == 0 && !keep_lines) {
+          if ((lane & 7) == 0) {
             discard_line(&fsc[(size_t)jp * 128 + t], fh.x);
             discard_line(&fsc[(size_t)(16 + jp) * 128 + t], fl.x);
           }
@@ -741,7 +736,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
                 for (int e = 0; e < 4; ++e) u[e] *= isc * sv[e];
               }
               // this group's sigma' line is dead: drop it from L2
-              if (st.sig >= 0 && (lane & 7) == 0 && !keep_lines) discard_line(sp, s4.x);
+              if (st.sig >= 0 && (lane & 7) == 0) discard_line(sp, s4.x);
             } else {   // K_RELU
 #pragma unroll
               for (int e = 0; e < 4; ++e) u[e] = fmaxf(fmaf(u[e], isc, b[e & 1]), 0.f);
@@ -920,37 +915,41 @@ size_t tc_pack_bytes() {
 }
 
 struct PackCtx {
-  Arena* a;
   cudaStream_t st;
   uint8_t* blob;
   int nslots;
   int nlayers;        // packed layers so far (index into scales / inv_scale)
   float* scales;      // [kMaxLayers][2] (scale, inv)
   float* inv_scale;   // [kMaxSteps]
-  int rc;
 };
 
-static int pack_layer(PackCtx& c, TcStep& stp, const float* W, int ld, int transposed, int n_off, int k_off,
-                      int n_valid, int k_valid, int nk, int total_elems, int perm16 = 0) {
-  const int first = c.nslots;
-  const int step = c.nlayers++;
-  stp.slot_off = first;
-  stp.sc = step;
+// One layer step: its descriptor, the 2^s scale of W and nk K-chunks of hi/lo weight slots holding B[n][k] = W[n_off + n][k]
+// (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere.  The n_valid output columns carry data.
+static int pack_layer(PackCtx& c, TcStep& stp, int epi, int flags, int sig, const float* bias, const float* W, int ld,
+                      int transposed, int n_off, int n_valid, int k_valid, int nk, int total_elems, int perm16 = 0) {
+  const int layer = c.nlayers++;
+  stp.nk = nk;
+  stp.epi = epi;
+  stp.flags = flags;
+  stp.sig = sig;
+  stp.bias = bias;
+  stp.ncols = n_valid;
+  stp.slot_off = c.nslots;
+  stp.sc = layer;
   stp.terms = 3;
-  if (c.rc) return first;
-  absmax_kernel<<<1, 256, 0, c.st>>>(W, total_elems, c.scales + 2 * step);
-  g_launches++;
+  absmax_kernel<<<1, 256, 0, c.st>>>(W, total_elems, c.scales + 2 * layer);
+  MP_LAUNCH_CHECK();
   for (int kc = 0; kc < nk; ++kc) {
     uint8_t* hi = c.blob + (size_t)c.nslots * kSlotBytes;
     uint8_t* lo = hi + kSlotBytes;
-    pack_slot_kernel<<<64, 256, 0, c.st>>>(W, ld, transposed, n_off, k_off, n_valid, k_valid, kc,
-                                           c.scales + 2 * step, hi, lo, perm16);
-    g_launches++;
+    pack_slot_kernel<<<64, 256, 0, c.st>>>(W, ld, transposed, n_off, 0, n_valid, k_valid, kc, c.scales + 2 * layer, hi,
+                                           lo, perm16);
+    MP_LAUNCH_CHECK();
     c.nslots += 2;
   }
-  copy_strided_kernel<<<1, 1, 0, c.st>>>(c.scales + 2 * step + 1, 1, 1, c.inv_scale + step);
-  g_launches++;
-  return first;
+  copy_strided_kernel<<<1, 1, 0, c.st>>>(c.scales + 2 * layer + 1, 1, 1, c.inv_scale + layer);
+  MP_LAUNCH_CHECK();
+  return 0;
 }
 
 void tc_free(Field& f) {
@@ -958,15 +957,14 @@ void tc_free(Field& f) {
   f.tc = nullptr;
 }
 
+// The three programs, one pack_layer per step (epilogue, flags, sigma' layer, bias, then the weight source).
 int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   TcBlob* tb = new TcBlob();
   memset(tb, 0, sizeof(*tb));
   f.tc = tb;
   const int E = f.emb_dim;
   PackCtx c;
-  c.a = &a;
   c.st = st;
-  c.rc = 0;
   c.nslots = 0;
   c.nlayers = 0;
   c.blob = (uint8_t*)a.take<uint4>((size_t)170 * kSlotBytes / 16);
@@ -990,23 +988,16 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   P.Wrgb = Wrgb;
   P.n_extra = f.ren_extra;
   copy_strided_kernel<<<1, 256, 0, st>>>(f.imp_W[8], 1, 256, w8row);     // W8[0,:]
-  g_launches++;
+  MP_LAUNCH_CHECK();
   copy_strided_kernel<<<1, 256, 0, st>>>(f.imp_b[8] + 1, 1, 256, b8feat);
-  g_launches++;
+  MP_LAUNCH_CHECK();
   int s = 0;
-  const int nk0 = (E + 63) / 64;
   // ---- forward L0..L7 ----
   for (int l = 0; l < 8; ++l) {
-    int in = f.imp_in[l], out = f.imp_out[l];
-    int nk = (l == 0) ? nk0 : 4;
-    pack_layer(c, P.step[s], f.imp_W[l], in, 0, 0, 0, out, (l == 0) ? E : in, nk, out * in);
-    P.step[s].nk = nk;
-    P.step[s].epi = EPI_SOFTPLUS;
-    P.step[s].flags = F_SAVE_SIG | ((l == f.skip_layer - 1) ? F_INJECT_EMB : 0) | ((l == 7) ? F_SDF_DOT : 0);
-    P.step[s].sig = l;
-    P.step[s].bias = (l == 0) ? f.imp_b0_eff : f.imp_b[l];
-    P.step[s].ncols = out;
-    ++s;
+    const int in = f.imp_in[l], out = f.imp_out[l];
+    const int flags = F_SAVE_SIG | ((l == f.skip_layer - 1) ? F_INJECT_EMB : 0) | ((l == 7) ? F_SDF_DOT : 0);
+    MP_TRY(pack_layer(c, P.step[s++], EPI_SOFTPLUS, flags, l, (l == 0) ? f.imp_b0_eff : f.imp_b[l], f.imp_W[l], in, 0,
+                      0, out, (l == 0) ? E : in, (l == 0) ? (E + 63) / 64 : 4, out * in));
   }
   // sdf-only program: the first 8 steps, no sigma' stash
   tb->sdf_prog = P;
@@ -1016,13 +1007,7 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   // ---- L8 features (operator API: sdf + features) ----
   {
     TcProgram F = P;
-    pack_layer(c, F.step[8], f.imp_W[8], 256, 0, 1, 0, 256, 256, 4, 257 * 256);
-    F.step[8].nk = 4;
-    F.step[8].epi = EPI_FEAT;
-    F.step[8].flags = F_FEAT_OUT;
-    F.step[8].sig = -1;
-    F.step[8].bias = b8feat;
-    F.step[8].ncols = 256;
+    MP_TRY(pack_layer(c, F.step[8], EPI_FEAT, F_FEAT_OUT, -1, b8feat, f.imp_W[8], 256, 0, 1, 256, 256, 4, 257 * 256));
     F.nsteps = 9;
     F.slots_per_tile = c.nslots;
     for (int i = 0; i < 8; ++i) F.step[i].flags &= ~F_SAVE_SIG;
@@ -1046,24 +1031,18 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
     const int o0 = f.ren_out[0];
     fold_mm_kernel<<<dim3(256 / 16, div_up(o0, 16)), dim3(16, 16), 0, st>>>(f.ren_W[0], in0, coff, f.imp_W[8] + 256, 256,
                                                                           f.imp_b[8] + 1, o0, Mfold, kLdM, f.ren_cb);
-    g_launches++;
+    MP_LAUNCH_CHECK();
     MP_REQUIRE(f.ren_extra <= 64, "tc_pack: more than 64 extra colour inputs");
     fill_extra_cols_kernel<<<64, 256, 0, st>>>(f.ren_Wt[0], o0, f.ren_extra, Mfold, kLdM);
-    g_launches++;
+    MP_LAUNCH_CHECK();
   }
   if (bg_chain) {
     // background: folded colour layer 0 (view embedding + h7 -> 128, ReLU) and the rgb head (multiply.py:531)
     const int o0 = f.ren_out[0];
-    pack_layer(c, P.step[s], Mfold, kLdM, 0, 0, 0, o0, kLdM, 5, 256 * kLdM);
-    P.step[s].nk = 5;
-    P.step[s].epi = EPI_RELU;
-    P.step[s].flags = F_EXTRA_IN | F_RGB_OUT;
-    P.step[s].sig = -1;
-    P.step[s].bias = f.ren_b0_fold;
-    P.step[s].ncols = o0;
-    ++s;
+    MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, F_EXTRA_IN | F_RGB_OUT, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, o0, kLdM, 5,
+                      256 * kLdM));
     pad_rows_kernel<<<div_up(3 * 256, 256), 256, 0, st>>>(f.ren_W[1], o0, 3, o0, Wrgb);
-    g_launches++;
+    MP_LAUNCH_CHECK();
     P.brgb = f.ren_b[1];
     P.nsteps = s;
     P.slots_per_tile = c.nslots;
@@ -1075,42 +1054,22 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
     P.step[s - 1].flags |= F_SEED_BWD | F_STASH_FEAT;
     // ---- reverse sweep B7..B1: g_{l-1} = (g_l * sigma'_l) . W_l ----
     for (int l = 7; l >= 1; --l) {
-      int in = f.imp_in[l], out = f.imp_out[l];
+      const int in = f.imp_in[l], out = f.imp_out[l];
       // B[n][k] = W_l[k][n] : n over in (valid in), k over out (valid out)
-      pack_layer(c, P.step[s], f.imp_W[l], in, 1, 0, 0, in, out, 4, out * in);
-      P.step[s].nk = 4;
-      P.step[s].epi = EPI_BWD;
-      P.step[s].flags = (l == f.skip_layer) ? F_SKIP_GRAD : 0;
-      P.step[s].sig = l - 1;
-      P.step[s].bias = nullptr;
-      P.step[s].ncols = in;
-      ++s;
+      MP_TRY(pack_layer(c, P.step[s++], EPI_BWD, (l == f.skip_layer) ? F_SKIP_GRAD : 0, l - 1, nullptr, f.imp_W[l], in, 1,
+                        0, in, out, 4, out * in));
     }
     // ---- B0: d/d embed = (g_0 * sigma'_0) . W0[:, :E] ----
     MP_REQUIRE(f.d_in <= 4 && 1 + 2 * f.multires <= 14,
                "tc_pack: the final-gradient step keeps 1 + 2 * multires <= 14 embedding columns per axis");
-    pack_layer(c, P.step[s], f.imp_W[0], f.imp_in[0], 1, 0, 0, E, 256, 4, 256 * f.imp_in[0], /*perm16=*/f.d_in);
-    P.step[s].nk = 4;
-    P.step[s].epi = EPI_BWD;
-    P.step[s].flags = F_FINAL_GRAD;
-    P.step[s].sig = -1;
-    P.step[s].bias = nullptr;
-    P.step[s].ncols = E;
-    ++s;
+    MP_TRY(pack_layer(c, P.step[s++], EPI_BWD, F_FINAL_GRAD, -1, nullptr, f.imp_W[0], f.imp_in[0], 1, 0, E, 256, 4,
+                      256 * f.imp_in[0], /*perm16=*/f.d_in));
     // ---- colour net: folded layer 0, then layers 1..3 ----
-    for (int l = 0; l < 4; ++l) {
-      if (l == 0)
-        pack_layer(c, P.step[s], Mfold, kLdM, 0, 0, 0, 256, kLdM, 5, 256 * kLdM);
-      else
-        pack_layer(c, P.step[s], f.ren_W[l], 256, 0, 0, 0, 256, 256, 4, 256 * 256);
-      P.step[s].nk = (l == 0) ? 5 : 4;
-      P.step[s].epi = EPI_RELU;
-      P.step[s].flags = ((l == 0) ? F_EXTRA_IN : 0) | ((l == 3) ? F_RGB_OUT : 0);
-      P.step[s].sig = -1;
-      P.step[s].bias = (l == 0) ? f.ren_b0_fold : f.ren_b[l];
-      P.step[s].ncols = 256;
-      ++s;
-    }
+    MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, F_EXTRA_IN, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, 256, kLdM, 5,
+                      256 * kLdM));
+    for (int l = 1; l < 4; ++l)
+      MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, (l == 3) ? F_RGB_OUT : 0, -1, f.ren_b[l], f.ren_W[l], 256, 0, 0, 256,
+                        256, 4, 256 * 256));
     // rgb head [3][256]
     MP_CHECK_CUDA(cudaMemcpyAsync(Wrgb, f.ren_W[4], (size_t)3 * 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     P.brgb = f.ren_b[4];
@@ -1119,19 +1078,12 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
     tb->full_prog = P;
   }
   MP_REQUIRE(c.nslots <= 170, "tc_pack: slot budget exceeded (%d)", c.nslots);
-  return c.rc;
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-int tc_trace_read(unsigned long long* out, int n) {
-  if (n > 4096) n = 4096;
-  MP_CHECK_CUDA(cudaDeviceSynchronize());
-  MP_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_trace, (size_t)n * sizeof(unsigned long long)));
-  return 0;
-}
-
 size_t tc_workspace_bytes(int N) { return (size_t)sm_count() * kScratchPerCta + 4096; }
 
 // optional per-launch timing of the tensor-core kernel (bench.py roofline): CUDA events on the
@@ -1231,18 +1183,11 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
              ws_bytes, (size_t)grid * kScratchPerCta);
   io.scratch = (char*)ws;
   io.scratch_per_cta = kScratchPerCta;
-  {
-    static int knobs = -1;
-    static float rz_scale = 1.f;
-    if (knobs < 0) {
-      const char* er = getenv("MP_TC_RZ_SCALE");      // experiment knob: multiplies kRzPerMma (0 switches it off)
-      rz_scale = er ? (float)atof(er) : 1.f;
-      const char* ek = getenv("MP_TC_KNOBS");
-      knobs = ek ? atoi(ek) : 0;
-    }
-    io.knobs = knobs;
-    io.rz = kRzPerMma * rz_scale;
-  }
+  static const float rz_scale = [] {
+    const char* er = getenv("MP_TC_RZ_SCALE");      // experiment knob: multiplies kRzPerMma (0 switches it off)
+    return er ? (float)atof(er) : 1.f;
+  }();
+  io.rz = kRzPerMma * rz_scale;
   {
     // the > 48 KB dynamic shared memory opt-in is per device
     static std::mutex attr_mu;

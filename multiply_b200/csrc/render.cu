@@ -8,58 +8,11 @@
 namespace mp {
 
 std::atomic<int> g_engine{1};
-extern std::atomic<int> g_precision;      // mlp_tc.cu
 
-// mlp_tc.cu
-int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                  const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                  float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int tc_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-          size_t ws_bytes, cudaStream_t st);
-size_t tc_workspace_bytes(int N);
-int tc_trace_read(unsigned long long* out, int n);
-int prof_enable(int on);
-int prof_read(double* ms, long long* launches, double* points, int reset);
-
-// sampler.cu / composite.cu / background.cu
-int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field, const float* dirs,
-                const float* cam, int R, float* z_final, float* z_bg, int* trips_out, void* ws, size_t ws_bytes,
-                cudaStream_t st, const int* R_dev = nullptr, const mp_sampler_rng_t* rng = nullptr, float* z_eik = nullptr);
-size_t sampler_ws_bytes(const mp_sampler_cfg_t& c, int R);
-struct CompositePersons {
-  int P;
-  int n_rows[MP_MAX_PERSONS];
-  const int* row_of_ray[MP_MAX_PERSONS];
-  const float* z[MP_MAX_PERSONS];
-  const float* sdf[MP_MAX_PERSONS];
-  const float* rgb[MP_MAX_PERSONS];
-  const float* nrm[MP_MAX_PERSONS];
-};
-int launch_composite(const CompositePersons& cp, int R, int n, float beta, float* fg_rgb, float* normal, float* acc,
-                     float* acc_person, float* bg_T, cudaStream_t st);
-int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cudaStream_t st, const int* n_dev = nullptr);
-int launch_final_compose(const float* fg, const float* bgT, const float* bg, int R, float* rgb, float* fg_out,
-                         cudaStream_t st);
-int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
-                      void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand = nullptr,
-                      float* tap_sdf = nullptr, float* tap_rgb = nullptr);
-size_t bg_ws_bytes(int R);
-// mesh.cu
-struct Mesh;
-const Mesh& mesh_of(const mp_mesh_t* h);
-int launch_surface_flags(const Mesh& m, const float* xc, const int* slot, const int* count_dev, int cap, int n,
-                         float thr, uint8_t* off, uint8_t* in, cudaStream_t st);
-int launch_merge_flags(const int64_t* idx, int rows, const int* rows_dev, const uint8_t* off_p, const uint8_t* in_p,
-                       uint8_t* off, uint8_t* in, cudaStream_t st);
-
-static size_t engine_ws_bytes(int N) {
+size_t field_ws_bytes(int N) {
   size_t a = simt_workspace_bytes(N), b = tc_workspace_bytes(N);
   return a > b ? a : b;
 }
-size_t field_sdf_ws_bytes(int cap) { return engine_ws_bytes(cap); }
-size_t field_bg_ws_bytes(int N) { return engine_ws_bytes(N); }
 
 int field_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
                    float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -220,7 +173,7 @@ static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
     b.off = flags ? a.take<uint8_t>(Rp) : nullptr;
     b.in = flags ? a.take<uint8_t>(Rp) : nullptr;
     sub = max(sub, sampler_ws_bytes(c, Rp));
-    sub = max(sub, engine_ws_bytes(Rp * n));
+    sub = max(sub, field_ws_bytes(Rp * n));
   }
   w.sub_bytes = sub;
   for (int i = 0; i <= sc.P; ++i) w.sub[i] = a.take<char>(sub);     // [P] = background branch
@@ -251,17 +204,12 @@ int mp_set_streams(int on) {
   return 0;
 }
 
-int mp_tc_trace_read(unsigned long long* out, int n) {
-  MP_REQUIRE(out && n > 0, "mp_tc_trace_read: null argument");
-  return mp::tc_trace_read(out, n);
-}
-
 int mp_profile_read(double* ms_host, long long* launches_host, double* points_host, int reset) {
   MP_REQUIRE(ms_host && launches_host && points_host, "mp_profile_read: null argument");
   return mp::prof_read(ms_host, launches_host, points_host, reset);
 }
 
-size_t mp_mlp_workspace_bytes(int N) { return mp::engine_ws_bytes(N) + (size_t)N * (9 + 1) * sizeof(float) + 4096; }
+size_t mp_mlp_workspace_bytes(int N) { return mp::field_ws_bytes(N) + (size_t)N * (9 + 1) * sizeof(float) + 4096; }
 
 int mp_implicit_forward(mp_net_t* f, const float* x, int N, float* sdf, float* feat, void* workspace,
                         size_t workspace_bytes, void* stream) {
@@ -301,7 +249,7 @@ int mp_bg_nets_forward(mp_net_t* bg_field, const float* pts, const float* view_d
 size_t mp_sdf_grid_workspace_bytes(int res) {
   long long n = (long long)(res + 1) * (res + 1) * (res + 1);
   int chunk = (int)(n < (1 << 20) ? n : (1 << 20));
-  return mp::engine_ws_bytes(chunk) + (size_t)chunk * 3 * sizeof(float) + 4096;
+  return mp::field_ws_bytes(chunk) + (size_t)chunk * 3 * sizeof(float) + 4096;
 }
 
 int mp_sdf_grid(mp_net_t* field, const float* center_host, float extent, float pad, int res, float* values,
@@ -314,7 +262,7 @@ int mp_sdf_grid(mp_net_t* field, const float* center_host, float extent, float p
   const int chunk = (int)(n < (1 << 20) ? n : (1 << 20));
   mp::Arena a(workspace, workspace_bytes);
   float* pts = a.take<float>((size_t)chunk * 3);
-  const size_t mb = mp::engine_ws_bytes(chunk);
+  const size_t mb = mp::field_ws_bytes(chunk);
   void* mws = a.take<char>(mb);
   MP_REQUIRE(a.ok, "mp_sdf_grid: workspace too small (%zu needed)", a.off);
   for (long long s0 = 0; s0 < n; s0 += chunk) {
@@ -334,7 +282,7 @@ int mp_sdf_with_deformer(mp_body_t* body, mp_net_t* field, const float* x, int N
   cudaStream_t st = (cudaStream_t)stream;
   mp::Arena a(workspace, workspace_bytes);
   uint8_t* outl = a.take<uint8_t>(N);
-  size_t mb = mp::engine_ws_bytes(N);
+  size_t mb = mp::field_ws_bytes(N);
   void* mws = a.take<char>(mb);
   MP_REQUIRE(a.ok, "mp_sdf_with_deformer: workspace too small (%zu needed)", a.off);
   MP_TRY(mp_deform_inverse(body, x, N, x_c, outl, 1, stream));

@@ -16,15 +16,10 @@
 
 namespace mp {
 
-int field_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                   float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);   // render.cu (engine dispatch)
-size_t field_sdf_ws_bytes(int cap);
-
 struct SamplerState {
   int not_converge[8];   // per trip: any ray with beta > beta0
   int active[8];         // per trip: loop still running at the start of trip t (active[0] = 1)
   int count[8];          // per trip: compact work-list length
-  int bad_sphere;        // some ray missed the bounding sphere (rend_util.py:140-142)
   int final_trip;        // trip whose resample produced the final samples
 };
 
@@ -59,7 +54,6 @@ __global__ void tables_kernel(SamplerTables t, int E, int S, int X, int max_iter
       st->active[k] = (k == 0) ? 1 : 0;
       st->count[k] = 0;
     }
-    st->bad_sphere = 0;
     st->final_trip = -1;
   }
 }
@@ -77,11 +71,10 @@ __global__ void sampler_init_kernel(const float* __restrict__ dirs, const float*
   if (ray >= R) return;
   const float* o = cam + 3 * ray;
   const float* d = dirs + 3 * ray;
-  // rend_util.get_sphere_intersections, :131-147
+  // rend_util.get_sphere_intersections, :131-147 (a miss is reported by mp_render_rays' sphere_status_kernel)
   float dot = d[0] * o[0] + d[1] * o[1] + d[2] * o[2];
   float nrm = sqrtf(o[0] * o[0] + o[1] * o[1] + o[2] * o[2]);
   float under = dot * dot - (nrm * nrm - r * r);
-  if (lane == 0 && !(under > 0.f)) atomicOr(&st->bad_sphere, 1);
   float far = fmaxf(sqrtf(under) * 1.f - dot, 0.f);
   if (lane == 0) far_out[ray] = far;
   float* zr = z + (size_t)ray * zcap;
@@ -204,23 +197,6 @@ __global__ void sampler_beta_kernel(const float* __restrict__ z, const float* __
   }
 }
 
-__device__ __forceinline__ int upper_bound_f(const float* a, int n, float v) {   // first i with a[i] > v
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    int mid = (lo + hi) >> 1;
-    if (a[mid] > v) hi = mid; else lo = mid + 1;
-  }
-  return lo;
-}
-__device__ __forceinline__ int lower_bound_f(const float* a, int n, float v) {   // first i with a[i] >= v
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    int mid = (lo + hi) >> 1;
-    if (a[mid] >= v) hi = mid; else lo = mid + 1;
-  }
-  return lo;
-}
-
 // Resampling of one trip: weights / error-bound pdf -> cdf -> inverse-CDF samples -> merge, or the
 // final sample set     ray_sampler.py:124-220
 __global__ void sampler_resample_kernel(const float* __restrict__ z, const float* __restrict__ sdf, int zcap, int M,
@@ -320,7 +296,7 @@ __global__ void sampler_resample_kernel(const float* __restrict__ z, const float
   const float* u_tab = cont ? tab.u_E : (rnd ? rng.u_final + (size_t)ray * S : tab.u_S);
   for (int j = lane; j < N; j += 32) {
     float u = u_tab[j];
-    int inds = upper_bound_f(sc, M, u);          // searchsorted(right=True)
+    int inds = upper_bound(sc, M, u);          // searchsorted(right=True)
     int below = max(0, inds - 1);
     int above = min(M - 1, inds);
     float c0 = sc[below], c1 = sc[above];
@@ -379,12 +355,12 @@ __global__ void sampler_resample_kernel(const float* __restrict__ z, const float
     float* so = sdf_out + (size_t)ray * zcap;
     int* pn = pos_new + (size_t)ray * E;
     for (int i = lane; i < M; i += 32) {
-      int p = i + lower_bound_f(sn, N, sz[i]);
+      int p = i + lower_bound(sn, N, sz[i]);
       zo[p] = sz[i];
       so[p] = ss[i];
     }
     for (int j = lane; j < N; j += 32) {
-      int p = j + upper_bound_f(sz, M, sn[j]);
+      int p = j + upper_bound(sz, M, sn[j]);
       zo[p] = sn[j];
       pn[j] = p;
     }
@@ -397,12 +373,12 @@ __global__ void sampler_resample_kernel(const float* __restrict__ z, const float
     int NB = X + 2;
     for (int k = lane; k < NB; k += 32) sp[k] = (k == 0) ? near : ((k == NB - 1) ? farv : sz[idx[k - 1]]);
     __syncwarp();
-    for (int j = lane; j < N; j += 32) zf[j + lower_bound_f(sp, NB, sn[j])] = sn[j];
-    for (int k = lane; k < NB; k += 32) zf[k + upper_bound_f(sn, N, sp[k])] = sp[k];
+    for (int j = lane; j < N; j += 32) zf[j + lower_bound(sp, NB, sn[j])] = sn[j];
+    for (int k = lane; k < NB; k += 32) zf[k + upper_bound(sn, N, sp[k])] = sp[k];
   }
 }
 
-__global__ void trips_kernel(const SamplerState* st, int max_iters, int* trips_out) {
+__global__ void trips_kernel(const SamplerState* st, int* trips_out) {
   *trips_out = st->final_trip + 1;
 }
 
@@ -451,7 +427,7 @@ static bool sampler_carve(Arena& a, const mp_sampler_cfg_t& c, int R, SamplerWs&
   w.tab.u_S = a.take<float>(S);
   w.tab.extra_idx = a.take<int>((size_t)c.max_total_iters * (X > 0 ? X : 1));
   w.tab.z_bg = a.take<float>(32);
-  w.mlp_ws_bytes = field_sdf_ws_bytes(R * E);
+  w.mlp_ws_bytes = field_ws_bytes(R * E);
   w.mlp_ws = a.take<char>(w.mlp_ws_bytes);
   return a.ok;
 }
@@ -521,7 +497,7 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
     float* ts = sc; sc = sn; sn = ts;
   }
   if (trips_out) {
-    trips_kernel<<<1, 1, 0, st>>>(w.st, c.max_total_iters, trips_out);
+    trips_kernel<<<1, 1, 0, st>>>(w.st, trips_out);
     MP_LAUNCH_CHECK();
   }
   if (z_bg) {

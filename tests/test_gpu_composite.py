@@ -1,8 +1,8 @@
 """GPU: the multi-person compositor (csrc/composite.cu: mp_composite, mp_final_compose) against a float64 restatement of
 multiply.py:427-480 at person-count, sample-count, block and tie edges.
 
-The kernel merges the P per-person lists of a ray by rank (binary searches: count_le for earlier persons, count_lt for
-later ones, so equal t_end values keep (person, sample) order), scans sigma * delta in chunks per lane and takes bg_T
+The kernel merges the P per-person lists of a ray by rank (binary searches: upper_bound for earlier persons, lower_bound
+for later ones, so equal t_end values keep (person, sample) order), scans sigma * delta in chunks per lane and takes bg_T
 from the exclusive prefix of the ray's last merged sample.  Whole renders only ever tie on the shared `far` where
 sigma ~ 0, so the tie order and the prefix there are checked here on synthetic inputs where they matter: identical z
 rows of two persons on one ray, zero-length intervals inside one list, and the shared far with a negative sdf on the
