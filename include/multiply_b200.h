@@ -331,7 +331,9 @@ int mp_final_compose_backward(const float* bg_T /*[R]*/, const float* bg_rgb_or_
                               float* d_fg_rgb /*[R,3]*/, float* d_bg_T /*[R]*/, float* d_bg_rgb_or_null /*[R,3]*/,
                               void* stream);
 
-/* background: inverse-sphere samples -> depth2pts_outside (multiply.py:698-726) -> bg nets -> bg_volume_rendering */
+/* background: inverse-sphere samples -> depth2pts_outside (multiply.py:698-726) -> bg nets -> bg_volume_rendering
+ * A ray through the sphere's centre (cross(o, p_sphere) = 0) gets the limit p_sphere / |p_sphere| where the reference
+ * returns NaN. */
 size_t mp_background_workspace_bytes(int R);
 int mp_background(mp_net_t* bg_field, const float* ray_dirs, const float* cam_loc, int R, float bound_r,
                   float* bg_rgb /*[R,3]*/, void* workspace, size_t workspace_bytes, void* stream);

@@ -47,7 +47,9 @@ __global__ void bg_points_kernel(const float* __restrict__ dirs, const float* __
   float pmn = sqrtf(pm[0] * pm[0] + pm[1] * pm[1] + pm[2] * pm[2]);
   float ax[3] = {o[1] * ps[2] - o[2] * ps[1], o[2] * ps[0] - o[0] * ps[2], o[0] * ps[1] - o[1] * ps[0]};
   float an = sqrtf(ax[0] * ax[0] + ax[1] * ax[1] + ax[2] * ax[2]);
-  for (int k = 0; k < 3; ++k) ax[k] = ax[k] / an;
+  // a ray through the sphere's centre has o x p_sphere = 0 and a rotation angle of exactly 0: a zero axis gives the
+  // limit p_sphere / |p_sphere| (the reference divides 0 by 0 here and returns NaN)
+  for (int k = 0; k < 3; ++k) ax[k] = (an > 0.f) ? ax[k] / an : 0.f;
   float phi = asinf(pmn / bound);
   float theta = asinf(pmn * depth);
   float ang = phi - theta;
