@@ -262,7 +262,8 @@ typedef struct {
   const int* eik_idx;      /* [T_max, R] int32            row T: torch.randint(S+X+2, (R,)) */
   const float* t_rand_bg;  /* [T_max, R, 32] or NULL      row T: torch.rand of the inverse-sphere UniformSampler */
 } mp_sampler_rng_t;
-/* outputs as mp_sample_rays plus z_eik [R] (z_samples_eik, may be NULL) */
+/* outputs as mp_sample_rays plus z_eik [R] (z_samples_eik, may be NULL).  Requires N_samples_extra <= N_samples_eval:
+ * after one trip randperm(E)[:X] has only min(X, E) entries, so a larger X is rejected with an error. */
 int mp_sample_rays_train(const mp_sampler_cfg_t* cfg, mp_body_t* body, mp_net_t* field,
                          const float* ray_dirs, const float* cam_loc, int R, const mp_sampler_rng_t* rng,
                          float* z_vals, float* z_bg, float* z_eik, int* trips_out,

@@ -444,6 +444,9 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
   MP_REQUIRE(E >= 2 && S >= 1 && X >= 0 && c.max_total_iters >= 1 && c.max_total_iters <= 8,
              "sampler: unsupported configuration (E=%d S=%d X=%d iters=%d)", E, S, X, c.max_total_iters);
   MP_REQUIRE(S <= E, "sampler: N_samples (%d) must not exceed N_samples_eval (%d)", S, E);
+  // training mode takes the extras from randperm(M)[:X] (ray_sampler.py:202), which has only min(X, M) entries when the
+  // loop ends after one trip (M = E); the row of S+X+2 samples would be padded with whatever the permutation row holds
+  MP_REQUIRE(!training || X <= E, "sampler: training mode needs N_samples_extra (%d) <= N_samples_eval (%d)", X, E);
   if (R <= 0) return 0;
   Arena a(ws, ws_bytes);
   SamplerWs w;

@@ -412,7 +412,7 @@ def get_sphere_intersections(cam_loc, ray_directions, r=1.0):
 def _error_bound(beta, sdf, z_vals, dists, d_star):
     """ErrorBoundSampler.get_error_bound, ray_sampler.py:222-230."""
     density = laplace_density(sdf.reshape(z_vals.shape), beta)
-    shifted = torch.cat([torch.zeros(dists.shape[0], 1), dists * density[:, :-1]], dim=-1)
+    shifted = torch.cat([torch.zeros(dists.shape[0], 1, dtype=dists.dtype), dists * density[:, :-1]], dim=-1)
     integral = torch.cumsum(shifted, dim=-1)
     eps_sec = torch.exp(-d_star / beta) * (dists ** 2.) / (4 * beta ** 2)
     err_int = torch.cumsum(eps_sec, dim=-1)
@@ -420,7 +420,46 @@ def _error_bound(beta, sdf, z_vals, dists, d_star):
     return bound.max(-1)[0]
 
 
-def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=None, stats=None, rng=None):
+def _inverse_cdf_step(z_vals, sdf, d_star, beta, cont, u, add_tiny):
+    """One trip's resampling after the line search, ray_sampler.py:124-186: the error-bound pdf (cont, :141-155) or the
+    weights' pdf (final set, :157-165), the cdf and the inverse CDF at abscissae u."""
+    dtype = z_vals.dtype
+    dists = z_vals[:, 1:] - z_vals[:, :-1]
+    density = laplace_density(sdf.reshape(z_vals.shape), beta.unsqueeze(-1))
+    dists = torch.cat([dists, torch.tensor([1e10], dtype=dtype).unsqueeze(0).repeat(dists.shape[0], 1)], -1)
+    free_energy = dists * density
+    shifted = torch.cat([torch.zeros(dists.shape[0], 1, dtype=dtype), free_energy[:, :-1]], dim=-1)
+    alpha = 1 - torch.exp(-free_energy)
+    transmittance = torch.exp(-torch.cumsum(shifted, dim=-1))
+    weights = alpha * transmittance
+    if cont:
+        eps_sec = torch.exp(-d_star / beta.unsqueeze(-1)) * (dists[:, :-1] ** 2.) / (4 * beta.unsqueeze(-1) ** 2)
+        err_int = torch.cumsum(eps_sec, dim=-1)
+        bound_opacity = (torch.clamp(torch.exp(err_int), max=1.e6) - 1.0) * transmittance[:, :-1]
+        pdf = bound_opacity + add_tiny
+    else:
+        pdf = weights[..., :-1]
+        pdf = pdf + 1e-5
+    pdf = pdf / torch.sum(pdf, -1, keepdim=True)
+    cdf = torch.cumsum(pdf, -1)
+    cdf = torch.cat([torch.zeros_like(cdf[..., :1]), cdf], -1)
+    bins = z_vals
+    inds = torch.searchsorted(cdf, u, right=True)
+    below = torch.max(torch.zeros_like(inds - 1), inds - 1)
+    above = torch.min((cdf.shape[-1] - 1) * torch.ones_like(inds), inds)
+    inds_g = torch.stack([below, above], -1)
+    matched = [inds_g.shape[0], inds_g.shape[1], cdf.shape[-1]]
+    cdf_g = torch.gather(cdf.unsqueeze(1).expand(matched), 2, inds_g)
+    bins_g = torch.gather(bins.unsqueeze(1).expand(matched), 2, inds_g)
+    denom_raw = cdf_g[..., 1] - cdf_g[..., 0]
+    denom = torch.where(denom_raw < 1e-5, torch.ones_like(denom_raw), denom_raw)
+    t = (u - cdf_g[..., 0]) / denom
+    samples = bins_g[..., 0] + t * (bins_g[..., 1] - bins_g[..., 0])
+    return dict(pdf=pdf, cdf=cdf, below=below, above=above, denom_raw=denom_raw, denom=denom, samples=samples)
+
+
+def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=None, stats=None, rng=None,
+                           dtype=torch.float32, ray_sdf_fn=None, trace=None):
     """ErrorBoundSampler.get_z_vals (inverse_sphere_bg=True), ray_sampler.py:66-220.
 
     Eval mode (``rng is None``): returns (z_vals [R,S+X+2], z_bg [R,32]).
@@ -432,7 +471,29 @@ def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=No
       eik_idx [R]    torch.randint(S+X+2, (R,)) for z_samples_eik         :212-213
       t_rand_bg [R,32]  jitter of the inverse-sphere samples (the UniformSampler sees model.training too)   :216
     — the SDF callback does not clamp outliers (multiply.py:142 is eval-only) and the return is
-    (z_vals, z_bg, z_samples_eik [R,1]).  ``stats`` (dict) receives 'trips'."""
+    (z_vals, z_bg, z_samples_eik [R,1]).  ``stats`` (dict) receives 'trips'.
+
+    ``dtype``: the floating type of every tensor the sampler creates (the reference's is float32; float64 gives a
+    high-precision restatement of the same algorithm).  ``ray_sdf_fn(cam_loc [R,3], z [R,N], ray_dirs [R,3]) -> sdf
+    [R*N,1]`` replaces ``sdf_fn`` when the caller builds the sample points itself.  ``trace`` (dict) receives
+    ``trips``, one dict per trip with the state after its line search and the margin of every discrete decision:
+      z, sdf [R,M], beta [R]      the sorted list, its SDF and the beta of the line search
+      err0 [R]                    the error bound at beta0 (get_error_bound, :222-230)
+      err_margin [R]              min over the line search's tests `err <= eps` of |err - eps| / eps
+      flag, flag_margin           the batch test beta.max() > beta0 (:137), and |max(err0) - eps| / eps: how far the
+                                  slowest ray's error is from eps
+      final                       whether this trip drew the final set
+      cdf [R,M]; u, below, above, denom_raw, denom, samples [R,N]   the inverse CDF (:166-186)
+      u_margin [R,N]              distance of each abscissa to the nearest cdf entry that can decide it: cdf[0] = 0 is
+                                  exact on every side and is left out; u = 1 gets inf, its bin is decided by how the
+                                  cdf's tail rounds against 1 (see cdf_last, pdf_last)
+      denom_margin [R,N]          |cdf[above] - cdf[below] - 1e-5|, the `denom < 1e-5` test
+      cdf_last [R]                cdf[M-1] - 1: at u = 1 this decides whether the sample is z[M-1] (cdf[M-1] <= 1) or
+                                  lies inside the last bin
+      pdf_last [R]                the last bin's normalised pdf: below 1e-5 the sample in the last bin is b0 + (1 -
+                                  cdf[M-2]) (b1 - b0), a whole interval from z[M-1]
+      merge_margin [R,N]          distance of each new sample to the nearest list value it is merged with (0 = tie)
+      order [R,M+N]               the sort index of cat([z, samples]) (non-final trips)."""
     S, E, X = cfg["N_samples"], cfg["N_samples_eval"], cfg["N_samples_extra"]
     eps, beta_iters, max_iters = cfg["eps"], cfg["beta_iters"], cfg["max_total_iters"]
     add_tiny, bound_r = cfg["add_tiny"], cfg["scene_bounding_sphere"]
@@ -440,32 +501,36 @@ def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=No
     training = rng is not None
     if sdf_fn is None:
         sdf_fn = lambda pts: sdf_func_with_smpl_deformer(pts, person, cfg, training=training)[0]
+    if ray_sdf_fn is None:
+        ray_sdf_fn = lambda o, z, d: sdf_fn((o.unsqueeze(1) + z.unsqueeze(2) * d.unsqueeze(1)).reshape(-1, 3))
+    if trace is not None:
+        trace["trips"] = []
+    ray_dirs, cam_loc = ray_dirs.to(dtype), cam_loc.to(dtype)
     R = ray_dirs.shape[0]
-    beta0 = get_beta(beta_param)
+    beta0 = get_beta(beta_param).to(dtype)
 
     # UniformSampler.get_z_vals, ray_sampler.py:21-42 (take_sphere_intersection=True, eval)
     si = get_sphere_intersections(cam_loc, ray_dirs, r=bound_r)
-    near = near_v * torch.ones(R, 1)
+    near = near_v * torch.ones(R, 1, dtype=dtype)
     far = si[:, 1:]
-    t_vals = torch.linspace(0., 1., steps=E)
+    t_vals = torch.linspace(0., 1., steps=E, dtype=dtype)
     z_vals = near * (1. - t_vals) + far * t_vals
     if training:      # ray_sampler.py:32-40
         mids = .5 * (z_vals[..., 1:] + z_vals[..., :-1])
         upper = torch.cat([mids, z_vals[..., -1:]], -1)
         lower = torch.cat([z_vals[..., :1], mids], -1)
-        z_vals = lower + (upper - lower) * rng["t_rand"]
+        z_vals = lower + (upper - lower) * rng["t_rand"].to(dtype)
     samples, samples_idx = z_vals, None
 
     dists = z_vals[:, 1:] - z_vals[:, :-1]
-    bound = (1.0 / (4.0 * torch.log(torch.tensor(eps + 1.0)))) * (dists ** 2.).sum(-1)
+    bound = (1.0 / (4.0 * torch.log(torch.tensor(eps + 1.0, dtype=dtype)))) * (dists ** 2.).sum(-1)
     beta = torch.sqrt(bound)
 
     total_iters, not_converge = 0, True
     sdf = None
     while not_converge and total_iters < max_iters:
-        points = cam_loc.unsqueeze(1) + samples.unsqueeze(2) * ray_dirs.unsqueeze(1)
         with torch.no_grad():
-            samples_sdf = sdf_fn(points.reshape(-1, 3))
+            samples_sdf = ray_sdf_fn(cam_loc, samples, ray_dirs).to(dtype)
         if samples_idx is not None:
             sdf_merge = torch.cat([sdf.reshape(-1, z_vals.shape[1] - samples.shape[1]),
                                    samples_sdf.reshape(-1, samples.shape[1])], -1)
@@ -478,7 +543,7 @@ def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=No
         a, b, c = dists, d[:, :-1].abs(), d[:, 1:].abs()
         first_cond = a.pow(2) + b.pow(2) <= c.pow(2)
         second_cond = a.pow(2) + c.pow(2) <= b.pow(2)
-        d_star = torch.zeros(z_vals.shape[0], z_vals.shape[1] - 1)
+        d_star = torch.zeros(z_vals.shape[0], z_vals.shape[1] - 1, dtype=dtype)
         d_star[first_cond] = b[first_cond]
         d_star[second_cond] = c[second_cond]
         s = (a + b + c) / 2.0
@@ -488,69 +553,58 @@ def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=No
         d_star = (d[:, 1:].sign() * d[:, :-1].sign() == 1) * d_star
 
         curr_error = _error_bound(beta0, sdf, z_vals, dists, d_star)
+        if trace is not None:
+            # the test at beta0 picks beta0 or the bisection result, which lies between beta0 and the start beta
+            tr = dict(z=z_vals.clone(), sdf=d.clone(), d_star=d_star, err0=curr_error.clone(), beta_init=beta.clone(),
+                      err_steps=[(curr_error - eps) / eps], brackets=[(beta - beta0).abs()])
         beta[curr_error <= eps] = beta0
         beta_min, beta_max = beta0.unsqueeze(0).repeat(z_vals.shape[0]), beta
         for _ in range(beta_iters):
             beta_mid = (beta_min + beta_max) / 2.
             curr_error = _error_bound(beta_mid.unsqueeze(-1), sdf, z_vals, dists, d_star)
+            if trace is not None:
+                tr["err_steps"].append((curr_error - eps) / eps)
+                tr["brackets"].append((beta_max - beta_min).abs())
             beta_max[curr_error <= eps] = beta_mid[curr_error <= eps]
             beta_min[curr_error > eps] = beta_mid[curr_error > eps]
         beta = beta_max
 
-        density = laplace_density(sdf.reshape(z_vals.shape), beta.unsqueeze(-1))
-        dists = torch.cat([dists, torch.tensor([1e10]).unsqueeze(0).repeat(dists.shape[0], 1)], -1)
-        free_energy = dists * density
-        shifted = torch.cat([torch.zeros(dists.shape[0], 1), free_energy[:, :-1]], dim=-1)
-        alpha = 1 - torch.exp(-free_energy)
-        transmittance = torch.exp(-torch.cumsum(shifted, dim=-1))
-        weights = alpha * transmittance
-
         total_iters += 1
         not_converge = bool(beta.max() > beta0)
-
-        if not_converge and total_iters < max_iters:
-            N = E
-            bins = z_vals
-            eps_sec = torch.exp(-d_star / beta.unsqueeze(-1)) * (dists[:, :-1] ** 2.) / (4 * beta.unsqueeze(-1) ** 2)
-            err_int = torch.cumsum(eps_sec, dim=-1)
-            bound_opacity = (torch.clamp(torch.exp(err_int), max=1.e6) - 1.0) * transmittance[:, :-1]
-            pdf = bound_opacity + add_tiny
-            pdf = pdf / torch.sum(pdf, -1, keepdim=True)
-            cdf = torch.cumsum(pdf, -1)
-            cdf = torch.cat([torch.zeros_like(cdf[..., :1]), cdf], -1)
+        cont = not_converge and total_iters < max_iters
+        if cont or not training:      # ray_sampler.py:166-170
+            u = torch.linspace(0., 1., steps=E if cont else S, dtype=dtype).unsqueeze(0).repeat(R, 1).contiguous()
         else:
-            N = S
-            bins = z_vals
-            pdf = weights[..., :-1]
-            pdf = pdf + 1e-5
-            pdf = pdf / torch.sum(pdf, -1, keepdim=True)
-            cdf = torch.cumsum(pdf, -1)
-            cdf = torch.cat([torch.zeros_like(cdf[..., :1]), cdf], -1)
+            u = rng["u_final"].to(dtype).contiguous()
+        st_ = _inverse_cdf_step(z_vals, sdf, d_star, beta, cont, u, add_tiny)
+        cdf, pdf, below, above, denom_raw, denom, samples = (st_[k] for k in (
+            "cdf", "pdf", "below", "above", "denom_raw", "denom", "samples"))
 
-        if (not_converge and total_iters < max_iters) or not training:      # ray_sampler.py:166-170
-            u = torch.linspace(0., 1., steps=N).unsqueeze(0).repeat(cdf.shape[0], 1).contiguous()
-        else:
-            u = rng["u_final"].contiguous()
-        inds = torch.searchsorted(cdf, u, right=True)
-        below = torch.max(torch.zeros_like(inds - 1), inds - 1)
-        above = torch.min((cdf.shape[-1] - 1) * torch.ones_like(inds), inds)
-        inds_g = torch.stack([below, above], -1)
-        matched = [inds_g.shape[0], inds_g.shape[1], cdf.shape[-1]]
-        cdf_g = torch.gather(cdf.unsqueeze(1).expand(matched), 2, inds_g)
-        bins_g = torch.gather(bins.unsqueeze(1).expand(matched), 2, inds_g)
-        denom = cdf_g[..., 1] - cdf_g[..., 0]
-        denom = torch.where(denom < 1e-5, torch.ones_like(denom), denom)
-        t = (u - cdf_g[..., 0]) / denom
-        samples = bins_g[..., 0] + t * (bins_g[..., 1] - bins_g[..., 0])
+        if trace is not None:
+            gap = (u.unsqueeze(-1) - cdf[:, 1:].unsqueeze(1)).abs()
+            gap = torch.where((u == 1).unsqueeze(-1), torch.full_like(gap, math.inf), gap)
+            # a ray raises the batch flag (beta.max() > beta0 after the line search) iff err0 > eps and its start beta
+            # exceeds beta0; the flag's margin is that of its most robust raiser, or of its least robust non-raiser
+            raise_m = torch.minimum((tr["err0"] - eps) / eps, (tr["beta_init"] - beta0) / beta0)
+            tr.update(beta=beta.clone(), flag=not_converge, final=not cont,
+                      flag_margin=float(raise_m.max() if not_converge else -raise_m.max()),
+                      err_steps=torch.stack(tr["err_steps"], 1), brackets=torch.stack(tr["brackets"], 1),
+                      cdf=cdf, u=u, below=below, above=above, denom_raw=denom_raw, denom=denom, samples=samples,
+                      u_margin=gap.min(-1)[0], denom_margin=(denom_raw - 1e-5).abs(), cdf_last=cdf[:, -1] - 1,
+                      pdf_last=pdf[:, -1],
+                      merge_margin=(samples.unsqueeze(-1) - z_vals.unsqueeze(1)).abs().min(-1)[0])
+            trace["trips"].append(tr)
 
-        if not_converge and total_iters < max_iters:
+        if cont:
             z_vals, samples_idx = torch.sort(torch.cat([z_vals, samples], -1), -1)
+            if trace is not None:
+                tr["order"] = samples_idx
 
     if stats is not None:
         stats["trips"] = total_iters
         stats["beta"] = beta.clone()
     z_samples = samples
-    near = near_v * torch.ones(R, 1)
+    near = near_v * torch.ones(R, 1, dtype=dtype)
     far = get_sphere_intersections(cam_loc, ray_dirs, r=bound_r)[:, 1:]
     if X > 0:
         if training:
@@ -564,14 +618,14 @@ def error_bound_get_z_vals(ray_dirs, cam_loc, person, cfg, beta_param, sdf_fn=No
     z_out, _ = torch.sort(torch.cat([z_samples, z_extra], -1), -1)
 
     # inverse-sphere background samples: UniformSampler(1.0, 0.0, 32, False, far=1.0), ray_sampler.py:215-218
-    tb = torch.linspace(0., 1., steps=32)
-    z_bg = torch.zeros(R, 1) * (1. - tb) + torch.ones(R, 1) * tb
+    tb = torch.linspace(0., 1., steps=32, dtype=dtype)
+    z_bg = torch.zeros(R, 1, dtype=dtype) * (1. - tb) + torch.ones(R, 1, dtype=dtype) * tb
     if training:
         z_eik = torch.gather(z_out, 1, rng["eik_idx"].long().unsqueeze(-1))      # ray_sampler.py:212-213
         mids = .5 * (z_bg[..., 1:] + z_bg[..., :-1])
         upper = torch.cat([mids, z_bg[..., -1:]], -1)
         lower = torch.cat([z_bg[..., :1], mids], -1)
-        z_bg = lower + (upper - lower) * rng["t_rand_bg"]
+        z_bg = lower + (upper - lower) * rng["t_rand_bg"].to(dtype)
         return z_out, z_bg * (1. / bound_r), z_eik
     return z_out, z_bg * (1. / bound_r)
 
