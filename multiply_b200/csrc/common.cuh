@@ -145,6 +145,11 @@ struct Field {
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
 static inline int clamp_wpc(size_t v) { return v < 1 ? 1 : (v > 8 ? 8 : (int)v); }
 
+// The sampler's beta (density.py:27-29; one fp32 add, the same with or without -fmad=false) and samples per ray
+// (multiply.py:290-292).
+static inline float sampler_beta(const mp_sampler_cfg_t& c) { return fabsf(c.beta_param) + c.beta_min; }
+static inline int samples_per_ray(const mp_sampler_cfg_t& c) { return c.N_samples + c.N_samples_extra + 1; }
+
 // ---- cross-file launchers: every internal function or type one .cu file uses from another --------
 
 // fp32 SIMT engine (mlp_simt.cu)
@@ -211,6 +216,14 @@ struct CompositePersons {
   const float* rgb[MP_MAX_PERSONS];        // [R_p, n, 3]
   const float* nrm[MP_MAX_PERSONS];        // [R_p, n, 3]
 };
+static inline void set_person(CompositePersons& cp, int p, const mp_person_samples_t& s, const int* row_of_ray) {
+  cp.n_rows[p] = s.n_rows;
+  cp.row_of_ray[p] = row_of_ray;
+  cp.z[p] = s.z_vals;
+  cp.sdf[p] = s.sdf;
+  cp.rgb[p] = s.rgb;
+  cp.nrm[p] = s.normal;
+}
 int launch_composite(const CompositePersons& cp, int R, int n, float beta, float* fg_rgb, float* normal, float* acc,
                      float* acc_person, float* bg_T, cudaStream_t st);
 int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cudaStream_t st,

@@ -23,6 +23,16 @@ __global__ void row_of_ray_kernel(const int64_t* __restrict__ idx, int n_rows, i
   if (i < n_rows) row_of_ray[idx[i]] = i;
 }
 
+// The ray's row in each person's hit list (-1: the person does not cover it); returns K, its samples over all persons.
+__device__ __forceinline__ int ray_rows(const CompositePersons& cp, int P, int ray, int n, int* row) {
+  int K = 0;
+  for (int p = 0; p < P; ++p) {
+    row[p] = cp.row_of_ray[p][ray];
+    if (row[p] >= 0) K += n;
+  }
+  return K;
+}
+
 // Rank of every sample of the ray in the merged (t_end, person, sample) order; scatters sigma * delta into ssd[rank]
 // and the rank into srank.  ste receives the t_end lists ([P][n]) and is free again when this returns.
 __device__ __forceinline__ void merge_ranks(const CompositePersons& cp, const int* row, int n, float beta, float* ste,
@@ -85,11 +95,7 @@ __global__ void composite_kernel(CompositePersons cp, int R, int n, float beta, 
   float* ssd = ste + P * n;                      // sigma*delta in merged order
   int* srank = (int*)(ssd + P * n);              // merged rank of (p,i)
   int row[MP_MAX_PERSONS];
-  int K = 0;
-  for (int p = 0; p < P; ++p) {
-    row[p] = cp.row_of_ray[p][ray];
-    if (row[p] >= 0) K += n;
-  }
+  const int K = ray_rows(cp, P, ray, n, row);
   if (K == 0) {
     if (lane == 0) {
       fg_rgb[3 * ray] = fg_rgb[3 * ray + 1] = fg_rgb[3 * ray + 2] = 0.f;
@@ -174,11 +180,7 @@ __global__ void composite_backward_kernel(CompositePersons cp, CompositeGrads g,
   float* ssd = ste + P * n;                      // sigma*delta -> exclusive prefix, in merged order
   int* srank = (int*)(ssd + P * n);
   int row[MP_MAX_PERSONS];
-  int K = 0;
-  for (int p = 0; p < P; ++p) {
-    row[p] = cp.row_of_ray[p][ray];
-    if (row[p] >= 0) K += n;
-  }
+  const int K = ray_rows(cp, P, ray, n, row);
   if (K == 0) {                                  // bg_T = 1 is a constant: nothing depends on a sample
     if (lane == 0) dbeta_ray[ray] = 0.f;
     return;
@@ -303,11 +305,19 @@ __global__ void final_compose_kernel(const float* __restrict__ fg, const float* 
   if (fg_out) fg_out[i] = fg[i] + bgT[r] * 1.0f;
 }
 
+// Dynamic shared memory per warp (one ray) of both compositor kernels: the t_end lists, sigma*delta and merged ranks of
+// its P*n samples; *wpc is set to the warps per CTA that fit in 200 KB.
+static size_t composite_smem(int P, int n, int* wpc) {
+  const size_t per_warp = (size_t)3 * P * n * sizeof(float);
+  *wpc = clamp_wpc((size_t)(200 * 1024) / per_warp);
+  return per_warp;
+}
+
 int launch_composite(const CompositePersons& cp, int R, int n, float beta, float* fg_rgb, float* normal, float* acc,
                      float* acc_person, float* bg_T, cudaStream_t st) {
-  size_t per_warp = (size_t)3 * cp.P * n * sizeof(float);
+  int wpc;
+  const size_t per_warp = composite_smem(cp.P, n, &wpc);
   MP_REQUIRE(per_warp <= 200 * 1024, "composite: P*n too large for shared memory");
-  int wpc = clamp_wpc((size_t)(200 * 1024) / per_warp);
   MP_CHECK_CUDA(cudaFuncSetAttribute(composite_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)(wpc * per_warp)));
   composite_kernel<<<div_up(R, wpc), wpc * 32, wpc * per_warp, st>>>(cp, R, n, beta, fg_rgb, normal, acc, acc_person,
@@ -318,9 +328,9 @@ int launch_composite(const CompositePersons& cp, int R, int n, float beta, float
 
 int launch_composite_backward(const CompositePersons& cp, const CompositeGrads& g, int R, int n, float beta,
                               float* dbeta_ray, float* d_beta, cudaStream_t st) {
-  size_t per_warp = (size_t)3 * cp.P * n * sizeof(float);
+  int wpc;
+  const size_t per_warp = composite_smem(cp.P, n, &wpc);
   MP_REQUIRE(per_warp <= 200 * 1024, "composite backward: P*n too large for shared memory");
-  int wpc = clamp_wpc((size_t)(200 * 1024) / per_warp);
   MP_CHECK_CUDA(cudaFuncSetAttribute(composite_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)(wpc * per_warp)));
   composite_backward_kernel<<<div_up(R, wpc), wpc * 32, wpc * per_warp, st>>>(cp, g, R, n, beta, dbeta_ray);
@@ -362,6 +372,20 @@ int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cu
   return 0;
 }
 
+// cp from the caller's person records: each person's row_of_ray map is carved from the arena (`who` names the entry
+// point in the error text) and filled from its hit list on st.
+static int composite_persons(Arena& a, const mp_person_samples_t* persons, int P, int R, const char* who,
+                             CompositePersons& cp, cudaStream_t st) {
+  cp.P = P;
+  for (int p = 0; p < P; ++p) {
+    int* ror = a.take<int>(R);
+    MP_REQUIRE(a.ok, "%s: workspace too small", who);
+    MP_TRY(launch_row_of_ray(persons[p].ray_index, persons[p].n_rows, R, ror, st, nullptr));
+    set_person(cp, p, persons[p], ror);
+  }
+  return 0;
+}
+
 int launch_final_compose(const float* fg, const float* bgT, const float* bg, int R, float* rgb, float* fg_out,
                          cudaStream_t st) {
   final_compose_kernel<<<div_up(3 * R, 256), 256, 0, st>>>(fg, bgT, bg, R, rgb, fg_out);
@@ -381,19 +405,8 @@ int mp_composite(const mp_person_samples_t* persons, int P, int R, int n, float 
   MP_REQUIRE(workspace_bytes >= mp_composite_workspace_bytes(R, P), "mp_composite: workspace too small");
   mp::Arena a(workspace, workspace_bytes);
   mp::CompositePersons cp;
-  cp.P = P;
   cudaStream_t st = (cudaStream_t)stream;
-  for (int p = 0; p < P; ++p) {
-    int* ror = a.take<int>(R);
-    MP_REQUIRE(a.ok, "mp_composite: workspace too small");
-    MP_TRY(mp::launch_row_of_ray(persons[p].ray_index, persons[p].n_rows, R, ror, st, nullptr));
-    cp.n_rows[p] = persons[p].n_rows;
-    cp.row_of_ray[p] = ror;
-    cp.z[p] = persons[p].z_vals;
-    cp.sdf[p] = persons[p].sdf;
-    cp.rgb[p] = persons[p].rgb;
-    cp.nrm[p] = persons[p].normal;
-  }
+  MP_TRY(mp::composite_persons(a, persons, P, R, "mp_composite", cp, st));
   return mp::launch_composite(cp, R, n, beta, fg_rgb, normal, acc, acc_person, bg_T, st);
 }
 
@@ -411,13 +424,13 @@ int mp_composite_backward(const mp_person_samples_t* persons, int P, int R, int 
     MP_REQUIRE(persons[p].n_rows == 0 || (grads[p].d_sdf && grads[p].d_rgb && grads[p].d_normal && persons[p].z_vals &&
                                           persons[p].sdf && persons[p].rgb && persons[p].normal && persons[p].ray_index),
                "mp_composite_backward: null argument for person %d", p);
-  MP_REQUIRE((size_t)3 * P * n * sizeof(float) <= 200 * 1024, "mp_composite_backward: P*n too large for shared memory");
+  int wpc;
+  MP_REQUIRE(mp::composite_smem(P, n, &wpc) <= 200 * 1024, "mp_composite_backward: P*n too large for shared memory");
   MP_REQUIRE(workspace_bytes >= mp_composite_backward_workspace_bytes(R, P),
              "mp_composite_backward: workspace too small");
   mp::Arena a(workspace, workspace_bytes);
   mp::CompositePersons cp;
   mp::CompositeGrads g;
-  cp.P = P;
   g.d_fg = d_fg_rgb;
   g.d_nrm = d_normal;
   g.d_acc = d_acc;
@@ -425,16 +438,8 @@ int mp_composite_backward(const mp_person_samples_t* persons, int P, int R, int 
   g.d_bgT = d_bg_T;
   cudaStream_t st = (cudaStream_t)stream;
   float* dbeta_ray = a.take<float>(R);
+  MP_TRY(mp::composite_persons(a, persons, P, R, "mp_composite_backward", cp, st));
   for (int p = 0; p < P; ++p) {
-    int* ror = a.take<int>(R);
-    MP_REQUIRE(a.ok, "mp_composite_backward: workspace too small");
-    MP_TRY(mp::launch_row_of_ray(persons[p].ray_index, persons[p].n_rows, R, ror, st, nullptr));
-    cp.n_rows[p] = persons[p].n_rows;
-    cp.row_of_ray[p] = ror;
-    cp.z[p] = persons[p].z_vals;
-    cp.sdf[p] = persons[p].sdf;
-    cp.rgb[p] = persons[p].rgb;
-    cp.nrm[p] = persons[p].normal;
     g.d_sdf[p] = grads[p].d_sdf;
     g.d_rgb[p] = grads[p].d_rgb;
     g.d_nrm_s[p] = grads[p].d_normal;

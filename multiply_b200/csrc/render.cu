@@ -144,7 +144,7 @@ struct RenderWs {
 
 static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
   const mp_sampler_cfg_t& c = sc.sampler;
-  int n = c.N_samples + c.N_samples_extra + 1;
+  int n = samples_per_ray(c);
   w.dirs = a.take<float>((size_t)R * 3);
   w.cam = a.take<float>((size_t)R * 3);
   w.fg = a.take<float>((size_t)R * 3);
@@ -310,7 +310,7 @@ namespace mp {
 static int render_person(const mp_scene_t* scene, int p, int R, const RenderWs& w, int prune, const mp_render_out_t* out,
                          CompositePersons& cp, cudaStream_t st, cudaEvent_t pre_shade) {
   const mp_sampler_cfg_t& c = scene->sampler;
-  const int n = c.N_samples + c.N_samples_extra + 1;     // multiply.py:290-292
+  const int n = samples_per_ray(c);
   MP_REQUIRE(scene->body[p] && scene->field[p] && scene->hit_index[p] && scene->hit_count[p] >= 1,
              "mp_render_rays: person %d incomplete", p);
   const Body& body = scene->body[p]->b;
@@ -349,12 +349,7 @@ static int render_person(const mp_scene_t* scene, int p, int R, const RenderWs& 
     MP_LAUNCH_CHECK();
   }
   MP_TRY(launch_row_of_ray(scene->hit_index[p], Rp, R, b.row_of_ray, st, Rp_dev));
-  cp.n_rows[p] = Rp;
-  cp.row_of_ray[p] = b.row_of_ray;
-  cp.z[p] = b.z;
-  cp.sdf[p] = b.sdf;
-  cp.rgb[p] = b.rgb;
-  cp.nrm[p] = b.nrm;
+  set_person(cp, p, mp_person_samples_t{Rp, scene->hit_index[p], b.z, b.sdf, b.rgb, b.nrm}, b.row_of_ray);
   auto tap = [&](float* dst, const float* src, size_t cnt) -> int {
     if (dst) MP_CHECK_CUDA(cudaMemcpyAsync(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -385,8 +380,8 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
   MP_REQUIRE(n_mesh == 0 || !isnan(tr->surface_threshold), "mp_render_rays: surface_threshold is NaN");
   const cudaStream_t caller = (cudaStream_t)stream;
   const mp_sampler_cfg_t& c = scene->sampler;
-  const int n = c.N_samples + c.N_samples_extra + 1;     // multiply.py:290-292
-  const float beta = fabsf(c.beta_param) + c.beta_min;
+  const int n = samples_per_ray(c);
+  const float beta = sampler_beta(c);
   const int prune = prune_is_exact(beta) ? 1 : 0;
   Arena a(workspace, workspace_bytes);
   RenderWs w;

@@ -452,7 +452,7 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
   SamplerWs w;
   MP_REQUIRE(sampler_carve(a, c, R, w), "sampler: workspace too small (%zu needed, %zu given)", a.off, ws_bytes);
   const int zcap = c.max_total_iters * E;
-  const float beta0 = fabsf(c.beta_param) + c.beta_min;                    // density.py:27-29
+  const float beta0 = sampler_beta(c);
   const float bound_coef = 1.0f / (4.0f * logf((float)(c.eps + 1.0)));     // ray_sampler.py:75
   int tn = max(max(E, S), max(32, c.max_total_iters * max(X, 1)));
   tables_kernel<<<div_up(tn, 128), 128, 0, st>>>(w.tab, E, S, X, c.max_total_iters,

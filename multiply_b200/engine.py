@@ -292,7 +292,27 @@ class CanonicalMesh:
             pass
 
 
-def sampler_cfg(cfg, beta_param, beta_min=1e-4):
+BETA_MIN = 1e-4      # LaplaceDensity's default (density.py:24)
+
+
+def sampler_beta(beta_param, beta_min=BETA_MIN):
+    """The sampler's and the compositor's beta: |beta_param| + beta_min in fp32, as mp_render_rays forms it."""
+    return float(np.float32(abs(np.float32(beta_param))) + np.float32(beta_min))
+
+
+def samples_per_ray(cfg):
+    """n, the samples per ray after the sampler (multiply.py:290-292)."""
+    return cfg["N_samples"] + cfg["N_samples_extra"] + 1
+
+
+def hit_list(ids, device=None):
+    """A person's ray ids (tensor or sequence) as a contiguous int64 tensor on ``device`` (default: where they are);
+    an empty list becomes ray 0 (multiply.py:262-263)."""
+    h = torch.as_tensor(ids, dtype=torch.int64).reshape(-1)
+    return (h if h.numel() else torch.zeros(1, dtype=torch.int64)).to(device).contiguous()
+
+
+def sampler_cfg(cfg, beta_param, beta_min=BETA_MIN):
     c = L.SamplerCfg()
     c.scene_bounding_sphere = cfg["scene_bounding_sphere"]
     c.near = cfg.get("near", 0.0)
@@ -319,14 +339,14 @@ class Renderer:
         device = self.device
         self.cfg = scene["cfg"]
         self.beta_param = float(scene["beta_param"])
-        self.beta_min = float(scene.get("beta_min", 1e-4))
+        self.beta_min = float(scene.get("beta_min", BETA_MIN))
         self.P = len(scene["persons"])
         self.fields, self.bodies = [], []
         with torch.cuda.device(self.device):
             self._build(scene, device)
         self._ws = None
         self._status = None
-        self.n = self.cfg["N_samples"] + self.cfg["N_samples_extra"] + 1
+        self.n = samples_per_ray(self.cfg)
 
     def _build(self, scene, device):
         for person in scene["persons"]:
@@ -401,9 +421,9 @@ class Renderer:
                 h, cnt = h
                 assert h.is_cuda and cnt.is_cuda and h.dtype == torch.int64 and cnt.dtype == torch.int32
                 dev_counts = True
-            elif h.numel() == 0:
-                h = torch.zeros(1, dtype=torch.int64)
-            h = h.to(device=dev, dtype=torch.int64).contiguous()
+                h = h.to(dev).contiguous()
+            else:
+                h = hit_list(h, dev)
             hits.append((h, cnt))
             sc.body[k] = self.bodies[p].handle
             sc.field[k] = self.fields[p].handle
@@ -418,9 +438,9 @@ class Renderer:
         grad_on = beta is not None
         if grad_on:
             assert torch.is_tensor(beta) and beta.numel() == 1, "train['beta'] must be a 0-d tensor"
-            want = np.float32(abs(np.float32(self.beta_param))) + np.float32(self.beta_min)
+            want = sampler_beta(self.beta_param, self.beta_min)
             assert np.float32(float(beta.detach())) == want, \
-                "train['beta'] = %r differs from the sampler's beta %r" % (float(beta.detach()), float(want))
+                "train['beta'] = %r differs from the sampler's beta %r" % (float(beta.detach()), want)
             assert not dev_counts, "render gradients need host-side hit counts"
         if train is not None:
             assert not dev_counts, "training mode needs host-side hit counts"
@@ -467,47 +487,25 @@ class Renderer:
         for k, v in res.items():
             setattr(out, k, v.data_ptr())
         out.status = self._status.data_ptr()
+        taps = {}
+        if debug or grad_on:       # per-sample taps: debug outputs and the compositor's inputs for RenderComposite
+            n = self.n
+            taps["bg_T"] = torch.empty(R, device=dev)
+            out.bg_T = taps["bg_T"].data_ptr()
+            for k in range(Pn):
+                Rp = hits[k][0].numel()
+                for name, shp in (("z_vals", (Rp, n + 1)), ("sdf", (Rp, n)), ("rgb", (Rp, n, 3)), ("normals", (Rp, n, 3))):
+                    taps[f"{name}_{k}"] = torch.empty(*shp, device=dev)
+                    getattr(out, name)[k] = taps[f"{name}_{k}"].data_ptr()
         dbg = {}
         if debug:
             assert not dev_counts, "debug taps need host-side hit counts"
-            n = self.n
-            dbg["trips"] = torch.zeros(Pn, dtype=torch.int32, device=dev)
-            dbg["bg_T"] = torch.empty(R, device=dev)
+            dbg = {"trips": torch.zeros(Pn, dtype=torch.int32, device=dev), **taps}
             out.trips = dbg["trips"].data_ptr()
-            out.bg_T = dbg["bg_T"].data_ptr()
-            for k in range(Pn):
-                Rp = hits[k][0].numel()
-                dbg[f"z_vals_{k}"] = torch.empty(Rp, n + 1, device=dev)
-                dbg[f"sdf_{k}"] = torch.empty(Rp, n, device=dev)
-                dbg[f"rgb_{k}"] = torch.empty(Rp, n, 3, device=dev)
-                dbg[f"normals_{k}"] = torch.empty(Rp, n, 3, device=dev)
-                out.z_vals[k] = dbg[f"z_vals_{k}"].data_ptr()
-                out.sdf[k] = dbg[f"sdf_{k}"].data_ptr()
-                out.rgb[k] = dbg[f"rgb_{k}"].data_ptr()
-                out.normals[k] = dbg[f"normals_{k}"].data_ptr()
-        taps = None
-        if grad_on:        # the compositor's inputs, kept for RenderComposite.backward
-            n = self.n
-            taps = dict(z=[], sdf=[], rgb=[], nrm=[], bg_T=torch.empty(R, device=dev))
-            for k in range(Pn):
-                Rp = hits[k][0].numel()
-                for key, shp in (("z", (Rp, n + 1)), ("sdf", (Rp, n)), ("rgb", (Rp, n, 3)), ("nrm", (Rp, n, 3))):
-                    name = {"z": "z_vals", "sdf": "sdf", "rgb": "rgb", "nrm": "normals"}[key]
-                    t = dbg.get(f"{name}_{k}")
-                    if t is None:
-                        t = torch.empty(*shp, device=dev)
-                        getattr(out, name)[k] = t.data_ptr()
-                    taps[key].append(t)
-            if out.bg_T:
-                taps["bg_T"] = dbg["bg_T"]
-            else:
-                out.bg_T = taps["bg_T"].data_ptr()
-            if self.bg is not None:
-                taps.update(bg_rgb=torch.empty(R, 3, device=dev), bg_sdf=torch.empty(R, 32, device=dev),
-                            bg_rgb_s=torch.empty(R, 32, 3, device=dev))
-                out.bg_rgb = taps["bg_rgb"].data_ptr()
-                out.bg_sdf = taps["bg_sdf"].data_ptr()
-                out.bg_rgb_samples = taps["bg_rgb_s"].data_ptr()
+        if grad_on and self.bg is not None:
+            for name, shp in (("bg_rgb", (R, 3)), ("bg_sdf", (R, 32)), ("bg_rgb_samples", (R, 32, 3))):
+                taps[name] = torch.empty(*shp, device=dev)
+                setattr(out, name, taps[name].data_ptr())
         L.check(lib.mp_render_rays(C.byref(sc), uv.data_ptr(), pose.data_ptr(), K.data_ptr(), R, C.byref(out),
                                    self._ws.data_ptr(), self._ws.numel(), L.stream_ptr()), "mp_render_rays")
         self._keep = (uv, pose, K, hits, keep_train)
@@ -524,17 +522,17 @@ class Renderer:
 
     def _attach_graph(self, res, taps, hits, beta, t_rand_bg, R, Pn):
         dev = self.device
-        samples = [dict(sdf=taps["sdf"][k].clone().requires_grad_(True), rgb=taps["rgb"][k].clone().requires_grad_(True),
-                        normal=taps["nrm"][k].clone().requires_grad_(True), z_vals=taps["z"][k], ray_index=hits[k][0])
+        samples = [dict(sdf=taps[f"sdf_{k}"].clone().requires_grad_(True), rgb=taps[f"rgb_{k}"].clone().requires_grad_(True),
+                        normal=taps[f"normals_{k}"].clone().requires_grad_(True), z_vals=taps[f"z_vals_{k}"], ray_index=hits[k][0])
                    for k in range(Pn)]
         leaves = [t for d in samples for t in (d["sdf"], d["rgb"], d["normal"])]
         extra = {}
-        info = dict(n=self.n, R=R, P=Pn, beta=float(beta.detach()), hits=[h[0] for h in hits], z=taps["z"],
+        info = dict(n=self.n, R=R, P=Pn, beta=float(beta.detach()), hits=[h[0] for h in hits], z=[d["z_vals"] for d in samples],
                     bg_T=taps["bg_T"], bound=float(self.cfg["scene_bounding_sphere"]), device=dev, bg=None)
         if self.bg is not None:
             t_rand = None if t_rand_bg is None else _dev(t_rand_bg, dev)
-            bg = dict(sdf=taps["bg_sdf"].clone().requires_grad_(True), rgb=taps["bg_rgb_s"].clone().requires_grad_(True),
-                      t_rand=t_rand, bg_rgb=taps["bg_rgb"])
+            bg = dict(sdf=taps["bg_sdf"].clone().requires_grad_(True),
+                      rgb=taps["bg_rgb_samples"].clone().requires_grad_(True), t_rand=t_rand, bg_rgb=taps["bg_rgb"])
             leaves += [bg["sdf"], bg["rgb"]]
             info["bg"] = dict(rgb=taps["bg_rgb"], t_rand=t_rand)
             extra["samples_bg"] = bg
@@ -581,16 +579,12 @@ class RenderComposite(torch.autograd.Function):
             L.check(lib.mp_final_compose_backward(info["bg_T"].data_ptr(), L.ptr(bg["rgb"]) if bg else None, R,
                                                   d_rgb.data_ptr(), L.ptr(d_fgv), d_fg.data_ptr(), d_bgT.data_ptr(),
                                                   L.ptr(d_bg), st), "mp_final_compose_backward")
-            arr = (L.PersonSamples * P)()
+            arr = person_samples([(info["hits"][k], info["z"][k], *leaves[3 * k: 3 * k + 3], info["hits"][k].numel())
+                                  for k in range(P)])
             gr = (L.PersonSampleGrads * P)()
             grads = []
             for k in range(P):
-                sdf, rgb, nrm = leaves[3 * k: 3 * k + 3]
-                arr[k].n_rows = info["hits"][k].numel()
-                arr[k].ray_index = info["hits"][k].data_ptr()
-                arr[k].z_vals = info["z"][k].data_ptr()
-                arr[k].sdf, arr[k].rgb, arr[k].normal = sdf.data_ptr(), rgb.data_ptr(), nrm.data_ptr()
-                gk = (torch.empty_like(sdf), torch.empty_like(rgb), torch.empty_like(nrm))
+                gk = tuple(torch.empty_like(t) for t in leaves[3 * k: 3 * k + 3])
                 gr[k].d_sdf, gr[k].d_rgb, gr[k].d_normal = (t.data_ptr() for t in gk)
                 grads += gk
             d_beta = torch.empty(1, device=dev)
@@ -606,6 +600,16 @@ class RenderComposite(torch.autograd.Function):
                                                      d_brgb.data_ptr(), st), "mp_bg_composite_backward")
                 grads += [d_bsdf, d_brgb]
         return (None, None, d_beta.reshape(ctx.beta_shape)) + tuple(grads)
+
+
+def person_samples(persons):
+    """mp_person_samples_t array from per-person (ray_index, z_vals, sdf, rgb, normal, n_rows); the caller keeps the
+    tensors alive while the array is in use."""
+    arr = (L.PersonSamples * len(persons))()
+    for a, (idx, z, sdf, rgb, nrm, n_rows) in zip(arr, persons):
+        a.ray_index, a.z_vals, a.sdf, a.rgb, a.normal = (t.data_ptr() for t in (idx, z, sdf, rgb, nrm))
+        a.n_rows = n_rows
+    return arr
 
 
 def sampler_rng_struct(rng, dev):

@@ -351,9 +351,7 @@ class Multiply(nn.Module):
                 v = pd["verts_p"]
                 lo, hi = v.min(0)[0], v.max(0)[0]
                 h = engine.ray_box_hits(cam, dirs, ((lo + hi) / 2).tolist(), ((hi - lo) / 2 * 1.2).tolist())
-            if h.numel() == 0:
-                h = torch.zeros(1, dtype=torch.int64, device=dev)                  # multiply.py:262-263
-            h = h.to(dev)
+            h = engine.hit_list(h, dev)
             hits.append(h)
             # the reference's draws for this person, in its order: get_z_vals (ray_sampler.py:38,171,202,212,216) ...
             rng = self.ray_sampler.draw_training_rng(h.numel())

@@ -36,8 +36,7 @@ class ErrorBoundSampler:
         body.set_pose(smpl_verts[0], smpl_tfs[0] if smpl_tfs.ndim == 4 else smpl_tfs)
         field = model.field_list[person_id]
         field.set_cond(cond["smpl"])
-        nz = self.N_samples + self.N_samples_extra + 2
-        z = torch.empty(R, nz, device=dev)
+        z = torch.empty(R, engine.samples_per_ray(self.cfg) + 1, device=dev)
         z_bg = torch.empty(R, 32, device=dev)
         trips = torch.zeros(1, dtype=torch.int32, device=dev)
         need = lib.mp_sampler_workspace_bytes(C.byref(c), R)

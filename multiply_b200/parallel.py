@@ -7,6 +7,8 @@ the reference)."""
 import torch
 import torch.distributed as dist
 
+from . import _lib as L, engine
+
 PIXEL_KEYS = ("rgb_values", "fg_rgb_values", "normal_values", "acc_map", "acc_person_list")
 
 
@@ -94,12 +96,8 @@ def person_owner(p, world):
 
 
 def normalize_hits(hit_lists):
-    """multiply.py:262-263: an empty hit list is replaced by ray 0."""
-    out = []
-    for h in hit_lists:
-        h = torch.as_tensor(h, dtype=torch.int64).reshape(-1)
-        out.append(h if h.numel() else torch.zeros(1, dtype=torch.int64))
-    return out
+    """engine.hit_list of every person's ray ids, left where they are (multiply.py:262-263: empty -> ray 0)."""
+    return [engine.hit_list(h) for h in hit_lists]
 
 
 def exchange_plan(hit_lists, total_rays, world):
@@ -147,7 +145,6 @@ class PersonShardedRenderer:
     """Eval forward with the persons' fields sharded over the ranks of the default process group."""
 
     def __init__(self, scene, device="cuda", group=None):
-        from . import engine
         self.group = group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -155,7 +152,7 @@ class PersonShardedRenderer:
         self.scene = scene
         self.P = len(scene["persons"])
         self.cfg = scene["cfg"]
-        self.n = self.cfg["N_samples"] + self.cfg["N_samples_extra"] + 1
+        self.n = engine.samples_per_ray(self.cfg)
         self.width = 8 * self.n + 1
         self.mine = [p for p in range(self.P) if person_owner(p, self.world) == self.rank]
         # this rank's persons only; no background in the per-person pass
@@ -168,9 +165,7 @@ class PersonShardedRenderer:
         if scene.get("bg_implicit") is not None:
             self.bg = engine.Field(scene["bg_implicit"], scene["bg_render"], background=True, device=device)
             self.bg.set_cond(scene["frame_code"])
-        import numpy as np
-        # fp32 arithmetic, as mp_render_rays does it (density.py:27-29)
-        self.beta = float(np.float32(abs(float(scene["beta_param"]))) + np.float32(1e-4))
+        self.beta = engine.sampler_beta(scene["beta_param"], scene.get("beta_min", engine.BETA_MIN))
 
     def person_rows(self, inputs, hits):
         """Step 1: [R_p, 8n+1] rows of the persons this rank owns."""
@@ -186,18 +181,14 @@ class PersonShardedRenderer:
 
     def composite_block(self, inputs, hits, got, lo, hi):
         """Step 3 for the ray block [lo, hi)."""
-        import ctypes as C
-        from . import _lib as L
         lib = L.lib()
         dev = self.device
         n, Rb = self.n, hi - lo
         keep = []
-        persons = (L.PersonSamples * self.P)()
-        plan_rank = [self._plan[p][self.rank] for p in range(self.P)]
         for p in range(self.P):
             r = got[p]
             cnt = r.shape[0]
-            rlo, rhi = plan_rank[p]
+            rlo, rhi = self._plan[p][self.rank]
             idx = (hits[p][rlo:rhi].to(dev) - lo).contiguous()
             z = r[:, : n + 1].contiguous()
             sdf = r[:, n + 1: 2 * n + 1].contiguous()
@@ -206,13 +197,8 @@ class PersonShardedRenderer:
             if cnt == 0:      # valid (never dereferenced) pointers for an empty person
                 idx = torch.zeros(1, dtype=torch.int64, device=dev)
                 z = sdf = rgb = nrm = torch.zeros(1, device=dev)
-            keep += [idx, z, sdf, rgb, nrm]
-            persons[p].n_rows = cnt
-            persons[p].ray_index = idx.data_ptr()
-            persons[p].z_vals = z.data_ptr()
-            persons[p].sdf = sdf.data_ptr()
-            persons[p].rgb = rgb.data_ptr()
-            persons[p].normal = nrm.data_ptr()
+            keep.append((idx, z, sdf, rgb, nrm, cnt))
+        persons = engine.person_samples(keep)
         fg = torch.empty(Rb, 3, device=dev)
         out = {"rgb_values": torch.empty(Rb, 3, device=dev), "fg_rgb_values": torch.empty(Rb, 3, device=dev),
                "normal_values": torch.empty(Rb, 3, device=dev), "acc_map": torch.empty(Rb, device=dev),

@@ -46,11 +46,10 @@ def _time(fn, steps):
 
 
 def workload(P, R, n, steps):
-    from multiply_b200 import _lib as L
+    from multiply_b200 import _lib as L, engine
     lib = L.lib()
     g = torch.Generator(device="cuda").manual_seed(R + n)
     dev = "cuda"
-    arr = (L.PersonSamples * P)()
     gr = (L.PersonSampleGrads * P)()
     keep = []
     for p in range(P):
@@ -61,9 +60,8 @@ def workload(P, R, n, steps):
                  d_sdf=torch.empty(R, n, device=dev), d_rgb=torch.empty(R, n, 3, device=dev),
                  d_nrm=torch.empty(R, n, 3, device=dev))
         keep.append(t)
-        arr[p].n_rows, arr[p].ray_index, arr[p].z_vals = R, t["idx"].data_ptr(), t["z"].data_ptr()
-        arr[p].sdf, arr[p].rgb, arr[p].normal = t["sdf"].data_ptr(), t["rgb"].data_ptr(), t["nrm"].data_ptr()
         gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = t["d_sdf"].data_ptr(), t["d_rgb"].data_ptr(), t["d_nrm"].data_ptr()
+    arr = engine.person_samples([(t["idx"], t["z"], t["sdf"], t["rgb"], t["nrm"], R) for t in keep])
     o = {k: torch.empty(*s, device=dev) for k, s in (("fg", (R, 3)), ("nrm", (R, 3)), ("acc", (R,)), ("accp", (R, P)),
                                                      ("bgT", (R,)))}
     u = {k: torch.randn(*v.shape, device=dev, generator=g) for k, v in o.items()}

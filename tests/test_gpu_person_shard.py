@@ -8,11 +8,15 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("P,empty", [(2, None), (3, 1)])
-def test_person_sharded_equals_fused_forward(P, empty):
+@pytest.mark.parametrize("P,empty,beta_min", [pytest.param(2, None, None, id="2-None"),
+                                               pytest.param(3, 1, None, id="3-1"),
+                                               pytest.param(2, None, 1e-3, id="2-None-beta_min1e-3")])
+def test_person_sharded_equals_fused_forward(P, empty, beta_min):
     from multiply_b200 import engine, parallel, scene as S
     engine.set_engine("tc")
     sc = S.make_scene(P=P, S=64, seed=11)
+    if beta_min is not None:                                  # a density.beta_min other than LaplaceDensity's default
+        sc["beta_min"] = beta_min
     inp = S.make_rays(sc, 257, seed=2, region="boxes")
     hits = S.make_hit_lists(sc, inp)
     if empty is not None:
