@@ -145,6 +145,10 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// bulk prefetch of `bytes` (a multiple of 16) of global memory into L2
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // barrier of one consumer warpgroup (ids 1, 2)
@@ -485,6 +489,16 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
       const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
       const bool one_term = st.terms == 1;
+      // The 132 CTAs' stash (1.2 MB each) does not fit in L2: the sigma' this reverse step's epilogue reads, and the
+      // features the final-gradient step reloads, were mostly evicted to DRAM since the forward sweep wrote them.  Pull
+      // this warpgroup's 64 KB block back into L2 while the step's MMAs run, so the epilogue's loads hit L2.  (Issued
+      // one step earlier it gains less: the block competes longer with the rest of the stash.)
+      if (t == 0) {
+        char* ws = io.scratch + (size_t)blockIdx.x * io.scratch_per_cta;
+        if (st.epi == EPI_BWD && st.sig >= 0)
+          prefetch_l2(ws + (((size_t)st.sig * kConsumers + g) * 32 * 128) * 16, 32 * 128 * 16);
+        if (st.flags & F_FINAL_GRAD) prefetch_l2(ws + kSigBytes + (size_t)g * 32 * 128 * 16, 32 * 128 * 16);
+      }
 
       // ---------------- MMAs: acc = A . W^T over st.nk K-blocks ----------------
       // this warpgroup's rows of A are complete: publish them to the tensor cores
