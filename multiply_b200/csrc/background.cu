@@ -148,7 +148,13 @@ int render_background(const Field& f, const float* dirs, const float* cam, int R
   float inv_bound = (float)(1.0 / bound);
   bg_points_kernel<<<div_up(N, 256), 256, 0, st>>>(dirs, cam, R, bound, inv_bound, pts, dexp, t_rand);
   MP_LAUNCH_CHECK();
-  MP_TRY(field_bg(f, pts, dexp, N, sdf, rgb, mws, mb, st));
+  MlpCall c{};
+  c.x = pts;
+  c.cap = N;
+  c.dirs = dexp;
+  c.sdf = sdf;
+  c.rgb = rgb;
+  MP_TRY(field_run(f, c, mws, mb, st));
   if (tap_sdf) MP_CHECK_CUDA(cudaMemcpyAsync(tap_sdf, sdf, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (tap_rgb) MP_CHECK_CUDA(cudaMemcpyAsync(tap_rgb, rgb, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   bg_composite_kernel<<<div_up(N, 256), 256, 0, st>>>(sdf, rgb, R, inv_bound, bg_rgb, t_rand);

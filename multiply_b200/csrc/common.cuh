@@ -152,27 +152,40 @@ static inline int samples_per_ray(const mp_sampler_cfg_t& c) { return c.N_sample
 
 // ---- cross-file launchers: every internal function or type one .cu file uses from another --------
 
+// One evaluation of a field's networks over a list of points, the same for both MLP engines.  Outputs left null are
+// not written.  sdf, rgb and nrm go to each point's slot (dense when `slot` is null); grad and feat are always dense.
+struct MlpCall {
+  const float* x;       // [cap, d_in] points (canonical space; background: [cap, 4])
+  const int* slot;      // [cap] output slot of each point, or nullptr (slot = index)
+  const int* count;     // device count of valid points, or nullptr (= cap)
+  int cap;
+  const float* jinv;    // [cap, 12] inverse deformation Jacobians (3x3 row-major, padded to 12): normals and rgb
+  const float* dirs;    // [cap, 3] view directions: the background networks
+  float* sdf;           // [slots]
+  float* rgb;           // [slots, 3]
+  float* nrm;           // [slots, 3]
+  float* grad;          // [cap, 3] d sdf / d x
+  float* feat;          // [cap, 256] ImplicitNet features
+};
+// Which chain a call runs; the values are also the profile kinds of mp_profile_read.
+enum class MlpProg { kSdf = 0, kForward = 1, kFull = 2, kBg = 3 };
+static inline MlpProg mlp_prog(const MlpCall& c) {
+  if (c.dirs) return MlpProg::kBg;                       // background: sdf + rgb
+  if (c.jinv || c.grad) return MlpProg::kFull;           // forward + reverse sweep (+ colour with jinv); a feat request
+                                                         // costs the tensor-core engine one more forward launch
+  if (c.feat) return MlpProg::kForward;                  // sdf + features
+  return MlpProg::kSdf;
+}
+
 // fp32 SIMT engine (mlp_simt.cu)
 size_t simt_workspace_bytes(int N);
-int simt_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                  float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int simt_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                    const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                    float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int simt_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-            size_t ws_bytes, cudaStream_t st);
+int simt_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st);
 int simt_render(const Field& f, const float* pts, const float* nrm, const float* feat, int N, float* rgb, void* ws,
                 size_t ws_bytes, cudaStream_t st);
 
 // tensor-core engine (mlp_tc.cu)
 size_t tc_workspace_bytes(int N);
-int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                  const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                  float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int tc_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-          size_t ws_bytes, cudaStream_t st);
+int tc_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st);
 int tc_pack(Field& f, Arena& a, cudaStream_t st);
 size_t tc_pack_bytes();
 void tc_free(Field& f);
@@ -183,13 +196,7 @@ extern std::atomic<int> g_precision;
 // engine dispatch (render.cu): g_engine 1 = tensor cores, 0 = SIMT; field_ws_bytes covers either engine
 extern std::atomic<int> g_engine;
 size_t field_ws_bytes(int N);
-int field_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                   float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int field_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                     const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                     float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st);
-int field_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-             size_t ws_bytes, cudaStream_t st);
+int field_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st);
 
 // deformer (deform.cu)
 int launch_deform_rays(const Body& b, const float* dirs, const float* cam, const float* z, int z_stride,

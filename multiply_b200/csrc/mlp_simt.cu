@@ -284,30 +284,7 @@ static int simt_trunk(const Field& f, const float* x, int N, const int* n_dev, S
   return 0;
 }
 
-// sdf only, scattered to slots.  xc_list [cap,3]
-int simt_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                  float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const int CH = 65536;
-  for (int s = 0; s < cap; s += CH) {
-    int n = min(CH, cap - s);
-    Arena a(ws, ws_bytes);
-    SimtBufs b;
-    int* nrem = a.take<int>(1);
-    MP_REQUIRE(simt_take(a, n, b, false), "simt_sdf_list: workspace too small (%zu needed)", a.off);
-    // remaining count for this chunk = count - s (clamped by the kernels through min(N, *n_dev))
-    sub_count_kernel<<<1, 1, 0, st>>>(count_dev, s, nrem);
-    MP_LAUNCH_CHECK();
-    float* h7;
-    MP_TRY(simt_trunk(f, xc_list + 3 * (size_t)s, n, nrem, b, false, &h7, st));
-    scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nrem,
-                                                            slot_list ? slot_list + s : nullptr,
-                                                            slot_list ? sdf_out : sdf_out + s);
-    MP_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-__global__ void sub_count_kernel(const int* c, int s, int* out) { *out = c ? max(0, *c - s) : 0x7fffffff; }
+__global__ void sub_count_kernel(const int* c, int s, int* out) { *out = max(0, *c - s); }
 
 // RenderingNet layers on the colour input cin [n, ldc] (networks.py:290-312): ReLU layers ping-ponging between c0 and
 // c1, the sigmoid head into a [n,4]-strided buffer, then rgb repacked 3-strided to its slot (dense when slot is null)
@@ -330,35 +307,51 @@ static int simt_colour(const Field& f, const float* cin, int ldc, int n, const i
   return 0;
 }
 
-// full foreground shading of a compact list: sdf (scatter), normals (scatter), rgb (scatter)
-// grad_out (optional, [cap,3] dense) receives d sdf / d x_c ; feat_out (optional, dense [cap,256]).
-int simt_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                    const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                    float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const int CH = 32768;
+// One MlpCall, the chain that mlp_prog picks, in chunks of the list.  sdf, rgb and normals are scattered to their slots.
+int simt_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const MlpProg prog = mlp_prog(c);
+  const bool bwd = prog == MlpProg::kFull;
+  const int CH = bwd ? 32768 : 65536;
   const int E = f.emb_dim;
-  for (int s = 0; s < cap; s += CH) {
-    int n = min(CH, cap - s);
+  for (int s = 0; s < c.cap; s += CH) {
+    int n = min(CH, c.cap - s);
     Arena a(ws, ws_bytes);
     SimtBufs b;
     int* nrem = a.take<int>(1);
-    MP_REQUIRE(simt_take(a, n, b, true), "simt_shade_list: workspace too small (%zu needed)", a.off);
-    sub_count_kernel<<<1, 1, 0, st>>>(count_dev, s, nrem);
-    MP_LAUNCH_CHECK();
-    const float* x = xc_list + 3 * (size_t)s;
+    MP_REQUIRE(simt_take(a, n, b, bwd), "simt_run: workspace too small (%zu needed)", a.off);
+    if (c.count) {
+      // remaining count for this chunk = count - s (clamped by the kernels through min(N, *n_dev))
+      sub_count_kernel<<<1, 1, 0, st>>>(c.count, s, nrem);
+      MP_LAUNCH_CHECK();
+    } else {
+      nrem = nullptr;
+    }
+    const float* x = c.x + (size_t)f.d_in * s;
+    const int* slot = c.slot ? c.slot + s : nullptr;
+    auto out = [&](float* p, int width) { return p && !c.slot ? p + (size_t)width * s : p; };   // slotted or dense
     float* h7;
-    MP_TRY(simt_trunk(f, x, n, nrem, b, true, &h7, st));
-    if (sdf_out) {
-      scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nrem,
-                                                              slot_list ? slot_list + s : nullptr,
-                                                              slot_list ? sdf_out : sdf_out + s);
+    MP_TRY(simt_trunk(f, x, n, nrem, b, bwd, &h7, st));
+    if (c.sdf) {
+      scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nrem, slot,
+                                                              out(c.sdf, 1));
       MP_LAUNCH_CHECK();
     }
+    if (prog == MlpProg::kSdf) continue;
+    if (prog == MlpProg::kBg) {     // multiply.py:524-531
+      const int X = f.ren_extra, ldc = X + 256;
+      view_embed_kernel<<<div_up(n, 128), 128, 0, st>>>(c.dirs + 3 * (size_t)s, f.multires_view, n, b.cin, ldc);
+      MP_LAUNCH_CHECK();
+      // features straight into the colour input block
+      MP_TRY(dense(h7, 256, nullptr, 0, f.imp_Wt[8] + 1, kHidden + 1, f.imp_b[8] + 1, b.cin + X, ldc, nullptr, n, nrem,
+                   kHidden, kHidden, ACT_NONE, st));
+      MP_TRY(simt_colour(f, b.cin, ldc, n, nrem, (h7 == b.H0) ? b.H1 : b.H0, h7, slot, out(c.rgb, 3), st));
+      continue;
+    }
     // features = h7 @ W8[1:,:]^T + b8[1:]
-    float* featp = feat_out ? feat_out + (size_t)s * 256 : b.feat;
+    float* featp = c.feat ? c.feat + (size_t)s * 256 : b.feat;
     MP_TRY(dense(h7, 256, nullptr, 0, f.imp_Wt[8] + 1, kHidden + 1, f.imp_b[8] + 1, featp, 256, nullptr, n, nrem,
                  kHidden, kHidden, ACT_NONE, st));
-    if (!Jinv_list && !grad_out) continue;
+    if (prog == MlpProg::kForward) continue;
     // ---- backward: d sdf / d x_c ---------------------------------------------------------
     float* g = (h7 == b.H0) ? b.H1 : b.H0;   // free buffer
     float* g2 = h7;                          // h7 no longer needed after features
@@ -382,22 +375,20 @@ int simt_shade_list(const Field& f, const float* xc_list, const int* slot_list, 
     // layer 0: d/d embed = (g * dact_0) @ W0[:, :E]
     MP_TRY(dense(g, 256, b.dact[0], 256, f.imp_W[0], f.imp_in[0], nullptr, g2, 256, nullptr, n, nrem, kHidden, E,
                  ACT_NONE, st));
-    float* gradp = grad_out ? grad_out + 3 * (size_t)s : b.grad;
+    float* gradp = c.grad ? c.grad + 3 * (size_t)s : b.grad;
     embed_backward_kernel<<<div_up(n, 128), 128, 0, st>>>(x, f.d_in, f.multires, n, nrem, g2, 256, b.ge0, 96, 0,
                                                           gradp);
     MP_LAUNCH_CHECK();
-    if (!Jinv_list) continue;
+    if (!c.jinv) continue;
     // ---- normals + colour ----------------------------------------------------------------
     const int ldc = 6 + 256;
-    normal_colour_input_kernel<<<div_up(n, 128), 128, 0, st>>>(x, gradp, Jinv_list + 12 * (size_t)s, featp, n, nrem,
+    normal_colour_input_kernel<<<div_up(n, 128), 128, 0, st>>>(x, gradp, c.jinv + 12 * (size_t)s, featp, n, nrem,
                                                                b.cin, ldc, b.ntmp);
     MP_LAUNCH_CHECK();
     copy_cols_kernel<<<div_up(n * 256, 256), 256, 0, st>>>(featp, 256, 0, 256, n, nrem, b.cin, ldc, 6);
     MP_LAUNCH_CHECK();
-    MP_TRY(simt_colour(f, b.cin, ldc, n, nrem, b.H0, b.H1, slot_list ? slot_list + s : nullptr,
-                       slot_list ? rgb_out : rgb_out + 3 * (size_t)s, st));
-    scatter3_kernel<<<div_up(n, 256), 256, 0, st>>>(b.ntmp, n, nrem, slot_list ? slot_list + s : nullptr,
-                                                    slot_list ? normal_out : normal_out + 3 * (size_t)s);
+    MP_TRY(simt_colour(f, b.cin, ldc, n, nrem, b.H0, b.H1, slot, out(c.rgb, 3), st));
+    scatter3_kernel<<<div_up(n, 256), 256, 0, st>>>(b.ntmp, n, nrem, slot, out(c.nrm, 3));
     MP_LAUNCH_CHECK();
   }
   return 0;
@@ -421,34 +412,6 @@ __global__ void scatter_rgb4_kernel(const float* __restrict__ src, int N, const 
   dst[3 * (size_t)s] = src[4 * i];
   dst[3 * (size_t)s + 1] = src[4 * i + 1];
   dst[3 * (size_t)s + 2] = src[4 * i + 2];
-}
-
-// background field: pts [N,4], dirs [N,3] -> sdf [N], rgb [N,3]     (multiply.py:524-531)
-int simt_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-            size_t ws_bytes, cudaStream_t st) {
-  const int CH = 65536;
-  for (int s = 0; s < N; s += CH) {
-    int n = min(CH, N - s);
-    Arena a(ws, ws_bytes);
-    SimtBufs b;
-    a.take<int>(1);
-    MP_REQUIRE(simt_take(a, n, b, false), "simt_bg: workspace too small (%zu needed)", a.off);
-    float* h7;
-    MP_TRY(simt_trunk(f, pts + 4 * (size_t)s, n, nullptr, b, false, &h7, st));
-    if (sdf) {     // may be NULL (mp_bg_nets_forward)
-      scatter_sdf_kernel<<<div_up(n * 32, 256), 256, 0, st>>>(h7, f.imp_Wt[8], 0.f, f.imp_b[8], n, nullptr, nullptr,
-                                                              sdf + s);
-      MP_LAUNCH_CHECK();
-    }
-    const int X = f.ren_extra, ldc = X + 256;
-    view_embed_kernel<<<div_up(n, 128), 128, 0, st>>>(dirs + 3 * (size_t)s, f.multires_view, n, b.cin, ldc);
-    MP_LAUNCH_CHECK();
-    // features straight into the colour input block
-    MP_TRY(dense(h7, 256, nullptr, 0, f.imp_Wt[8] + 1, kHidden + 1, f.imp_b[8] + 1, b.cin + X, ldc, nullptr, n,
-                 nullptr, kHidden, kHidden, ACT_NONE, st));
-    MP_TRY(simt_colour(f, b.cin, ldc, n, nullptr, (h7 == b.H0) ? b.H1 : b.H0, h7, nullptr, rgb + 3 * (size_t)s, st));
-  }
-  return 0;
 }
 
 __global__ void colour_input_kernel(const float* __restrict__ pts, const float* __restrict__ nrm,

@@ -28,6 +28,7 @@
 #include "common.cuh"
 #include <vector>
 #include <mutex>
+#include <type_traits>
 #include <stdlib.h>
 
 namespace mp {
@@ -35,31 +36,41 @@ namespace mp {
 // ---------------------------------------------------------------------------------------------
 // program description
 // ---------------------------------------------------------------------------------------------
-enum { EPI_SOFTPLUS = 0, EPI_FEAT = 1, EPI_BWD = 2, EPI_RELU = 3 };
+// Step kinds: the epilogue of a layer step is compiled once per kind, so that every kind gets its own instruction
+// schedule and register allocation instead of one loop that tests the step descriptor in its body.
 enum {
-  F_SAVE_SIG = 1,      // store d softplus / dz to the sigma' scratch (forward, grad mode)
-  F_INJECT_EMB = 2,    // columns >= inj_col receive the input embedding (skip connection, networks.py:166)
-  F_SDF_DOT = 4,       // sdf = h7 . W8[0,:] + b8[0]
-  F_SEED_BWD = 8,      // after this step: A = W8[0,:] * sigma'_7 (start of the reverse sweep)
-  F_SKIP_GRAD = 16,    // reverse sweep: columns >= inj_col are d/d embed of the skip; park them, zero A there
-  F_FINAL_GRAD = 32,   // reverse sweep end: d sdf / d x -> normal ; then reload the features into A
-  F_EXTRA_IN = 64,     // colour layer 0: a fifth K-block carries the extra inputs ([x_c, n] or the view embedding): they are
+  K_SP_PLAIN = 0,      // softplus
+  K_SP_SAVE = 1,       // softplus; store d softplus / dz to the sigma' scratch (forward of the fused chain)
+  K_SP_SEED = 2,       // last SDF layer of the fused chain: park h7 in scratch (it returns as the colour net's input
+                       // after the reverse sweep), then A = W8[0,:] * sigma'_7 (start of the reverse sweep)
+  K_FEAT = 3,          // L8 features, written to feat (operator API)
+  K_BWD = 4,           // reverse sweep: g_{l-1} = (g_l * sigma'_l) . W_l
+  K_FINAL_GRAD = 5,    // reverse sweep end: d sdf / d x -> grad, normal ; then reload the features into A
+  K_RELU = 6           // colour layers
+};
+// Modifiers of a step within its kind
+enum {
+  F_INJECT_EMB = 1,    // columns >= inj_col receive the input embedding (skip connection, networks.py:166)
+  F_SDF_DOT = 2,       // sdf = h7 . W8[0,:] + b8[0]
+  F_SKIP_GRAD = 4,     // reverse sweep: columns >= inj_col are d/d embed of the skip; park them, zero A there
+  F_EXTRA_IN = 8,      // colour layer 0: a fifth K-block carries the extra inputs ([x_c, n] or the view embedding): they are
                        // staged into A's K-block 0 once its MMAs have drained, and accumulate into the same tile
-  F_RGB_OUT = 128,     // last colour layer: rgb = sigmoid(h . Wrgb^T + b)
-  F_FEAT_OUT = 256,    // write the fp32 features to feat_out (operator API)
-  F_STASH_FEAT = 512   // park the feature chunks in scratch (they return as the colour net's input after the reverse sweep)
+  F_RGB_OUT = 16       // last colour layer: rgb = sigmoid(h . Wrgb^T + b)
 };
 constexpr int kMaxSteps = 24;
 constexpr int kSlotBytes = 32768;          // 256 rows x 64 fp16
 constexpr int kRing = 3;
+// Weight slots of a field's blob.  The programs share their slots (the full program contains the forward one, which
+// contains the sdf-only one); the longest, the foreground's full program, has at most 2 * 2 (L0, E <= 96) +
+// 7 * 8 (L1..L7) + 8 (L8) + 8 * 8 (B7..B0) + 10 (folded colour layer 0) + 3 * 8 (colour layers 1..3) = 166.
+constexpr int kBlobSlots = 170;
 
 struct TcStep {
   int nk;               // 64-wide K chunks of A consumed by this layer (5 with F_EXTRA_IN: the last one re-uses K-block 0)
-  int epi;
-  int flags;
+  int kind;             // K_*
+  int flags;            // F_*
   int sig;              // sigma' scratch layer (save: forward, load: reverse) or -1
   const float* bias;    // [256] or nullptr
-  int ncols;            // output columns that carry data (the rest are padding)
   int slot_off;         // first weight slot of this step in the blob
   int sc;               // index of this layer's 2^-s in inv_scale[]
   int terms;            // split-precision terms of this step's products: 3 = A_hi.W_hi + A_lo.W_hi + A_hi.W_lo (default),
@@ -68,30 +79,18 @@ struct TcStep {
 
 struct TcProgram {
   int nsteps;
-  int slots_per_tile;
   TcStep step[kMaxSteps];
   const uint4* blob;     // weight slots in consumption order
   const float* inv_scale;   // [nsteps] 2^-s of each step's weights
   // network constants
-  int d_in, multires, E, inj_col, n_extra, col_n;   // col_n: width of the colour hidden layers
+  int d_in, multires, E, inj_col, n_extra;
   const float* w8row;    // W8[0,:]  [256]
   const float* b8;       // b8[0]
   const float* Wrgb;     // [3][256]
   const float* brgb;     // [3]
 };
 
-struct TcIO {
-  const float* x;        // [cap, d_in] canonical points (compact list)
-  const int* slot;       // [cap] output slot of each point or nullptr (identity)
-  const int* count;      // device count or nullptr (= cap)
-  int cap;
-  const float* jinv;     // [cap, 12] (3x3 row-major, padded to three float4) or nullptr
-  const float* extra;    // [cap, n_extra] extra colour inputs (background view embedding) or nullptr
-  float* sdf_out;        // scattered by slot
-  float* rgb_out;        // [slots,3]
-  float* nrm_out;        // [slots,3]
-  float* grad_out;       // [cap,3] dense or nullptr
-  float* feat_out;       // [cap,256] dense or nullptr
+struct TcIO : MlpCall {
   float rz;              // relative truncation loss of ONE tensor-core accumulation (see kRzPerMma)
   char* scratch;         // per-CTA scratch
   size_t scratch_per_cta;
@@ -328,17 +327,86 @@ __device__ __forceinline__ void softplus_fast_grad(float z, float& y, float& d) 
   d = big ? 1.f : u * r;
 }
 
+// Last step of the reverse sweep (K_FINAL_GRAD): d sdf / d x of the thread's two rows from B0's accumulator, written to
+// io.grad, and the normals, written to io.nrm and returned in nrm (the foreground colour net's extra inputs).
+// B0's output columns are permuted at pack time BY AXIS: columns [16 a, 16 a + 16) (a < d_in) hold every embedding index
+// that depends on x_a -- [x_a, sin(2^0 x_a), cos(2^0 x_a), sin(2^1 x_a), ...] (embedders.py:8-34) -- so the chain rule
+//   d sdf / d x_a = sum_k (g_k + skip_k) * d embed_k / d x_a
+// of one axis lives in column groups 2 a, 2 a + 1, reduced over the quad.  The skip gradient (parked at the F_SKIP_GRAD
+// step) and the partner sin / cos of each index (parked by the tile prologue) come from scratch.
+__device__ __forceinline__ void final_grad(const TcProgram& P, const TcIO& io, const float* acc, float isc, int q,
+                                           const float* ge, const float* emb, const int (&rowt)[2],
+                                           const bool (&valid)[2], const int (&pt)[2], const int (&slot)[2],
+                                           float (&nrm)[2][3]) {
+  const int d = P.d_in;
+  float gax[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+  const int nterm = 1 + 2 * P.multires;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (j < 2 * d) {
+      const int a = j >> 1;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int jj = (8 * j + 2 * q + (e & 1)) & 15;
+        if (jj < nterm) {
+          const int h = e >> 1;
+          // jj = 0: x_a itself; jj = 1 + 2 f: sin(2^f x_a); jj = 2 + 2 f: cos(2^f x_a)
+          const int fq = (jj - 1) >> 1;
+          const bool is_cos = ((jj - 1) & 1) != 0;
+          const int k = (jj == 0) ? a : d + 2 * fq * d + (is_cos ? d : 0) + a;
+          const float pg = ge[(size_t)k * 128 + rowt[h]];
+          const float tot = fmaf(acc[4 * j + e], isc, pg);     // through layer 0 + through the skip connection
+          float w = 1.f;
+          if (jj > 0) {
+            // partner: cos for a sin entry (+d), sin for a cos entry (-d)
+            const float pe = emb[(size_t)(is_cos ? k - d : k + d) * 128 + rowt[h]];
+            // d sin(2^f x) = 2^f cos(2^f x) ; d cos(2^f x) = -2^f sin(2^f x)
+            w = (float)(1 << fq) * (is_cos ? -pe : pe);
+          }
+          gax[h][a] = fmaf(w, tot, gax[h][a]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int a = 0; a < 4; ++a) gax[h][a] = quad_sum(gax[h][a]);
+    // normal = normalize(g . J^-1) (multiply.py:661), normalised again with eps 1e-6 (:606)
+    const float gx0 = gax[h][0], gx1 = d > 1 ? gax[h][1] : 0.f, gx2 = d > 2 ? gax[h][2] : 0.f;
+    if (q == 0 && io.grad && valid[h]) {
+      io.grad[3 * (size_t)pt[h]] = gx0;
+      io.grad[3 * (size_t)pt[h] + 1] = gx1;
+      io.grad[3 * (size_t)pt[h] + 2] = gx2;
+    }
+    float n0 = 0.f, n1 = 0.f, n2 = 0.f;
+    if (io.jinv && valid[h]) {
+      const float4* J4 = (const float4*)(io.jinv + 12 * (size_t)pt[h]);
+      const float4 ja = __ldg(J4), jb = __ldg(J4 + 1), jc = __ldg(J4 + 2);
+      float v0 = gx0 * ja.x + gx1 * ja.w + gx2 * jb.z;
+      float v1 = gx0 * ja.y + gx1 * jb.x + gx2 * jb.w;
+      float v2 = gx0 * ja.z + gx1 * jb.y + gx2 * jc.x;
+      float nr = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);     // multiply.py:661
+      const float inr = 1.f / nr;
+      v0 *= inr; v1 *= inr; v2 *= inr;
+      float n2r = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-6f);     // multiply.py:606
+      const float in2 = 1.f / n2r;
+      n0 = v0 * in2; n1 = v1 * in2; n2 = v2 * in2;
+      if (q == 0 && io.nrm) {
+        io.nrm[3 * (size_t)slot[h]] = n0;
+        io.nrm[3 * (size_t)slot[h] + 1] = n1;
+        io.nrm[3 * (size_t)slot[h] + 2] = n2;
+      }
+    }
+    nrm[h][0] = n0;
+    nrm[h][1] = n1;
+    nrm[h][2] = n2;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
-// Step kinds: the epilogue of a layer step is compiled once per kind (compile-time tag), so that every kind gets its own
-// instruction schedule and register allocation instead of one loop that tests the step descriptor in its body.
-enum { K_SP_PLAIN = 0, K_SP_SAVE = 1, K_SP_SEED = 2, K_FEAT = 3, K_BWD = 4, K_RELU = 5 };
-template <int K>
-struct KTag {
-  static constexpr int value = K;
-};
-
 __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
                                                                const __grid_constant__ TcIO io) {
   extern __shared__ uint8_t smem_raw[];
@@ -446,12 +514,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         for (int a = 0; a < d; ++a)
 #pragma unroll
           for (int h = 0; h < 2; ++h) emb[(size_t)a * 128 + rowt[h]] = x[h][a];
-      if (io.extra) {
+      if (io.dirs) {
         // background: embedding of the view direction (n_extra = 3 + 6 * frequencies values), same split
         float dv[2][3];
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          for (int a = 0; a < 3; ++a) dv[h][a] = valid[h] ? io.extra[(size_t)pt[h] * 3 + a] : 0.f;
+          for (int a = 0; a < 3; ++a) dv[h][a] = valid[h] ? io.dirs[(size_t)pt[h] * 3 + a] : 0.f;
         const int nvp = (P.n_extra - 3) / 2;
         for (int pi = q; pi < nvp; pi += 4) {
           const int f = pi / 3, a = pi - f * 3;
@@ -495,9 +563,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       // one step earlier it gains less: the block competes longer with the rest of the stash.)
       if (t == 0) {
         char* ws = io.scratch + (size_t)blockIdx.x * io.scratch_per_cta;
-        if (st.epi == EPI_BWD && st.sig >= 0)
+        if (st.kind == K_BWD && st.sig >= 0)
           prefetch_l2(ws + (((size_t)st.sig * kConsumers + g) * 32 * 128) * 16, 32 * 128 * 16);
-        if (st.flags & F_FINAL_GRAD) prefetch_l2(ws + kSigBytes + (size_t)g * 32 * 128 * 16, 32 * 128 * 16);
+        if (st.kind == K_FINAL_GRAD) prefetch_l2(ws + kSigBytes + (size_t)g * 32 * 128 * 16, 32 * 128 * 16);
       }
 
       // ---------------- MMAs: acc = A . W^T over st.nk K-blocks ----------------
@@ -538,7 +606,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
               float xv[8];
 #pragma unroll
               for (int j = 0; j < 8; ++j) xv[j] = 0.f;
-              if (io.extra) {
+              if (io.dirs) {
 #pragma unroll
                 for (int j = 0; j < 8; ++j)
                   if (e0 + j < P.n_extra) xv[j] = ge[(size_t)(e0 + j) * 128 + rowt[h]];
@@ -592,84 +660,15 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
           }
         }
       };
-      if (st.flags & F_FINAL_GRAD) {
-        // ---- last step of the reverse sweep ----
-        // B0's output columns are permuted at pack time BY AXIS: columns [16 a, 16 a + 16) (a < d_in) hold every
-        // embedding index that depends on x_a -- [x_a, sin(2^0 x_a), cos(2^0 x_a), sin(2^1 x_a), ...]
-        // (embedders.py:8-34) -- so the chain rule
-        //   d sdf / d x_a = sum_k (g_k + skip_k) * d embed_k / d x_a
-        // of one axis lives in column groups 2 a, 2 a + 1, reduced over the quad.  The skip gradient (parked at the
-        // F_SKIP_GRAD step) and the partner sin / cos of each index (parked by the tile prologue) come from scratch.
-        float gax[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-        const int nterm = 1 + 2 * P.multires;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (j < 2 * d) {
-            const int a = j >> 1;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int jj = (8 * j + 2 * q + (e & 1)) & 15;
-              if (jj < nterm) {
-                const int h = e >> 1;
-                // jj = 0: x_a itself; jj = 1 + 2 f: sin(2^f x_a); jj = 2 + 2 f: cos(2^f x_a)
-                const int fq = (jj - 1) >> 1;
-                const bool is_cos = ((jj - 1) & 1) != 0;
-                const int k = (jj == 0) ? a : d + 2 * fq * d + (is_cos ? d : 0) + a;
-                const float pg = ge[(size_t)k * 128 + rowt[h]];
-                const float tot = fmaf(acc[4 * j + e], isc, pg);     // through layer 0 + through the skip connection
-                float w = 1.f;
-                if (jj > 0) {
-                  // partner: cos for a sin entry (+d), sin for a cos entry (-d)
-                  const float pe = emb[(size_t)(is_cos ? k - d : k + d) * 128 + rowt[h]];
-                  // d sin(2^f x) = 2^f cos(2^f x) ; d cos(2^f x) = -2^f sin(2^f x)
-                  w = (float)(1 << fq) * (is_cos ? -pe : pe);
-                }
-                gax[h][a] = fmaf(w, tot, gax[h][a]);
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int a = 0; a < 4; ++a) gax[h][a] = quad_sum(gax[h][a]);
-          // normal = normalize(g . J^-1) (multiply.py:661), normalised again with eps 1e-6 (:606)
-          const float gx0 = gax[h][0], gx1 = d > 1 ? gax[h][1] : 0.f, gx2 = d > 2 ? gax[h][2] : 0.f;
-          if (q == 0 && io.grad_out && valid[h]) {
-            io.grad_out[3 * (size_t)pt[h]] = gx0;
-            io.grad_out[3 * (size_t)pt[h] + 1] = gx1;
-            io.grad_out[3 * (size_t)pt[h] + 2] = gx2;
-          }
-          float n0 = 0.f, n1 = 0.f, n2 = 0.f;
-          if (io.jinv && valid[h]) {
-            const float4* J4 = (const float4*)(io.jinv + 12 * (size_t)pt[h]);
-            const float4 ja = __ldg(J4), jb = __ldg(J4 + 1), jc = __ldg(J4 + 2);
-            float v0 = gx0 * ja.x + gx1 * ja.w + gx2 * jb.z;
-            float v1 = gx0 * ja.y + gx1 * jb.x + gx2 * jb.w;
-            float v2 = gx0 * ja.z + gx1 * jb.y + gx2 * jc.x;
-            float nr = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);     // multiply.py:661
-            const float inr = 1.f / nr;
-            v0 *= inr; v1 *= inr; v2 *= inr;
-            float n2r = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-6f);     // multiply.py:606
-            const float in2 = 1.f / n2r;
-            n0 = v0 * in2; n1 = v1 * in2; n2 = v2 * in2;
-            if (q == 0 && io.nrm_out) {
-              io.nrm_out[3 * (size_t)slot[h]] = n0;
-              io.nrm_out[3 * (size_t)slot[h] + 1] = n1;
-              io.nrm_out[3 * (size_t)slot[h] + 2] = n2;
-            }
-          }
-          nrm[h][0] = n0;
-          nrm[h][1] = n1;
-          nrm[h][2] = n2;
-        }
+      if (st.kind == K_FINAL_GRAD) {
+        final_grad(P, io, acc, isc, q, ge, emb, rowt, valid, pt, slot, nrm);
         // the MMAs of the reverse sweep are done with A: the features return as the colour net's input
         if (s + 1 < P.nsteps) reload_features();
         continue;
       }
 
-      auto run_epi = [&](auto ktag) {
-        constexpr int KIND = decltype(ktag)::value;
+      auto run_epi = [&](auto kind) {
+        constexpr int KIND = decltype(kind)::value;
         float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};     // sdf / rgb partial dots of the two rows
 #pragma unroll
         for (int jp = 0; jp < 16; ++jp) {
@@ -722,10 +721,10 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
             } else if constexpr (KIND == K_FEAT) {
 #pragma unroll
               for (int e = 0; e < 4; ++e) u[e] = fmaf(u[e], isc, b[e & 1]);
-              if ((st.flags & F_FEAT_OUT) && io.feat_out) {
+              if (io.feat) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
-                  if (valid[h]) *(float2*)(io.feat_out + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
+                  if (valid[h]) *(float2*)(io.feat + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
               }
             } else if constexpr (KIND == K_BWD) {
               float4 s4 = make_float4(1.f, 1.f, 1.f, 1.f);
@@ -765,12 +764,10 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
             }
           }
           if constexpr (KIND == K_SP_SEED) {
-            if (st.flags & F_STASH_FEAT) {
-              uint4 fh, fl;
-              split8(yv, fh, fl);
-              st_stream(&fsc[(size_t)jp * 128 + t], fh);
-              st_stream(&fsc[(size_t)(16 + jp) * 128 + t], fl);
-            }
+            uint4 fh, fl;
+            split8(yv, fh, fl);
+            st_stream(&fsc[(size_t)jp * 128 + t], fh);
+            st_stream(&fsc[(size_t)(16 + jp) * 128 + t], fl);
           }
           // activations of these 16 columns -> A (fp16 hi/lo, swizzled) unless this is the last layer
           bool to_a = true;
@@ -782,7 +779,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const float sdot = quad_sum(dot[h][0]);
-            if (q == 0 && valid[h] && io.sdf_out) io.sdf_out[slot[h]] = __ldg(P.b8) + sdot;
+            if (q == 0 && valid[h] && io.sdf) io.sdf[slot[h]] = __ldg(P.b8) + sdot;
           }
         }
         if constexpr (KIND == K_RELU) {
@@ -792,25 +789,19 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
 #pragma unroll
               for (int k = 0; k < 3; ++k) {
                 const float z = __ldg(P.brgb + k) + quad_sum(dot[h][k]);
-                if (q == 0 && valid[h] && io.rgb_out) io.rgb_out[3 * (size_t)slot[h] + k] = 1.f / (1.f + __expf(-z));
+                if (q == 0 && valid[h] && io.rgb) io.rgb[3 * (size_t)slot[h] + k] = 1.f / (1.f + __expf(-z));
               }
             }
           }
         }
       };
-      if (st.epi == EPI_SOFTPLUS) {
-        if ((st.flags & (F_SAVE_SIG | F_SEED_BWD)) == (F_SAVE_SIG | F_SEED_BWD))
-          run_epi(KTag<K_SP_SEED>{});
-        else if (st.flags & F_SAVE_SIG)
-          run_epi(KTag<K_SP_SAVE>{});
-        else
-          run_epi(KTag<K_SP_PLAIN>{});
-      } else if (st.epi == EPI_FEAT) {
-        run_epi(KTag<K_FEAT>{});
-      } else if (st.epi == EPI_BWD) {
-        run_epi(KTag<K_BWD>{});
-      } else {
-        run_epi(KTag<K_RELU>{});
+      switch (st.kind) {
+        case K_SP_PLAIN: run_epi(std::integral_constant<int, K_SP_PLAIN>{}); break;
+        case K_SP_SAVE: run_epi(std::integral_constant<int, K_SP_SAVE>{}); break;
+        case K_SP_SEED: run_epi(std::integral_constant<int, K_SP_SEED>{}); break;
+        case K_FEAT: run_epi(std::integral_constant<int, K_FEAT>{}); break;
+        case K_BWD: run_epi(std::integral_constant<int, K_BWD>{}); break;
+        default: run_epi(std::integral_constant<int, K_RELU>{}); break;
       }
       // the skip gradient parked in `ge` is read by other lanes of the quad at the final-gradient step
       if (st.flags & F_SKIP_GRAD) __threadfence_block();
@@ -828,7 +819,8 @@ struct TcBlob {
   bool has_full;
 };
 
-__global__ void absmax_kernel(const float* __restrict__ W, int n, float* __restrict__ out) {
+// inv_scale[0] = 2^-s of the weights W[0, n)
+__global__ void absmax_kernel(const float* __restrict__ W, int n, float* __restrict__ inv_scale) {
   __shared__ float s[256];
   float m = 0.f;
   for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(W[i]));
@@ -844,8 +836,7 @@ __global__ void absmax_kernel(const float* __restrict__ W, int n, float* __restr
     int ex = 0;
     if (mx > 0.f) frexpf(mx, &ex);       // mx = f * 2^ex, f in [0.5,1)
     float sc = ldexpf(1.f, 14 - ex);
-    out[0] = sc;
-    out[1] = 1.f / sc;
+    inv_scale[0] = 1.f / sc;
   }
 }
 
@@ -853,7 +844,7 @@ __global__ void absmax_kernel(const float* __restrict__ W, int n, float* __restr
 //   transposed == 0 : B[n][k] = W[(n_off + n) * ld + k_off + kc*64 + k]   (n < n_valid, kk < k_valid)
 //   transposed == 1 : B[n][k] = W[(k_off + kc*64 + k) * ld + n_off + n]
 __global__ void pack_slot_kernel(const float* __restrict__ W, int ld, int transposed, int n_off, int k_off,
-                                 int n_valid, int k_valid, int kc, const float* __restrict__ scale,
+                                 int n_valid, int k_valid, int kc, const float* __restrict__ inv_scale,
                                  uint8_t* __restrict__ dst_hi, uint8_t* __restrict__ dst_lo, int perm16) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= 256 * 64) return;
@@ -875,7 +866,7 @@ __global__ void pack_slot_kernel(const float* __restrict__ W, int ld, int transp
   float w = 0.f;
   if (ns < n_valid && kk < k_valid)
     w = transposed ? W[(size_t)(k_off + kk) * ld + n_off + ns] : W[(size_t)(n_off + ns) * ld + k_off + kk];
-  w *= scale[0];
+  w = __fdiv_rn(w, inv_scale[0]);     // = w * 2^s exactly rounded, as inv_scale is a power of two
   __half h = __float2half_rn(w);
   __half l = __float2half_rn(w - __half2float(h));
   uint32_t off = (uint32_t)(n * 128 + ((((k >> 3) ^ (n & 7))) << 4) + (k & 7) * 2);
@@ -923,46 +914,40 @@ __global__ void fill_extra_cols_kernel(const float* __restrict__ Wt, int n_out, 
   M[(size_t)n * ldm + 256 + e] = (n < n_out && e < n_extra) ? Wt[(size_t)e * n_out + n] : 0.f;
 }
 
-size_t tc_pack_bytes() {
-  // sdf (58) + fwd (66) + full (162) slots ... share: full program contains fwd which contains sdf
-  return (size_t)170 * kSlotBytes + (1 << 20);
-}
+size_t tc_pack_bytes() { return (size_t)kBlobSlots * kSlotBytes + (1 << 20); }
 
 struct PackCtx {
   cudaStream_t st;
   uint8_t* blob;
   int nslots;
-  int nlayers;        // packed layers so far (index into scales / inv_scale)
-  float* scales;      // [kMaxLayers][2] (scale, inv)
+  int nlayers;        // packed layers so far (index into inv_scale)
   float* inv_scale;   // [kMaxSteps]
 };
 
 // One layer step: its descriptor, the 2^s scale of W and nk K-chunks of hi/lo weight slots holding B[n][k] = W[n_off + n][k]
-// (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere.  The n_valid output columns carry data.
-static int pack_layer(PackCtx& c, TcStep& stp, int epi, int flags, int sig, const float* bias, const float* W, int ld,
+// (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere.
+static int pack_layer(PackCtx& c, TcStep& stp, int kind, int flags, int sig, const float* bias, const float* W, int ld,
                       int transposed, int n_off, int n_valid, int k_valid, int nk, int total_elems, int perm16 = 0) {
+  MP_REQUIRE(c.nslots + 2 * nk <= kBlobSlots, "tc_pack: slot budget exceeded (%d)", c.nslots + 2 * nk);
   const int layer = c.nlayers++;
   stp.nk = nk;
-  stp.epi = epi;
+  stp.kind = kind;
   stp.flags = flags;
   stp.sig = sig;
   stp.bias = bias;
-  stp.ncols = n_valid;
   stp.slot_off = c.nslots;
   stp.sc = layer;
   stp.terms = 3;
-  absmax_kernel<<<1, 256, 0, c.st>>>(W, total_elems, c.scales + 2 * layer);
+  absmax_kernel<<<1, 256, 0, c.st>>>(W, total_elems, c.inv_scale + layer);
   MP_LAUNCH_CHECK();
   for (int kc = 0; kc < nk; ++kc) {
     uint8_t* hi = c.blob + (size_t)c.nslots * kSlotBytes;
     uint8_t* lo = hi + kSlotBytes;
-    pack_slot_kernel<<<64, 256, 0, c.st>>>(W, ld, transposed, n_off, 0, n_valid, k_valid, kc, c.scales + 2 * layer, hi,
+    pack_slot_kernel<<<64, 256, 0, c.st>>>(W, ld, transposed, n_off, 0, n_valid, k_valid, kc, c.inv_scale + layer, hi,
                                            lo, perm16);
     MP_LAUNCH_CHECK();
     c.nslots += 2;
   }
-  copy_strided_kernel<<<1, 1, 0, c.st>>>(c.scales + 2 * layer + 1, 1, 1, c.inv_scale + layer);
-  MP_LAUNCH_CHECK();
   return 0;
 }
 
@@ -971,7 +956,9 @@ void tc_free(Field& f) {
   f.tc = nullptr;
 }
 
-// The three programs, one pack_layer per step (epilogue, flags, sigma' layer, bias, then the weight source).
+// The three programs, one pack_layer per step (kind, flags, sigma' layer, bias, then the weight source).  L0..L7 are
+// packed once and shared: the sdf-only, forward and background programs run them as plain softplus steps, the fused
+// foreground program saves sigma' and seeds the reverse sweep.
 int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   TcBlob* tb = new TcBlob();
   memset(tb, 0, sizeof(*tb));
@@ -981,14 +968,13 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   c.st = st;
   c.nslots = 0;
   c.nlayers = 0;
-  c.blob = (uint8_t*)a.take<uint4>((size_t)170 * kSlotBytes / 16);
-  c.scales = a.take<float>(2 * 32);
+  c.blob = (uint8_t*)a.take<uint4>((size_t)kBlobSlots * kSlotBytes / 16);
   c.inv_scale = a.take<float>(32);
   float* w8row = a.take<float>(256);
   float* Wrgb = a.take<float>(3 * 256);
   float* b8feat = a.take<float>(256);      // b8[1:], 16-byte aligned copy (the epilogue loads float4)
   MP_REQUIRE(a.ok, "tc_pack: storage too small");
-  MP_CHECK_CUDA(cudaMemsetAsync(c.blob, 0, (size_t)170 * kSlotBytes, st));
+  MP_CHECK_CUDA(cudaMemsetAsync(c.blob, 0, (size_t)kBlobSlots * kSlotBytes, st));
   TcProgram P;
   memset(&P, 0, sizeof(P));
   P.blob = (const uint4*)c.blob;
@@ -1006,27 +992,19 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   copy_strided_kernel<<<1, 256, 0, st>>>(f.imp_b[8] + 1, 1, 256, b8feat);
   MP_LAUNCH_CHECK();
   int s = 0;
-  // ---- forward L0..L7 ----
+  // ---- forward L0..L7: the sdf-only program ----
   for (int l = 0; l < 8; ++l) {
     const int in = f.imp_in[l], out = f.imp_out[l];
-    const int flags = F_SAVE_SIG | ((l == f.skip_layer - 1) ? F_INJECT_EMB : 0) | ((l == 7) ? F_SDF_DOT : 0);
-    MP_TRY(pack_layer(c, P.step[s++], EPI_SOFTPLUS, flags, l, (l == 0) ? f.imp_b0_eff : f.imp_b[l], f.imp_W[l], in, 0,
+    const int flags = ((l == f.skip_layer - 1) ? F_INJECT_EMB : 0) | ((l == 7) ? F_SDF_DOT : 0);
+    MP_TRY(pack_layer(c, P.step[s++], K_SP_PLAIN, flags, l, (l == 0) ? f.imp_b0_eff : f.imp_b[l], f.imp_W[l], in, 0,
                       0, out, (l == 0) ? E : in, (l == 0) ? (E + 63) / 64 : 4, out * in));
   }
-  // sdf-only program: the first 8 steps, no sigma' stash
+  P.nsteps = s;
   tb->sdf_prog = P;
-  tb->sdf_prog.nsteps = 8;
-  tb->sdf_prog.slots_per_tile = c.nslots;
-  for (int i = 0; i < 8; ++i) tb->sdf_prog.step[i].flags &= ~F_SAVE_SIG;
   // ---- L8 features (operator API: sdf + features) ----
-  {
-    TcProgram F = P;
-    MP_TRY(pack_layer(c, F.step[8], EPI_FEAT, F_FEAT_OUT, -1, b8feat, f.imp_W[8], 256, 0, 1, 256, 256, 4, 257 * 256));
-    F.nsteps = 9;
-    F.slots_per_tile = c.nslots;
-    for (int i = 0; i < 8; ++i) F.step[i].flags &= ~F_SAVE_SIG;
-    tb->fwd_prog = F;
-  }
+  tb->fwd_prog = P;
+  MP_TRY(pack_layer(c, tb->fwd_prog.step[s], K_FEAT, 0, -1, b8feat, f.imp_W[8], 256, 0, 1, 256, 256, 4, 257 * 256));
+  tb->fwd_prog.nsteps = s + 1;
   const bool fg_chain = (f.ren_mode == 0) && (f.n_ren == 5) && f.ren_out[0] == 256;
   const bool bg_chain = (f.ren_mode == 1) && (f.n_ren == 2) && f.ren_out[0] <= 256 && f.ren_extra <= 27;
   tb->has_full = fg_chain || bg_chain;
@@ -1053,45 +1031,42 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
   if (bg_chain) {
     // background: folded colour layer 0 (view embedding + h7 -> 128, ReLU) and the rgb head (multiply.py:531)
     const int o0 = f.ren_out[0];
-    MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, F_EXTRA_IN | F_RGB_OUT, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, o0, kLdM, 5,
+    MP_TRY(pack_layer(c, P.step[s++], K_RELU, F_EXTRA_IN | F_RGB_OUT, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, o0, kLdM, 5,
                       256 * kLdM));
     pad_rows_kernel<<<div_up(3 * 256, 256), 256, 0, st>>>(f.ren_W[1], o0, 3, o0, Wrgb);
     MP_LAUNCH_CHECK();
     P.brgb = f.ren_b[1];
     P.nsteps = s;
-    P.slots_per_tile = c.nslots;
     tb->full_prog = P;
-    for (int i = 0; i < 8; ++i) tb->full_prog.step[i].flags &= ~F_SAVE_SIG;   // no reverse sweep in the background
   }
   if (fg_chain) {
-    // h7 is parked (it returns as the folded colour layer's input) and the reverse sweep starts right after L7
-    P.step[s - 1].flags |= F_SEED_BWD | F_STASH_FEAT;
+    // L0..L7 save sigma' for the reverse sweep, which starts right after L7; h7 is parked (it returns as the folded
+    // colour layer's input)
+    for (int l = 0; l < 8; ++l) P.step[l].kind = (l == 7) ? K_SP_SEED : K_SP_SAVE;
     // ---- reverse sweep B7..B1: g_{l-1} = (g_l * sigma'_l) . W_l ----
     for (int l = 7; l >= 1; --l) {
       const int in = f.imp_in[l], out = f.imp_out[l];
       // B[n][k] = W_l[k][n] : n over in (valid in), k over out (valid out)
-      MP_TRY(pack_layer(c, P.step[s++], EPI_BWD, (l == f.skip_layer) ? F_SKIP_GRAD : 0, l - 1, nullptr, f.imp_W[l], in, 1,
+      MP_TRY(pack_layer(c, P.step[s++], K_BWD, (l == f.skip_layer) ? F_SKIP_GRAD : 0, l - 1, nullptr, f.imp_W[l], in, 1,
                         0, in, out, 4, out * in));
     }
     // ---- B0: d/d embed = (g_0 * sigma'_0) . W0[:, :E] ----
     MP_REQUIRE(f.d_in <= 4 && 1 + 2 * f.multires <= 14,
                "tc_pack: the final-gradient step keeps 1 + 2 * multires <= 14 embedding columns per axis");
-    MP_TRY(pack_layer(c, P.step[s++], EPI_BWD, F_FINAL_GRAD, -1, nullptr, f.imp_W[0], f.imp_in[0], 1, 0, E, 256, 4,
+    MP_TRY(pack_layer(c, P.step[s++], K_FINAL_GRAD, 0, -1, nullptr, f.imp_W[0], f.imp_in[0], 1, 0, E, 256, 4,
                       256 * f.imp_in[0], /*perm16=*/f.d_in));
     // ---- colour net: folded layer 0, then layers 1..3 ----
-    MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, F_EXTRA_IN, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, 256, kLdM, 5,
+    MP_TRY(pack_layer(c, P.step[s++], K_RELU, F_EXTRA_IN, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, 256, kLdM, 5,
                       256 * kLdM));
     for (int l = 1; l < 4; ++l)
-      MP_TRY(pack_layer(c, P.step[s++], EPI_RELU, (l == 3) ? F_RGB_OUT : 0, -1, f.ren_b[l], f.ren_W[l], 256, 0, 0, 256,
+      MP_TRY(pack_layer(c, P.step[s++], K_RELU, (l == 3) ? F_RGB_OUT : 0, -1, f.ren_b[l], f.ren_W[l], 256, 0, 0, 256,
                         256, 4, 256 * 256));
     // rgb head [3][256]
     MP_CHECK_CUDA(cudaMemcpyAsync(Wrgb, f.ren_W[4], (size_t)3 * 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     P.brgb = f.ren_b[4];
     P.nsteps = s;
-    P.slots_per_tile = c.nslots;
     tb->full_prog = P;
   }
-  MP_REQUIRE(c.nslots <= 170, "tc_pack: slot budget exceeded (%d)", c.nslots);
   return 0;
 }
 
@@ -1104,7 +1079,7 @@ size_t tc_workspace_bytes(int N) { return (size_t)sm_count() * kScratchPerCta + 
 // launching stream + an async copy of the device-side point count into pinned memory
 struct ProfEntry {
   cudaEvent_t e0, e1;
-  int kind;        // 0 sdf-only, 1 forward (sdf+features), 2 full shade, 3 background
+  int kind;        // MlpProg: 0 sdf-only, 1 forward (sdf+features), 2 full shade, 3 background
   int cap;
   int* host_count; // pinned
 };
@@ -1174,12 +1149,12 @@ std::atomic<int> g_precision{0};
 // measures the per-sample SDF / gradient / normal error against the fp64 evaluation of the same weights.
 constexpr float kRzPerMma = 1.72e-8f;
 
-static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cudaStream_t st, int kind) {
+static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cudaStream_t st, MlpProg kind) {
   TcProgram P = P0;
   {
     const int mode = g_precision.load();
     for (int s = 0; s < P.nsteps; ++s)
-      P.step[s].terms = (mode == 2 || (mode == 1 && P.step[s].epi == EPI_RELU)) ? 1 : 3;
+      P.step[s].terms = (mode == 2 || (mode == 1 && P.step[s].kind == K_RELU)) ? 1 : 3;
   }
   int grid = sm_count();
   {
@@ -1221,7 +1196,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
   if (prof) {
     MP_CHECK_CUDA(cudaEventCreate(&pe.e0));
     MP_CHECK_CUDA(cudaEventCreate(&pe.e1));
-    pe.kind = kind;
+    pe.kind = (int)kind;
     pe.cap = io.cap;
     pe.host_count = nullptr;
     if (io.count) {
@@ -1239,64 +1214,32 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
   return 0;
 }
 
-int tc_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+int tc_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st) {
   MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
-  TcBlob* tb = (TcBlob*)f.tc;
-  TcIO io;
-  memset(&io, 0, sizeof(io));
-  io.x = xc_list;
-  io.slot = slot_list;
-  io.count = count_dev;
-  io.cap = cap;
-  io.sdf_out = sdf_out;
-  return tc_launch(tb->sdf_prog, io, ws, ws_bytes, st, 0);
-}
-
-int tc_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                  const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                  float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
-  TcBlob* tb = (TcBlob*)f.tc;
-  TcIO io;
-  memset(&io, 0, sizeof(io));
-  io.x = xc_list;
-  io.slot = slot_list;
-  io.count = count_dev;
-  io.cap = cap;
-  io.jinv = Jinv_list;
-  io.sdf_out = sdf_out;
-  io.rgb_out = rgb_out;
-  io.nrm_out = normal_out;
-  io.grad_out = grad_out;
-  io.feat_out = feat_out;
-  if (!Jinv_list && !grad_out) return tc_launch(tb->fwd_prog, io, ws, ws_bytes, st, 1);
-  MP_REQUIRE(tb->has_full, "tensor-core engine: this field has no fused shading program");
-  if (feat_out) {
+  const TcBlob& tb = *(const TcBlob*)f.tc;
+  const MlpProg prog = mlp_prog(c);
+  TcIO io{};
+  static_cast<MlpCall&>(io) = c;
+  if (prog == MlpProg::kSdf) return tc_launch(tb.sdf_prog, io, ws, ws_bytes, st, prog);
+  if (prog == MlpProg::kForward) return tc_launch(tb.fwd_prog, io, ws, ws_bytes, st, prog);
+  if (prog == MlpProg::kBg) {
+    MP_REQUIRE(tb.has_full && f.ren_mode == 1, "tensor-core engine: not a background field");
+    return tc_launch(tb.full_prog, io, ws, ws_bytes, st, prog);
+  }
+  MP_REQUIRE(tb.has_full, "tensor-core engine: this field has no fused shading program");
+  if (c.feat) {
     // the fused program folds L8's feature rows into the colour layer and never materialises the features: the
     // forward program writes them (operator API only; the render passes no feature output)
-    TcIO fio = io;
-    fio.jinv = nullptr;
-    fio.sdf_out = fio.rgb_out = fio.nrm_out = fio.grad_out = nullptr;
-    MP_TRY(tc_launch(tb->fwd_prog, fio, ws, ws_bytes, st, 1));
-    io.feat_out = nullptr;
+    TcIO fio{};
+    fio.x = c.x;
+    fio.slot = c.slot;
+    fio.count = c.count;
+    fio.cap = c.cap;
+    fio.feat = c.feat;
+    MP_TRY(tc_launch(tb.fwd_prog, fio, ws, ws_bytes, st, MlpProg::kForward));
+    io.feat = nullptr;
   }
-  return tc_launch(tb->full_prog, io, ws, ws_bytes, st, 2);
-}
-
-int tc_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-          size_t ws_bytes, cudaStream_t st) {
-  MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
-  TcBlob* tb = (TcBlob*)f.tc;
-  MP_REQUIRE(tb->has_full && f.ren_mode == 1, "tensor-core engine: not a background field");
-  TcIO io;
-  memset(&io, 0, sizeof(io));
-  io.x = pts;
-  io.cap = N;
-  io.extra = dirs;
-  io.sdf_out = sdf;
-  io.rgb_out = rgb;
-  return tc_launch(tb->full_prog, io, ws, ws_bytes, st, 3);
+  return tc_launch(tb.full_prog, io, ws, ws_bytes, st, prog);
 }
 
 }  // namespace mp

@@ -14,26 +14,9 @@ size_t field_ws_bytes(int N) {
   return a > b ? a : b;
 }
 
-int field_sdf_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                   float* sdf_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (cap <= 0) return 0;
-  if (g_engine == 1) return tc_sdf_list(f, xc_list, slot_list, count_dev, cap, sdf_out, ws, ws_bytes, st);
-  return simt_sdf_list(f, xc_list, slot_list, count_dev, cap, sdf_out, ws, ws_bytes, st);
-}
-int field_shade_list(const Field& f, const float* xc_list, const int* slot_list, const int* count_dev, int cap,
-                     const float* Jinv_list, float* sdf_out, float* rgb_out, float* normal_out, float* grad_out,
-                     float* feat_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (cap <= 0) return 0;
-  if (g_engine == 1)
-    return tc_shade_list(f, xc_list, slot_list, count_dev, cap, Jinv_list, sdf_out, rgb_out, normal_out, grad_out,
-                         feat_out, ws, ws_bytes, st);
-  return simt_shade_list(f, xc_list, slot_list, count_dev, cap, Jinv_list, sdf_out, rgb_out, normal_out, grad_out,
-                         feat_out, ws, ws_bytes, st);
-}
-int field_bg(const Field& f, const float* pts, const float* dirs, int N, float* sdf, float* rgb, void* ws,
-             size_t ws_bytes, cudaStream_t st) {
-  if (g_engine == 1) return tc_bg(f, pts, dirs, N, sdf, rgb, ws, ws_bytes, st);
-  return simt_bg(f, pts, dirs, N, sdf, rgb, ws, ws_bytes, st);
+int field_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st) {
+  if (c.cap <= 0) return 0;
+  return g_engine == 1 ? tc_run(f, c, ws, ws_bytes, st) : simt_run(f, c, ws, ws_bytes, st);
 }
 
 __global__ void gather_rays_kernel(const float* __restrict__ dirs, const float* __restrict__ cam,
@@ -215,18 +198,25 @@ int mp_implicit_forward(mp_net_t* f, const float* x, int N, float* sdf, float* f
                         size_t workspace_bytes, void* stream) {
   MP_REQUIRE(f && x, "mp_implicit_forward: null argument");
   if (N <= 0) return 0;      // networks.py:131
-  cudaStream_t st = (cudaStream_t)stream;
-  if (feat == nullptr) return mp::field_sdf_list(f->f, x, nullptr, nullptr, N, sdf, workspace, workspace_bytes, st);
-  return mp::field_shade_list(f->f, x, nullptr, nullptr, N, nullptr, sdf, nullptr, nullptr, nullptr, feat, workspace,
-                              workspace_bytes, st);
+  mp::MlpCall c{};
+  c.x = x;
+  c.cap = N;
+  c.sdf = sdf;
+  c.feat = feat;
+  return mp::field_run(f->f, c, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mp_implicit_forward_grad(mp_net_t* f, const float* x, int N, float* sdf, float* feat, float* grad,
                              void* workspace, size_t workspace_bytes, void* stream) {
   MP_REQUIRE(f && x && grad, "mp_implicit_forward_grad: null argument");
   if (N <= 0) return 0;
-  return mp::field_shade_list(f->f, x, nullptr, nullptr, N, nullptr, sdf, nullptr, nullptr, grad, feat, workspace,
-                              workspace_bytes, (cudaStream_t)stream);
+  mp::MlpCall c{};
+  c.x = x;
+  c.cap = N;
+  c.sdf = sdf;
+  c.grad = grad;
+  c.feat = feat;
+  return mp::field_run(f->f, c, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mp_render_forward(mp_net_t* f, const float* points, const float* normals, const float* feat, int N, float* rgb,
@@ -243,7 +233,13 @@ int mp_bg_nets_forward(mp_net_t* bg_field, const float* pts, const float* view_d
   MP_REQUIRE(bg_field && pts && view_dirs && rgb, "mp_bg_nets_forward: null argument");
   MP_REQUIRE(bg_field->f.is_bg, "mp_bg_nets_forward: not a background field");
   if (N <= 0) return 0;
-  return mp::field_bg(bg_field->f, pts, view_dirs, N, sdf, rgb, workspace, workspace_bytes, (cudaStream_t)stream);
+  mp::MlpCall c{};
+  c.x = pts;
+  c.cap = N;
+  c.dirs = view_dirs;
+  c.sdf = sdf;
+  c.rgb = rgb;
+  return mp::field_run(bg_field->f, c, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t mp_sdf_grid_workspace_bytes(int res) {
@@ -270,7 +266,11 @@ int mp_sdf_grid(mp_net_t* field, const float* center_host, float extent, float p
     mp::grid_points_kernel<<<mp::div_up(cnt, 256), 256, 0, st>>>(center_host[0], center_host[1], center_host[2], extent,
                                                                   pad, res, s0, cnt, pts);
     MP_LAUNCH_CHECK();
-    MP_TRY(mp::field_sdf_list(field->f, pts, nullptr, nullptr, cnt, values + s0, mws, mb, st));
+    mp::MlpCall c{};
+    c.x = pts;
+    c.cap = cnt;
+    c.sdf = values + s0;
+    MP_TRY(mp::field_run(field->f, c, mws, mb, st));
   }
   return 0;
 }
@@ -286,11 +286,12 @@ int mp_sdf_with_deformer(mp_body_t* body, mp_net_t* field, const float* x, int N
   void* mws = a.take<char>(mb);
   MP_REQUIRE(a.ok, "mp_sdf_with_deformer: workspace too small (%zu needed)", a.off);
   MP_TRY(mp_deform_inverse(body, x, N, x_c, outl, 1, stream));
-  if (feat)
-    MP_TRY(mp::field_shade_list(field->f, x_c, nullptr, nullptr, N, nullptr, sdf, nullptr, nullptr, nullptr, feat, mws,
-                                mb, st));
-  else
-    MP_TRY(mp::field_sdf_list(field->f, x_c, nullptr, nullptr, N, sdf, mws, mb, st));
+  mp::MlpCall c{};
+  c.x = x_c;
+  c.cap = N;
+  c.sdf = sdf;
+  c.feat = feat;
+  MP_TRY(mp::field_run(field->f, c, mws, mb, st));
   mp::force_outlier_sdf_kernel<<<mp::div_up(N, 256), 256, 0, st>>>(outl, N, sdf);
   MP_LAUNCH_CHECK();
   return 0;
@@ -336,8 +337,16 @@ static int render_person(const mp_scene_t* scene, int p, int R, const RenderWs& 
                             b.slot_list, b.count, b.outl, nullptr, st, Rp_dev));
   MP_TRY(launch_forward_jac(body, b.xc_list, Rp * n, b.count, nullptr, b.jinv, 12, st));
   if (pre_shade) MP_CHECK_CUDA(cudaEventRecord(pre_shade, st));
-  MP_TRY(field_shade_list(field, b.xc_list, b.slot_list, b.count, Rp * n, b.jinv, b.sdf, b.rgb, b.nrm, nullptr,
-                          nullptr, w.sub[p], w.sub_bytes, st));
+  MlpCall shade{};
+  shade.x = b.xc_list;
+  shade.slot = b.slot_list;
+  shade.count = b.count;
+  shade.cap = Rp * n;
+  shade.jinv = b.jinv;
+  shade.sdf = b.sdf;
+  shade.rgb = b.rgb;
+  shade.nrm = b.nrm;
+  MP_TRY(field_run(field, shade, w.sub[p], w.sub_bytes, st));
   if (tr && tr->cano_mesh[p]) {     // check_off_in_surface_points_cano_mesh on the main pass's points (:313-316)
     MP_CHECK_CUDA(cudaMemsetAsync(b.off, 1, Rp, st));
     MP_CHECK_CUDA(cudaMemsetAsync(b.in, 0, Rp, st));

@@ -481,7 +481,13 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
     // (training mode: the SDF callback does not clamp outliers, multiply.py:142 is eval-only -> exact far search)
     MP_TRY(launch_deform_rays(body, dirs, cam, zc, zcap, t == 0 ? nullptr : w.pos_new, E, E, R, /*prune=*/training ? 0 : 1, sc,
                               zcap, w.xc_list, w.slot_list, &w.st->count[t], nullptr, &w.st->active[t], st, R_dev));
-    MP_TRY(field_sdf_list(field, w.xc_list, w.slot_list, &w.st->count[t], R * E, sc, w.mlp_ws, w.mlp_ws_bytes, st));
+    MlpCall mlp{};
+    mlp.x = w.xc_list;
+    mlp.slot = w.slot_list;
+    mlp.count = &w.st->count[t];
+    mlp.cap = R * E;
+    mlp.sdf = sc;
+    MP_TRY(field_run(field, mlp, w.mlp_ws, w.mlp_ws_bytes, st));
     // shared memory per ray sized for THIS trip's list (M = (t+1) E entries; the final-set staging needs X + 2):
     // trip 0 -- usually the only active one -- then keeps every ray of the batch resident at once instead of
     // 13 warps per SM sized for the longest possible list
