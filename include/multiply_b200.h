@@ -381,6 +381,42 @@ int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int
                           uint8_t* in, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * mesh extraction: lib/utils/mesh.py:generate_mesh (:78-132) — MISE, marching cubes, largest component (DESIGN §3.7).
+ * Grids are [(R+1)^3] fp32, x-major: value (ix, iy, iz) at (ix*(R+1) + iy)*(R+1) + iz, as mp_sdf_grid writes them.
+ * ---------------------------------------------------------------------------------------- */
+/* MISE (generate_mesh :87-109 driving lib/libmise/mise.pyx, then to_dense :130-164) with R = res_init << depth in
+ * [1, 1024]: starts from the (res_init+1)^3 points at stride 2^depth, evaluates every added point once through the
+ * sdf-only program (points placed as mp_sdf_grid places them; the field's cond as set by mp_field_set_cond), splits
+ * every leaf below depth that some known point marks both ways (value >= level and value <= level; a point marks every
+ * leaf whose closed box holds it) and stops when a round adds no point.  grid receives the evaluated values, the rest
+ * filled by copying forward along x, then y, then z.  evaluated [(R+1)^3] (uint8, may be NULL) = 1 where a point was
+ * evaluated; *n_evaluated_host (may be NULL) their number.  Synchronises `stream` once per round (the number of
+ * points to evaluate). */
+size_t mp_mise_workspace_bytes(int res_init, int depth);
+int mp_mise(mp_net_t* field, const float* center_host /*[3]*/, float extent, float pad, int res_init, int depth,
+            double level, float* grid /*[(R+1)^3]*/, uint8_t* evaluated, long long* n_evaluated_host,
+            void* workspace, size_t workspace_bytes, void* stream);
+/* Marching cubes on any grid (generate_mesh :111-119; the tiling is DESIGN §3.7's, not skimage's Lewiner tables).  A
+ * corner is below when (double)v < level; an edge with one end below owns one vertex at t = (level - v0) / (v1 - v0)
+ * (fp64, v0 at the lower index), in world space ((p / R - 0.5) * pad) * extent + centre (fp64, rounded to fp32 once).
+ * Vertices in lattice-edge order, faces in cube order, oriented so that (v1-v0) x (v2-v0) points toward increasing
+ * value.  Two calls sharing one workspace: _count reads the sizes back (one synchronisation), _emit fills verts [V,3]
+ * and faces [F,3] (either may be NULL: not written). */
+size_t mp_marching_cubes_workspace_bytes(int res);
+int mp_marching_cubes_count(const float* grid, int res, double level, long long* V_host, long long* F_host,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int mp_marching_cubes_emit(const float* grid, int res, double level, const double* center_host /*[3]*/, double extent,
+                           double pad, float* verts, int64_t* faces, void* workspace, size_t workspace_bytes,
+                           void* stream);
+/* The connected component of largest area (generate_mesh :122-130; faces connected through shared vertices), areas
+ * summed in fp64 in a fixed order; on equal areas the component holding the lowest face index.  Its faces and vertices
+ * are compacted in their order into verts_out [V,3] / faces_out [F,3] (capacity V / F) and re-indexed; the kept sizes go
+ * to *V_out_host / *F_out_host (one synchronisation).  V == 0 or F == 0: an empty result, no error. */
+size_t mp_largest_component_workspace_bytes(int V, int F);
+int mp_largest_component(const float* verts, int V, const int64_t* faces, int F, float* verts_out, int64_t* faces_out,
+                         int* V_out_host, int* F_out_host, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * the fused entry used by Multiply.forward (multiply.py:174-598, eval branch)
  * ---------------------------------------------------------------------------------------- */
 /* Training-mode forward VALUES (multiply.py:174-598 with self.training, shipped loss weights, current_epoch >= 250):

@@ -158,6 +158,15 @@ SIGNATURES = {
     "mp_mesh_distance": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP]),
     "mp_mesh_check_sign": (_I, [_VP, _VP, _I, _VP, _VP]),
     "mp_mesh_surface_flags": (_I, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP]),
+    "mp_mise_workspace_bytes": (_SZ, [_I, _I]),
+    "mp_mise": (_I, [_VP, c_float_p, _F, _F, _I, _I, C.c_double, _VP, _VP, C.POINTER(C.c_longlong), _VP, _SZ, _VP]),
+    "mp_marching_cubes_workspace_bytes": (_SZ, [_I]),
+    "mp_marching_cubes_count": (_I, [_VP, _I, C.c_double, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _VP, _SZ,
+                                     _VP]),
+    "mp_marching_cubes_emit": (_I, [_VP, _I, C.c_double, C.POINTER(C.c_double), C.c_double, C.c_double, _VP, _VP, _VP,
+                                    _SZ, _VP]),
+    "mp_largest_component_workspace_bytes": (_SZ, [_I, _I]),
+    "mp_largest_component": (_I, [_VP, _I, _VP, _I, _VP, _VP, c_int_p, c_int_p, _VP, _SZ, _VP]),
     "mp_render_workspace_bytes": (_SZ, [C.POINTER(Scene), _I]),
     "mp_render_rays": (_I, [C.POINTER(Scene), _VP, _VP, _VP, _I, C.POINTER(RenderOut), _VP, _SZ, _VP]),
 }

@@ -310,6 +310,16 @@ __device__ __forceinline__ int lower_bound(const float* a, int n, float v) {   /
   return lo;
 }
 
+// One coordinate of a lattice point of lib/utils/mesh.py:generate_mesh (:92-95): ((idx / res - 0.5) * pad) * extent +
+// centre, every step rounded to fp32 separately as numpy does.  mp_sdf_grid and mp_mise both place their points here.
+__device__ __forceinline__ float lattice_coord(int idx, int res, float pad, float extent, float centre) {
+  float v = __fdiv_rn((float)idx, (float)res);
+  v = __fadd_rn(v, -0.5f);
+  v = __fmul_rn(v, pad);
+  v = __fmul_rn(v, extent);
+  return __fadd_rn(v, centre);
+}
+
 // LaplaceDensity.density_func (lib/model/density.py:20-25):
 //   alpha * (0.5 + 0.5 * sign(sdf) * expm1(-|sdf| / beta)),  alpha = 1 / beta
 __device__ __forceinline__ float laplace_density(float sdf, float beta) {

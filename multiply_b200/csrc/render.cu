@@ -35,8 +35,8 @@ __global__ void force_outlier_sdf_kernel(const uint8_t* __restrict__ outl, int n
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && outl[i]) sdf[i] = 4.0f;     // multiply.py:142-143
 }
-// lattice points of lib/utils/mesh.py:generate_mesh (:88-93): p = ((idx / res - 0.5) * pad) * extent + centre, every
-// step rounded to fp32 separately as numpy does; point i = (ix * (res+1) + iy) * (res+1) + iz
+// lattice points of lib/utils/mesh.py:generate_mesh (:88-93), see lattice_coord; point i = (ix * (res+1) + iy) *
+// (res+1) + iz
 __global__ void grid_points_kernel(float cx, float cy, float cz, float extent, float pad, int res, long long start,
                                    int count, float* __restrict__ pts) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -46,13 +46,7 @@ __global__ void grid_points_kernel(float cx, float cy, float cz, float extent, f
   int iz = (int)(i % n1), iy = (int)((i / n1) % n1), ix = (int)(i / ((long long)n1 * n1));
   const float c[3] = {cx, cy, cz};
   const int id[3] = {ix, iy, iz};
-  for (int k = 0; k < 3; ++k) {
-    float v = __fdiv_rn((float)id[k], (float)res);
-    v = __fadd_rn(v, -0.5f);
-    v = __fmul_rn(v, pad);
-    v = __fmul_rn(v, extent);
-    pts[3 * (size_t)t + k] = __fadd_rn(v, c[k]);
-  }
+  for (int k = 0; k < 3; ++k) pts[3 * (size_t)t + k] = lattice_coord(id[k], res, pad, extent, c[k]);
 }
 
 __global__ void iota_kernel(int* p, int n, int* count) {

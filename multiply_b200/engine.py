@@ -125,6 +125,29 @@ class Field:
                                 ws.numel(), L.stream_ptr()), "mp_sdf_grid")
         return vals
 
+    def mise(self, center, extent, res_init, depth, level=0.0, pad=1.1, want_evaluated=False):
+        """MISE of generate_mesh (lib/utils/mesh.py:87-109, lib/libmise/mise.pyx) on the device: returns (grid
+        [R+1]*3 fp32 = to_dense(), number of points evaluated[, evaluated [R+1]*3 bool]), R = res_init << depth."""
+        lib = L.lib()
+        n1 = (int(res_init) << int(depth)) + 1
+        grid = torch.empty(n1, n1, n1, device=self.device)
+        ev = torch.empty(n1, n1, n1, dtype=torch.uint8, device=self.device) if want_evaluated else None
+        ws = torch.empty(max(lib.mp_mise_workspace_bytes(int(res_init), int(depth)), 1), dtype=torch.uint8,
+                         device=self.device)
+        c = (C.c_float * 3)(*[float(v) for v in center])
+        n = C.c_longlong(0)
+        L.check(lib.mp_mise(self.handle, c, float(extent), float(pad), int(res_init), int(depth), float(level),
+                            grid.data_ptr(), L.ptr(ev), C.byref(n), ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_mise")
+        return (grid, n.value, ev.bool()) if want_evaluated else (grid, n.value)
+
+    def extract_mesh(self, center, extent, res_init=32, depth=3, level=0.0, pad=1.1):
+        """generate_mesh (lib/utils/mesh.py:78-132) for this field: MISE -> marching cubes -> largest component.
+        Returns (verts [V,3] fp32, faces [F,3] int64, number of points evaluated); device tensors."""
+        grid, n = self.mise(center, extent, res_init, depth, level, pad)
+        v, f = marching_cubes(grid, level, center, extent, pad)
+        v, f = largest_component(v, f)
+        return v, f, n
+
     def bg_forward(self, pts, view_dirs):
         """Background pair at given points (multiply.py:523-526): pts [N,4], view_dirs [N,3] -> (sdf [N], rgb [N,3])."""
         lib = L.lib()
@@ -290,6 +313,48 @@ class CanonicalMesh:
                 L.lib().mp_mesh_free(self.handle)
         except Exception:
             pass
+
+
+def marching_cubes(grid, level=0.0, center=(0.0, 0.0, 0.0), extent=None, pad=1.1):
+    """Marching cubes (DESIGN §3.7) on a device grid [R+1]*3 (x-major): returns (verts [V,3] fp32 in world space
+    ((p / R - 0.5) * pad) * extent + centre, faces [F,3] int64).  extent=None: lattice coordinates (pad 1, extent R,
+    centre R/2)."""
+    lib = L.lib()
+    g = grid.detach().to(torch.float32).contiguous()
+    R = g.shape[0] - 1
+    if extent is None:
+        center, extent, pad = (R / 2.0,) * 3, float(R), 1.0
+    with torch.cuda.device(g.device):
+        ws = torch.empty(max(lib.mp_marching_cubes_workspace_bytes(R), 1), dtype=torch.uint8, device=g.device)
+        V, F = C.c_longlong(0), C.c_longlong(0)
+        L.check(lib.mp_marching_cubes_count(g.data_ptr(), R, float(level), C.byref(V), C.byref(F), ws.data_ptr(),
+                                            ws.numel(), L.stream_ptr()), "mp_marching_cubes_count")
+        verts = torch.empty(V.value, 3, device=g.device)
+        faces = torch.empty(F.value, 3, dtype=torch.int64, device=g.device)
+        c = (C.c_double * 3)(*[float(v) for v in center])
+        L.check(lib.mp_marching_cubes_emit(g.data_ptr(), R, float(level), c, float(extent), float(pad),
+                                           verts.data_ptr() if V.value else None, faces.data_ptr() if F.value else None,
+                                           ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_marching_cubes_emit")
+        return verts, faces
+
+
+def largest_component(verts, faces):
+    """The connected component of largest area (generate_mesh :122-130): (verts [V,3], faces [F,3] int64) of that
+    component, in their original order and re-indexed.  No faces: empty tensors."""
+    lib = L.lib()
+    dev = verts.device
+    v = verts.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    f = faces.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    V, F = v.shape[0], f.shape[0]
+    with torch.cuda.device(dev):
+        ws = torch.empty(lib.mp_largest_component_workspace_bytes(V, F), dtype=torch.uint8, device=dev)
+        vo = torch.empty(max(V, 1), 3, device=dev)
+        fo = torch.empty(max(F, 1), 3, dtype=torch.int64, device=dev)
+        Vo, Fo = C.c_int(0), C.c_int(0)
+        L.check(lib.mp_largest_component(v.data_ptr() if V else None, V, f.data_ptr() if F else None, F, vo.data_ptr(),
+                                         fo.data_ptr(), C.byref(Vo), C.byref(Fo), ws.data_ptr(), ws.numel(),
+                                         L.stream_ptr()), "mp_largest_component")
+        return vo[:Vo.value], fo[:Fo.value]
 
 
 BETA_MIN = 1e-4      # LaplaceDensity's default (density.py:24)

@@ -127,6 +127,15 @@ class Multiply(nn.Module):
         self.mesh_f_cano_list[person_id] = torch.as_tensor(faces).detach().to(torch.int64).reshape(-1, 3)
         self._cano_meshes.pop(person_id, None)
 
+    def get_deformed_mesh_fast_mode_multiple_person(self, verts, smpl_tfs, person_id):
+        """multiply.py:129-134: LBS of canonical mesh vertices verts [V,3] (or [1,V,3]) with the weights of the nearest
+        canonical SMPL vertex and smpl_tfs [24,4,4] (or [1,24,4,4]) -> [1,V,3] (SMPLDeformer.forward_skinning)."""
+        b = self.deformer_list[person_id].body(verts.device)
+        # forward skinning reads only the canonical vertices; the posed ones keep the body's current frame
+        b.set_pose(getattr(b, "verts_p", b.verts_c), smpl_tfs.reshape(24, 4, 4))
+        xd, _ = b.forward_jac(verts.reshape(-1, 3))
+        return xd[None]
+
     def _canonical_mesh(self, person_id, device):
         if self.mesh_f_cano_list[person_id] is None:
             raise ValueError("person %d has no canonical mesh: the SMPL server provides no faces; call "
