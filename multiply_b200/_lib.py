@@ -2,9 +2,14 @@
 
 There is no fallback: if the shared library is missing the import of anything that needs it
 raises, and every entry point raises ``MpError`` with the library's error text on failure.
+
+The product package reaches the library through ``call`` alone: it refuses a tensor the kernels could not read (host
+memory, a strided view) before anything is enqueued, and names the failing function from the table, not from the caller.
 """
 import ctypes as C
 import os
+
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MP_LIB") or os.path.join(HERE, "libmultiply_b200.so")     # MP_LIB: A/B builds (scripts/)
@@ -92,83 +97,90 @@ class PersonSampleGrads(C.Structure):
     _fields_ = [("d_sdf", C.c_void_p), ("d_rgb", C.c_void_p), ("d_normal", C.c_void_p)]
 
 
+# Two markers stand in the table for a C type and tell ``call`` what the header's convention is:
+STATUS = "int: 0, or an error code with its text in mp_last_error()"      # every other restype is a value
+STREAM = "void* stream, the last parameter: the current stream unless the caller passes one"
+_CTYPE = {STATUS: C.c_int, STREAM: C.c_void_p}
+
 # name -> (restype, argtypes) ; mirrors include/multiply_b200.h one to one
 _VP, _I, _F, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 SIGNATURES = {
     "mp_version": (_I, []),
     "mp_last_error": (C.c_char_p, []),
     "mp_device_sm_count": (_I, []),
-    "mp_linspace_host": (_I, [_F, _F, _I, c_float_p]),
+    "mp_linspace_host": (STATUS, [_F, _F, _I, c_float_p]),
     "mp_launch_count": (C.c_longlong, [_I]),
     "mp_field_pack_bytes": (_SZ, []),
-    "mp_field_pack": (_I, [C.POINTER(ImplicitDesc), C.POINTER(RenderDesc), _I, _VP, _SZ, C.POINTER(_VP), _VP]),
+    "mp_field_pack": (STATUS, [C.POINTER(ImplicitDesc), C.POINTER(RenderDesc), _I, _VP, _SZ, C.POINTER(_VP), STREAM]),
     "mp_field_free": (None, [_VP]),
-    "mp_field_set_cond": (_I, [_VP, _VP, _VP]),
-    "mp_set_engine": (_I, [_I]),
+    "mp_field_set_cond": (STATUS, [_VP, _VP, STREAM]),
+    "mp_set_engine": (STATUS, [_I]),
     "mp_get_engine": (_I, []),
-    "mp_set_precision": (_I, [_I]),
+    "mp_set_precision": (STATUS, [_I]),
     "mp_get_precision": (_I, []),
-    "mp_profile_enable": (_I, [_I]),
-    "mp_set_streams": (_I, [_I]),
-    "mp_profile_read": (_I, [C.POINTER(C.c_double), C.POINTER(C.c_longlong), C.POINTER(C.c_double), _I]),
-    "mp_implicit_forward": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),
-    "mp_implicit_forward_grad": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, _VP]),
-    "mp_render_forward": (_I, [_VP, _VP, _VP, _VP, _I, _VP, _VP, _SZ, _VP]),
+    "mp_profile_enable": (STATUS, [_I]),
+    "mp_set_streams": (STATUS, [_I]),
+    "mp_profile_read": (STATUS, [C.POINTER(C.c_double), C.POINTER(C.c_longlong), C.POINTER(C.c_double), _I]),
+    "mp_implicit_forward": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_implicit_forward_grad": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_render_forward": (STATUS, [_VP, _VP, _VP, _VP, _I, _VP, _VP, _SZ, STREAM]),
     "mp_mlp_workspace_bytes": (_SZ, [_I]),
-    "mp_bg_nets_forward": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),
+    "mp_bg_nets_forward": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_sdf_grid_workspace_bytes": (_SZ, [_I]),
-    "mp_sdf_grid": (_I, [_VP, c_float_p, _F, _F, _I, _VP, _VP, _SZ, _VP]),
+    "mp_sdf_grid": (STATUS, [_VP, c_float_p, _F, _F, _I, _VP, _VP, _SZ, STREAM]),
     "mp_body_bytes": (_SZ, [_I]),
-    "mp_body_create": (_I, [_VP, _VP, _I, _F, _VP, _SZ, C.POINTER(_VP), _VP]),
+    "mp_body_create": (STATUS, [_VP, _VP, _I, _F, _VP, _SZ, C.POINTER(_VP), STREAM]),
     "mp_body_free": (None, [_VP]),
-    "mp_body_set_pose": (_I, [_VP, _VP, _VP, _VP]),
-    "mp_deform_inverse": (_I, [_VP, _VP, _I, _VP, _VP, _I, _VP]),
-    "mp_deform_forward_jac": (_I, [_VP, _VP, _I, _VP, _VP, _VP]),
-    "mp_deform_broyden": (_I, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _VP]),
-    "mp_body_set_root_finder": (_I, [_VP, _I, _F]),
-    "mp_laplace_density": (_I, [_VP, _I, _F, _VP, _VP]),
-    "mp_camera_rays": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP]),
-    "mp_sphere_intersections": (_I, [_VP, _VP, _I, _F, _VP, _VP, _VP]),
-    "mp_ray_box_hits": (_I, [_VP, _VP, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), _VP, _VP, _VP, _VP]),
-    "mp_hit_list_finalize": (_I, [_VP, _VP, _VP]),
-    "mp_ray_aabb_hits": (_I, [_VP, _VP, _I, _VP, _I, C.c_double, _VP, _VP, _VP, _VP]),
+    "mp_body_set_pose": (STATUS, [_VP, _VP, _VP, STREAM]),
+    "mp_deform_inverse": (STATUS, [_VP, _VP, _I, _VP, _VP, _I, STREAM]),
+    "mp_deform_forward_jac": (STATUS, [_VP, _VP, _I, _VP, _VP, STREAM]),
+    "mp_deform_broyden": (STATUS, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, STREAM]),
+    "mp_body_set_root_finder": (STATUS, [_VP, _I, _F]),
+    "mp_laplace_density": (STATUS, [_VP, _I, _F, _VP, STREAM]),
+    "mp_camera_rays": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, STREAM]),
+    "mp_sphere_intersections": (STATUS, [_VP, _VP, _I, _F, _VP, _VP, STREAM]),
+    "mp_ray_box_hits": (STATUS, [_VP, _VP, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), _VP, _VP, _VP, STREAM]),
+    "mp_hit_list_finalize": (STATUS, [_VP, _VP, STREAM]),
+    "mp_ray_aabb_hits": (STATUS, [_VP, _VP, _I, _VP, _I, C.c_double, _VP, _VP, _VP, STREAM]),
     "mp_smpl_bytes": (_SZ, [_I]),
-    "mp_smpl_create": (_I, [_VP, _VP, _VP, _VP, C.POINTER(C.c_int), _VP, _I, _VP, _VP, _SZ, C.POINTER(_VP), _VP]),
+    "mp_smpl_create": (STATUS, [_VP, _VP, _VP, _VP, C.POINTER(C.c_int), _VP, _I, _VP, _VP, _SZ, C.POINTER(_VP),
+                                STREAM]),
     "mp_smpl_free": (None, [_VP]),
-    "mp_smpl_canonical": (_I, [_VP, _VP, _VP, _VP]),
-    "mp_smpl_forward": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP]),
+    "mp_smpl_canonical": (STATUS, [_VP, _VP, _VP, STREAM]),
+    "mp_smpl_forward": (STATUS, [_VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, STREAM]),
     "mp_sampler_workspace_bytes": (_SZ, [C.POINTER(SamplerCfg), _I]),
-    "mp_sample_rays": (_I, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, _VP]),
-    "mp_sample_rays_train": (_I, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, C.POINTER(SamplerRng), _VP, _VP, _VP, _VP,
-                                  _VP, _SZ, _VP]),
-    "mp_sdf_with_deformer": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, _VP]),
+    "mp_sample_rays": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_sample_rays_train": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, C.POINTER(SamplerRng), _VP, _VP, _VP,
+                                      _VP, _VP, _SZ, STREAM]),
+    "mp_sdf_with_deformer": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_composite_workspace_bytes": (_SZ, [_I, _I]),
-    "mp_composite": (_I, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
-    "mp_final_compose": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _VP]),
+    "mp_composite": (STATUS, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_final_compose": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, STREAM]),
     "mp_composite_backward_workspace_bytes": (_SZ, [_I, _I]),
-    "mp_composite_backward": (_I, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP,
-                                   C.POINTER(PersonSampleGrads), _VP, _VP, _SZ, _VP]),
-    "mp_bg_composite_backward": (_I, [_VP, _VP, _I, _F, _VP, _VP, _VP, _VP, _VP]),
-    "mp_final_compose_backward": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "mp_composite_backward": (STATUS, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP,
+                                       C.POINTER(PersonSampleGrads), _VP, _VP, _SZ, STREAM]),
+    "mp_bg_composite_backward": (STATUS, [_VP, _VP, _I, _F, _VP, _VP, _VP, _VP, STREAM]),
+    "mp_final_compose_backward": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, STREAM]),
     "mp_background_workspace_bytes": (_SZ, [_I]),
-    "mp_background": (_I, [_VP, _VP, _VP, _I, _F, _VP, _VP, _SZ, _VP]),
-    "mp_mesh_plan": (_I, [_VP, _I, _VP, _I, _F, _VP, C.POINTER(MeshPlan), _VP]),
-    "mp_mesh_create": (_I, [C.POINTER(MeshPlan), _VP, _VP, _VP, _SZ, C.POINTER(_VP), _VP]),
+    "mp_background": (STATUS, [_VP, _VP, _VP, _I, _F, _VP, _VP, _SZ, STREAM]),
+    "mp_mesh_plan": (STATUS, [_VP, _I, _VP, _I, _F, _VP, C.POINTER(MeshPlan), STREAM]),
+    "mp_mesh_create": (STATUS, [C.POINTER(MeshPlan), _VP, _VP, _VP, _SZ, C.POINTER(_VP), STREAM]),
     "mp_mesh_free": (None, [_VP]),
-    "mp_mesh_distance": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP]),
-    "mp_mesh_check_sign": (_I, [_VP, _VP, _I, _VP, _VP]),
-    "mp_mesh_surface_flags": (_I, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP]),
+    "mp_mesh_distance": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, STREAM]),
+    "mp_mesh_check_sign": (STATUS, [_VP, _VP, _I, _VP, STREAM]),
+    "mp_mesh_surface_flags": (STATUS, [_VP, _VP, _I, _I, _F, _VP, _VP, STREAM]),
     "mp_mise_workspace_bytes": (_SZ, [_I, _I]),
-    "mp_mise": (_I, [_VP, c_float_p, _F, _F, _I, _I, C.c_double, _VP, _VP, C.POINTER(C.c_longlong), _VP, _SZ, _VP]),
+    "mp_mise": (STATUS, [_VP, c_float_p, _F, _F, _I, _I, C.c_double, _VP, _VP, C.POINTER(C.c_longlong), _VP, _SZ,
+                         STREAM]),
     "mp_marching_cubes_workspace_bytes": (_SZ, [_I]),
-    "mp_marching_cubes_count": (_I, [_VP, _I, C.c_double, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _VP, _SZ,
-                                     _VP]),
-    "mp_marching_cubes_emit": (_I, [_VP, _I, C.c_double, C.POINTER(C.c_double), C.c_double, C.c_double, _VP, _VP, _VP,
-                                    _SZ, _VP]),
+    "mp_marching_cubes_count": (STATUS, [_VP, _I, C.c_double, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), _VP,
+                                         _SZ, STREAM]),
+    "mp_marching_cubes_emit": (STATUS, [_VP, _I, C.c_double, C.POINTER(C.c_double), C.c_double, C.c_double, _VP, _VP,
+                                        _VP, _SZ, STREAM]),
     "mp_largest_component_workspace_bytes": (_SZ, [_I, _I]),
-    "mp_largest_component": (_I, [_VP, _I, _VP, _I, _VP, _VP, c_int_p, c_int_p, _VP, _SZ, _VP]),
+    "mp_largest_component": (STATUS, [_VP, _I, _VP, _I, _VP, _VP, c_int_p, c_int_p, _VP, _SZ, STREAM]),
     "mp_render_workspace_bytes": (_SZ, [C.POINTER(Scene), _I]),
-    "mp_render_rays": (_I, [C.POINTER(Scene), _VP, _VP, _VP, _I, C.POINTER(RenderOut), _VP, _SZ, _VP]),
+    "mp_render_rays": (STATUS, [C.POINTER(Scene), _VP, _VP, _VP, _I, C.POINTER(RenderOut), _VP, _SZ, STREAM]),
 }
 
 _lib = None
@@ -184,8 +196,8 @@ def lib():
         h = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(h, name)
-            fn.restype = res
-            fn.argtypes = args
+            fn.restype = _CTYPE.get(res, res)
+            fn.argtypes = [_CTYPE.get(a, a) for a in args]
         _lib = h
     return _lib
 
@@ -207,5 +219,63 @@ def ptr(t):
 
 
 def stream_ptr():
-    import torch
     return torch.cuda.current_stream().cuda_stream
+
+
+def call(name, *args):
+    """Calls library function ``name``.  A tensor argument becomes its device pointer through ``ptr``; a structure is
+    passed by reference where the parameter is a pointer to it; everything else (None, numbers, handles, ctypes arrays,
+    ``byref`` objects) is ctypes' to convert.  The trailing stream of a function that takes one may be left out: it is
+    the current stream.  A non-zero status raises ``MpError`` with the library's message; a value is returned."""
+    res, params = SIGNATURES[name]
+    fn = getattr(lib(), name)
+    own_stream = len(args) == len(params) - 1 and params[-1] is STREAM
+    if len(args) + own_stream != len(params):
+        raise MpError("%s takes %d arguments, got %d" % (name, len(params), len(args)))
+    conv = []
+    for i, (a, p) in enumerate(zip(args, params)):
+        if isinstance(a, torch.Tensor):
+            try:
+                a = ptr(a)
+            except MpError as e:
+                raise MpError("%s, argument %d: %s" % (name, i, e)) from None
+        elif isinstance(a, C.Structure) and p is C.POINTER(type(a)):
+            a = C.byref(a)
+        conv.append(a)
+    if own_stream:
+        conv.append(stream_ptr())
+    out = fn(*conv)
+    if res is not STATUS:
+        return out
+    check(out, name)
+
+
+def dev(t, device, dtype=torch.float32):
+    """``t`` (or None) detached, on ``device``, of ``dtype`` and contiguous: the form every tensor the library reads has."""
+    return None if t is None else t.detach().to(device=device, dtype=dtype).contiguous()
+
+
+def workspace(nbytes, device):
+    """Uninitialised device bytes for a ``*_bytes`` query's answer; never empty, so its pointer is always valid."""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+def vec3(ctype, v):
+    """A host [3] array of ``ctype`` (a centre, half extents)."""
+    return (ctype * 3)(*[float(x) for x in v])
+
+
+class Handle(C.c_void_p):
+    """An object the library built in caller storage (the ``out`` of mp_field_pack / mp_*_create); passes wherever a
+    ``void*`` does.  Dropping it calls the ``mp_*_free`` named at construction."""
+
+    def __init__(self, free):
+        super().__init__()
+        self.free = free
+
+    def __del__(self):
+        try:
+            if self.value:
+                call(self.free, self)
+        except Exception:       # interpreter shutdown: the library or this module may already be gone
+            pass

@@ -12,23 +12,19 @@ import torch
 from . import _lib as L
 
 
-def _dev(t, device):
-    return t.detach().to(device=device, dtype=torch.float32).contiguous()
-
-
 def set_engine(name):
     """'tc' = wgmma split-fp16 tensor-core engine (default), 'simt' = fp32 validation engine."""
-    L.check(L.lib().mp_set_engine({"simt": 0, "tc": 1}[name]), "mp_set_engine")
+    L.call("mp_set_engine", {"simt": 0, "tc": 1}[name])
 
 
 def set_precision(mode):
     """Tensor-core engine precision: 'parity' (default, three split terms), 'colour1' (single-term colour layers),
     'throughput' (single fp16 term everywhere; outside the 1e-4 gate)."""
-    L.check(L.lib().mp_set_precision({"parity": 0, "colour1": 1, "throughput": 2}[mode]), "mp_set_precision")
+    L.call("mp_set_precision", {"parity": 0, "colour1": 1, "throughput": 2}[mode])
 
 
 def get_engine():
-    return {0: "simt", 1: "tc"}[L.lib().mp_get_engine()]
+    return {0: "simt", 1: "tc"}[L.call("mp_get_engine")]
 
 
 def _stack(sd, n_layers, dev, keep):
@@ -36,19 +32,13 @@ def _stack(sd, n_layers, dev, keep):
     st.n_layers = n_layers
     for l in range(n_layers):
         if f"lin{l}.weight_v" in sd:
-            v = _dev(sd[f"lin{l}.weight_v"], dev)
-            g = _dev(sd[f"lin{l}.weight_g"], dev)
-            keep += [v, g]
-            st.weight_v[l] = v.data_ptr()
-            st.weight_g[l] = g.data_ptr()
+            v = L.dev(sd[f"lin{l}.weight_v"], dev)
+            g = L.dev(sd[f"lin{l}.weight_g"], dev)
         else:
-            v = _dev(sd[f"lin{l}.weight"], dev)
-            keep.append(v)
-            st.weight_v[l] = v.data_ptr()
-            st.weight_g[l] = None
-        b = _dev(sd[f"lin{l}.bias"], dev)
-        keep.append(b)
-        st.bias[l] = b.data_ptr()
+            v, g = L.dev(sd[f"lin{l}.weight"], dev), None
+        b = L.dev(sd[f"lin{l}.bias"], dev)
+        keep += [v, g, b]
+        st.weight_v[l], st.weight_g[l], st.bias[l] = L.ptr(v), L.ptr(g), L.ptr(b)
         st.out_dim[l], st.in_dim[l] = v.shape
     return st
 
@@ -57,7 +47,6 @@ class Field:
     """Packed ImplicitNet + RenderingNet pair (mp_field_pack)."""
 
     def __init__(self, implicit_sd, render_sd, background=False, device="cuda"):
-        lib = L.lib()
         self.device = torch.device(device)
         keep = []
         imp = L.ImplicitDesc()
@@ -72,72 +61,53 @@ class Field:
         ren.mode = 1 if background else 0
         ren.multires_view = 4 if background else -1
         if not background:
-            pw, pb = _dev(render_sd["lin_pose.weight"], self.device), _dev(render_sd["lin_pose.bias"], self.device)
+            pw, pb = L.dev(render_sd["lin_pose.weight"], self.device), L.dev(render_sd["lin_pose.bias"], self.device)
             keep += [pw, pb]
-            ren.lin_pose_weight, ren.lin_pose_bias = pw.data_ptr(), pb.data_ptr()
-        nbytes = lib.mp_field_pack_bytes()
-        self.storage = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        L.check(lib.mp_field_pack(C.byref(imp), C.byref(ren), int(background), self.storage.data_ptr(), nbytes,
-                                  C.byref(h), L.stream_ptr()), "mp_field_pack")
+            ren.lin_pose_weight, ren.lin_pose_bias = L.ptr(pw), L.ptr(pb)
+        self.storage = L.workspace(L.call("mp_field_pack_bytes"), self.device)
+        self.handle = L.Handle("mp_field_free")
+        L.call("mp_field_pack", imp, ren, int(background), self.storage, self.storage.numel(), C.byref(self.handle))
         torch.cuda.current_stream().synchronize()   # raw parameter tensors may be released now
-        self.handle = h
         self.background = background
 
     def set_cond(self, cond):
-        c = _dev(cond.reshape(-1), self.device)
-        L.check(L.lib().mp_field_set_cond(self.handle, c.data_ptr(), L.stream_ptr()), "mp_field_set_cond")
+        c = L.dev(cond.reshape(-1), self.device)
+        L.call("mp_field_set_cond", self.handle, c)
         self._cond = c
-
-    def __del__(self):
-        try:
-            if getattr(self, "handle", None):
-                L.lib().mp_field_free(self.handle)
-        except Exception:
-            pass
 
     # operator-level entry points ------------------------------------------------------
     def implicit_forward(self, x, want_feat=True, want_grad=False):
-        lib = L.lib()
-        x = _dev(x, self.device)
+        x = L.dev(x, self.device)
         N = x.shape[0]
         sdf = torch.empty(N, device=self.device)
         feat = torch.empty(N, 256, device=self.device) if want_feat else None
-        ws = torch.empty(lib.mp_mlp_workspace_bytes(N), dtype=torch.uint8, device=self.device)
+        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N), self.device)
         if want_grad:
             grad = torch.empty(N, 3, device=self.device)
-            L.check(lib.mp_implicit_forward_grad(self.handle, x.data_ptr(), N, sdf.data_ptr(), L.ptr(feat),
-                                                 grad.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                    "mp_implicit_forward_grad")
+            L.call("mp_implicit_forward_grad", self.handle, x, N, sdf, feat, grad, ws, ws.numel())
             return sdf, feat, grad
-        L.check(lib.mp_implicit_forward(self.handle, x.data_ptr(), N, sdf.data_ptr(), L.ptr(feat), ws.data_ptr(),
-                                        ws.numel(), L.stream_ptr()), "mp_implicit_forward")
+        L.call("mp_implicit_forward", self.handle, x, N, sdf, feat, ws, ws.numel())
         return sdf, feat
 
     def sdf_grid(self, center, extent, res, pad=1.1):
         """Canonical SDF on the (res+1)^3 lattice of generate_mesh (lib/utils/mesh.py:78-105): returns [res+1]*3 fp32."""
-        lib = L.lib()
         n1 = res + 1
         vals = torch.empty(n1, n1, n1, device=self.device)
-        ws = torch.empty(lib.mp_sdf_grid_workspace_bytes(res), dtype=torch.uint8, device=self.device)
-        c = (C.c_float * 3)(*[float(v) for v in center])
-        L.check(lib.mp_sdf_grid(self.handle, c, float(extent), float(pad), int(res), vals.data_ptr(), ws.data_ptr(),
-                                ws.numel(), L.stream_ptr()), "mp_sdf_grid")
+        ws = L.workspace(L.call("mp_sdf_grid_workspace_bytes", res), self.device)
+        L.call("mp_sdf_grid", self.handle, L.vec3(C.c_float, center), float(extent), float(pad), int(res), vals, ws,
+               ws.numel())
         return vals
 
     def mise(self, center, extent, res_init, depth, level=0.0, pad=1.1, want_evaluated=False):
         """MISE of generate_mesh (lib/utils/mesh.py:87-109, lib/libmise/mise.pyx) on the device: returns (grid
         [R+1]*3 fp32 = to_dense(), number of points evaluated[, evaluated [R+1]*3 bool]), R = res_init << depth."""
-        lib = L.lib()
         n1 = (int(res_init) << int(depth)) + 1
         grid = torch.empty(n1, n1, n1, device=self.device)
         ev = torch.empty(n1, n1, n1, dtype=torch.uint8, device=self.device) if want_evaluated else None
-        ws = torch.empty(max(lib.mp_mise_workspace_bytes(int(res_init), int(depth)), 1), dtype=torch.uint8,
-                         device=self.device)
-        c = (C.c_float * 3)(*[float(v) for v in center])
+        ws = L.workspace(L.call("mp_mise_workspace_bytes", int(res_init), int(depth)), self.device)
         n = C.c_longlong(0)
-        L.check(lib.mp_mise(self.handle, c, float(extent), float(pad), int(res_init), int(depth), float(level),
-                            grid.data_ptr(), L.ptr(ev), C.byref(n), ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_mise")
+        L.call("mp_mise", self.handle, L.vec3(C.c_float, center), float(extent), float(pad), int(res_init), int(depth),
+               float(level), grid, ev, C.byref(n), ws, ws.numel())
         return (grid, n.value, ev.bool()) if want_evaluated else (grid, n.value)
 
     def extract_mesh(self, center, extent, res_init=32, depth=3, level=0.0, pad=1.1):
@@ -150,24 +120,30 @@ class Field:
 
     def bg_forward(self, pts, view_dirs):
         """Background pair at given points (multiply.py:523-526): pts [N,4], view_dirs [N,3] -> (sdf [N], rgb [N,3])."""
-        lib = L.lib()
-        pts, view_dirs = _dev(pts, self.device), _dev(view_dirs, self.device)
+        pts, view_dirs = L.dev(pts, self.device), L.dev(view_dirs, self.device)
         N = pts.shape[0]
         sdf = torch.empty(N, device=self.device)
         rgb = torch.empty(N, 3, device=self.device)
-        ws = torch.empty(lib.mp_mlp_workspace_bytes(N), dtype=torch.uint8, device=self.device)
-        L.check(lib.mp_bg_nets_forward(self.handle, pts.data_ptr(), view_dirs.data_ptr(), N, sdf.data_ptr(),
-                                       rgb.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_bg_nets_forward")
+        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N), self.device)
+        L.call("mp_bg_nets_forward", self.handle, pts, view_dirs, N, sdf, rgb, ws, ws.numel())
         return sdf, rgb
 
+    def bg_pixels(self, ray_dirs, cam_loc, bound_r):
+        """The background pixel of every ray (mp_background: inverse-sphere samples -> background pair -> volume
+        rendering, multiply.py:482-539): ray_dirs [R,3], cam_loc [R,3] -> bg_rgb [R,3]."""
+        ray_dirs, cam_loc = L.dev(ray_dirs, self.device), L.dev(cam_loc, self.device)
+        R = ray_dirs.shape[0]
+        rgb = torch.empty(R, 3, device=self.device)
+        ws = L.workspace(L.call("mp_background_workspace_bytes", R), self.device)
+        L.call("mp_background", self.handle, ray_dirs, cam_loc, R, float(bound_r), rgb, ws, ws.numel())
+        return rgb
+
     def render_forward(self, points, normals, feat):
-        lib = L.lib()
-        points, normals, feat = (_dev(t, self.device) for t in (points, normals, feat))
+        points, normals, feat = (L.dev(t, self.device) for t in (points, normals, feat))
         N = points.shape[0]
         rgb = torch.empty(N, 3, device=self.device)
-        ws = torch.empty(lib.mp_mlp_workspace_bytes(N), dtype=torch.uint8, device=self.device)
-        L.check(lib.mp_render_forward(self.handle, points.data_ptr(), normals.data_ptr(), feat.data_ptr(), N,
-                                      rgb.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_render_forward")
+        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N), self.device)
+        L.call("mp_render_forward", self.handle, points, normals, feat, N, rgb, ws, ws.numel())
         return rgb
 
 
@@ -175,70 +151,53 @@ class Body:
     """Canonical SMPL vertices + skinning weights (SMPLDeformer state) and the per-frame pose."""
 
     def __init__(self, verts_cano, weights, cano_cell=0.2, device="cuda"):
-        lib = L.lib()
         self.device = torch.device(device)
-        self.verts_c = _dev(verts_cano, self.device)
-        self.weights = _dev(weights, self.device)
-        V = self.verts_c.shape[0]
-        nbytes = lib.mp_body_bytes(V)
-        self.storage = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        h = C.c_void_p()
-        L.check(lib.mp_body_create(self.verts_c.data_ptr(), self.weights.data_ptr(), V, float(cano_cell),
-                                   self.storage.data_ptr(), nbytes, C.byref(h), L.stream_ptr()), "mp_body_create")
-        self.handle = h
-        self.V = V
+        self.verts_c = L.dev(verts_cano, self.device)
+        self.weights = L.dev(weights, self.device)
+        self.V = self.verts_c.shape[0]
+        self.storage = L.workspace(L.call("mp_body_bytes", self.V), self.device)
+        self.handle = L.Handle("mp_body_free")
+        L.call("mp_body_create", self.verts_c, self.weights, self.V, float(cano_cell), self.storage, self.storage.numel(),
+               C.byref(self.handle))
 
     def set_pose(self, verts_posed, tfs):
-        self.verts_p = _dev(verts_posed, self.device)
-        self.tfs = _dev(tfs.reshape(24, 4, 4), self.device)
-        L.check(L.lib().mp_body_set_pose(self.handle, self.verts_p.data_ptr(), self.tfs.data_ptr(), L.stream_ptr()),
-                "mp_body_set_pose")
+        self.verts_p = L.dev(verts_posed, self.device)
+        self.tfs = L.dev(tfs.reshape(24, 4, 4), self.device)
+        L.call("mp_body_set_pose", self.handle, self.verts_p, self.tfs)
 
     def deform_inverse(self, x, exact_far=True):
-        x = _dev(x, self.device)
+        x = L.dev(x, self.device)
         N = x.shape[0]
         xc = torch.empty(N, 3, device=self.device)
         out = torch.empty(N, dtype=torch.uint8, device=self.device)
-        L.check(L.lib().mp_deform_inverse(self.handle, x.data_ptr(), N, xc.data_ptr(), out.data_ptr(),
-                                          int(exact_far), L.stream_ptr()), "mp_deform_inverse")
+        L.call("mp_deform_inverse", self.handle, x, N, xc, out, int(exact_far))
         return xc, out.bool()
 
     def deform_broyden(self, x, max_steps=10, cvg_threshold=1e-5):
         """Root of forward_skinning(x_c) = x by Broyden's method from the closed-form inverse (row f4, not in the
         reference): returns dict(x_c, residual, converged, outlier, steps)."""
-        x = _dev(x, self.device)
+        x = L.dev(x, self.device)
         N = x.shape[0]
         xc = torch.empty(N, 3, device=self.device)
         res = torch.empty(N, device=self.device)
         conv = torch.empty(N, dtype=torch.uint8, device=self.device)
         out = torch.empty(N, dtype=torch.uint8, device=self.device)
         steps = torch.empty(N, dtype=torch.int32, device=self.device)
-        L.check(L.lib().mp_deform_broyden(self.handle, x.data_ptr(), N, int(max_steps), float(cvg_threshold),
-                                          xc.data_ptr(), res.data_ptr(), conv.data_ptr(), out.data_ptr(),
-                                          steps.data_ptr(), L.stream_ptr()), "mp_deform_broyden")
+        L.call("mp_deform_broyden", self.handle, x, N, int(max_steps), float(cvg_threshold), xc, res, conv, out, steps)
         return dict(x_c=xc, residual=res, converged=conv.bool(), outlier=out.bool(), steps=steps)
 
     def set_root_finder(self, max_steps, cvg_threshold=1e-5):
         """max_steps > 0: every inverse-deformer call on this body refines its non-outlier points with Broyden
         iterations (mp_body_set_root_finder); 0 restores the reference's closed-form inverse."""
-        L.check(L.lib().mp_body_set_root_finder(self.handle, int(max_steps), float(cvg_threshold)),
-                "mp_body_set_root_finder")
+        L.call("mp_body_set_root_finder", self.handle, int(max_steps), float(cvg_threshold))
 
     def forward_jac(self, xc):
-        xc = _dev(xc, self.device)
+        xc = L.dev(xc, self.device)
         N = xc.shape[0]
         xd = torch.empty(N, 3, device=self.device)
         J = torch.empty(N, 9, device=self.device)
-        L.check(L.lib().mp_deform_forward_jac(self.handle, xc.data_ptr(), N, xd.data_ptr(), J.data_ptr(),
-                                              L.stream_ptr()), "mp_deform_forward_jac")
+        L.call("mp_deform_forward_jac", self.handle, xc, N, xd, J)
         return xd, J
-
-    def __del__(self):
-        try:
-            if getattr(self, "handle", None):
-                L.lib().mp_body_free(self.handle)
-        except Exception:
-            pass
 
 
 class CanonicalMesh:
@@ -248,23 +207,18 @@ class CanonicalMesh:
     reads the grid size back once (one synchronisation); the queries do not synchronise."""
 
     def __init__(self, verts, faces, margin=0.01, device="cuda"):
-        lib = L.lib()
         self.device = torch.device(device)
         with torch.cuda.device(self.device):
-            v = _dev(verts.reshape(-1, 3), self.device)
-            f = torch.as_tensor(faces).detach().to(device=self.device, dtype=torch.int64).reshape(-1, 3).contiguous()
+            v = L.dev(verts.reshape(-1, 3), self.device)
+            f = L.dev(torch.as_tensor(faces).reshape(-1, 3), self.device, torch.int64)
             self.V, self.F = v.shape[0], f.shape[0]
-            scratch = torch.empty(L.MP_MESH_PLAN_SCRATCH_BYTES, dtype=torch.uint8, device=self.device)
-            plan = L.MeshPlan()
-            L.check(lib.mp_mesh_plan(v.data_ptr(), self.V, f.data_ptr(), self.F, float(margin), scratch.data_ptr(),
-                                     C.byref(plan), L.stream_ptr()), "mp_mesh_plan")
-            self.plan = plan
-            self.storage = torch.empty(plan.storage_bytes, dtype=torch.uint8, device=self.device)
-            h = C.c_void_p()
-            L.check(lib.mp_mesh_create(C.byref(plan), v.data_ptr(), f.data_ptr(), self.storage.data_ptr(),
-                                       plan.storage_bytes, C.byref(h), L.stream_ptr()), "mp_mesh_create")
+            scratch = L.workspace(L.MP_MESH_PLAN_SCRATCH_BYTES, self.device)
+            self.plan = L.MeshPlan()
+            L.call("mp_mesh_plan", v, self.V, f, self.F, float(margin), scratch, self.plan)
+            self.storage = L.workspace(self.plan.storage_bytes, self.device)
+            self.handle = L.Handle("mp_mesh_free")
+            L.call("mp_mesh_create", self.plan, v, f, self.storage, self.plan.storage_bytes, C.byref(self.handle))
             self._src = (v, f)        # read by the build kernels enqueued above
-            self.handle = h
 
     @property
     def grid_dims(self):
@@ -274,86 +228,69 @@ class CanonicalMesh:
         """pts [N,3] -> (dist2 [N] fp32 squared distance, face_idx [N] int64, dist_type [N] int32), kaolin's
         convention: 0 face interior, 1/2/3 vertex 0/1/2, 4/5/6 edge 01/12/20; ties go to the lowest face index."""
         with torch.cuda.device(self.device):
-            p = _dev(pts.reshape(-1, 3), self.device)
+            p = L.dev(pts.reshape(-1, 3), self.device)
             N = p.shape[0]
             d2 = torch.empty(N, device=self.device)
             fi = torch.empty(N, dtype=torch.int64, device=self.device)
             dt = torch.empty(N, dtype=torch.int32, device=self.device)
-            L.check(L.lib().mp_mesh_distance(self.handle, p.data_ptr(), N, d2.data_ptr(), fi.data_ptr(), dt.data_ptr(),
-                                             L.stream_ptr()), "mp_mesh_distance")
+            L.call("mp_mesh_distance", self.handle, p, N, d2, fi, dt)
             return d2, fi, dt
 
     def check_sign(self, pts):
         """pts [N,3] -> inside [N] bool: odd number of crossings of the ray p + t (0,0,1), t > 0."""
         with torch.cuda.device(self.device):
-            p = _dev(pts.reshape(-1, 3), self.device)
+            p = L.dev(pts.reshape(-1, 3), self.device)
             N = p.shape[0]
             ins = torch.empty(N, dtype=torch.uint8, device=self.device)
-            L.check(L.lib().mp_mesh_check_sign(self.handle, p.data_ptr(), N, ins.data_ptr(), L.stream_ptr()),
-                    "mp_mesh_check_sign")
+            L.call("mp_mesh_check_sign", self.handle, p, N, ins)
             return ins.bool()
 
     def surface_flags(self, x_c, N_samples, threshold=0.05):
         """check_off_in_surface_points_cano_mesh (multiply.py:153-167): x_c [rows*N_samples,3] ->
         (index_off_surface [rows], index_in_surface [rows]) bool."""
         with torch.cuda.device(self.device):
-            x = _dev(x_c.reshape(-1, 3), self.device)
+            x = L.dev(x_c.reshape(-1, 3), self.device)
             rows = x.shape[0] // int(N_samples)
             assert rows * int(N_samples) == x.shape[0], "x_c must hold rows * N_samples points"
             off = torch.empty(rows, dtype=torch.uint8, device=self.device)
             ins = torch.empty(rows, dtype=torch.uint8, device=self.device)
-            L.check(L.lib().mp_mesh_surface_flags(self.handle, x.data_ptr(), rows, int(N_samples), float(threshold),
-                                                  off.data_ptr(), ins.data_ptr(), L.stream_ptr()),
-                    "mp_mesh_surface_flags")
+            L.call("mp_mesh_surface_flags", self.handle, x, rows, int(N_samples), float(threshold), off, ins)
             return off.bool(), ins.bool()
-
-    def __del__(self):
-        try:
-            if getattr(self, "handle", None):
-                L.lib().mp_mesh_free(self.handle)
-        except Exception:
-            pass
 
 
 def marching_cubes(grid, level=0.0, center=(0.0, 0.0, 0.0), extent=None, pad=1.1):
     """Marching cubes (DESIGN §3.7) on a device grid [R+1]*3 (x-major): returns (verts [V,3] fp32 in world space
     ((p / R - 0.5) * pad) * extent + centre, faces [F,3] int64).  extent=None: lattice coordinates (pad 1, extent R,
     centre R/2)."""
-    lib = L.lib()
-    g = grid.detach().to(torch.float32).contiguous()
+    g = L.dev(grid, grid.device)
     R = g.shape[0] - 1
     if extent is None:
         center, extent, pad = (R / 2.0,) * 3, float(R), 1.0
     with torch.cuda.device(g.device):
-        ws = torch.empty(max(lib.mp_marching_cubes_workspace_bytes(R), 1), dtype=torch.uint8, device=g.device)
+        ws = L.workspace(L.call("mp_marching_cubes_workspace_bytes", R), g.device)
         V, F = C.c_longlong(0), C.c_longlong(0)
-        L.check(lib.mp_marching_cubes_count(g.data_ptr(), R, float(level), C.byref(V), C.byref(F), ws.data_ptr(),
-                                            ws.numel(), L.stream_ptr()), "mp_marching_cubes_count")
+        L.call("mp_marching_cubes_count", g, R, float(level), C.byref(V), C.byref(F), ws, ws.numel())
         verts = torch.empty(V.value, 3, device=g.device)
         faces = torch.empty(F.value, 3, dtype=torch.int64, device=g.device)
-        c = (C.c_double * 3)(*[float(v) for v in center])
-        L.check(lib.mp_marching_cubes_emit(g.data_ptr(), R, float(level), c, float(extent), float(pad),
-                                           verts.data_ptr() if V.value else None, faces.data_ptr() if F.value else None,
-                                           ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_marching_cubes_emit")
+        L.call("mp_marching_cubes_emit", g, R, float(level), L.vec3(C.c_double, center), float(extent), float(pad),
+               verts if V.value else None, faces if F.value else None, ws, ws.numel())
         return verts, faces
 
 
 def largest_component(verts, faces):
     """The connected component of largest area (generate_mesh :122-130): (verts [V,3], faces [F,3] int64) of that
     component, in their original order and re-indexed.  No faces: empty tensors."""
-    lib = L.lib()
     dev = verts.device
-    v = verts.detach().to(torch.float32).reshape(-1, 3).contiguous()
-    f = faces.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    v = L.dev(verts.reshape(-1, 3), dev)
+    f = L.dev(faces.reshape(-1, 3), dev, torch.int64)
     V, F = v.shape[0], f.shape[0]
     with torch.cuda.device(dev):
-        ws = torch.empty(lib.mp_largest_component_workspace_bytes(V, F), dtype=torch.uint8, device=dev)
+        ws = L.workspace(L.call("mp_largest_component_workspace_bytes", V, F), dev)
         vo = torch.empty(max(V, 1), 3, device=dev)
         fo = torch.empty(max(F, 1), 3, dtype=torch.int64, device=dev)
         Vo, Fo = C.c_int(0), C.c_int(0)
-        L.check(lib.mp_largest_component(v.data_ptr() if V else None, V, f.data_ptr() if F else None, F, vo.data_ptr(),
-                                         fo.data_ptr(), C.byref(Vo), C.byref(Fo), ws.data_ptr(), ws.numel(),
-                                         L.stream_ptr()), "mp_largest_component")
+        L.call("mp_largest_component", v if V else None, V, f if F else None, F, vo, fo, C.byref(Vo), C.byref(Fo), ws,
+               ws.numel())
         return vo[:Vo.value], fo[:Fo.value]
 
 
@@ -465,11 +402,10 @@ class Renderer:
             return self._render(inputs, hit_lists, debug, persons, check, out, train)
 
     def _render(self, inputs, hit_lists, debug, persons, check, out_bufs=None, train=None):
-        lib = L.lib()
         dev = self.device
-        uv = _dev(inputs["uv"].reshape(-1, 2), dev)
-        pose = _dev(inputs["pose"].reshape(4, 4), dev)
-        K = _dev(inputs["intrinsics"].reshape(4, 4), dev)
+        uv = L.dev(inputs["uv"].reshape(-1, 2), dev)
+        pose = L.dev(inputs["pose"].reshape(4, 4), dev)
+        K = L.dev(inputs["intrinsics"].reshape(4, 4), dev)
         R = uv.shape[0]
         plist = list(range(self.P)) if persons is None else [int(p) for p in persons]
         Pn = len(plist)
@@ -492,9 +428,9 @@ class Renderer:
             hits.append((h, cnt))
             sc.body[k] = self.bodies[p].handle
             sc.field[k] = self.fields[p].handle
-            sc.hit_index[k] = h.data_ptr()
+            sc.hit_index[k] = L.ptr(h)
             sc.hit_count[k] = h.numel()
-            sc.hit_count_dev[k] = cnt.data_ptr() if cnt is not None else None
+            sc.hit_count_dev[k] = L.ptr(cnt)
         sc.bg_field = self.bg.handle if self.bg is not None else None
         keep_train = []
         z_eik = {}
@@ -515,12 +451,10 @@ class Renderer:
                 keep_train += [rs, kp]
                 tr.rng[k] = C.pointer(rs)
                 z_eik[k] = torch.empty(hits[k][0].numel(), device=dev)
-                tr.z_eik[k] = z_eik[k].data_ptr()
-            tb = train.get("t_rand_bg")
-            if tb is not None:
-                tb = _dev(tb, dev)
-                keep_train.append(tb)
-                tr.t_rand_bg = tb.data_ptr()
+                tr.z_eik[k] = L.ptr(z_eik[k])
+            tb = L.dev(train.get("t_rand_bg"), dev)
+            keep_train.append(tb)
+            tr.t_rand_bg = L.ptr(tb)
             meshes = train.get("meshes")
             if meshes is not None:
                 assert len(meshes) == Pn and all(m is not None for m in meshes), "one canonical mesh per rendered person"
@@ -530,13 +464,13 @@ class Renderer:
                 tr.surface_threshold = float(train.get("threshold", 0.05))
                 flags = {"index_off_surface": torch.empty(R, dtype=torch.uint8, device=dev),
                          "index_in_surface": torch.empty(R, dtype=torch.uint8, device=dev)}
-                tr.index_off_surface = flags["index_off_surface"].data_ptr()
-                tr.index_in_surface = flags["index_in_surface"].data_ptr()
+                tr.index_off_surface = L.ptr(flags["index_off_surface"])
+                tr.index_in_surface = L.ptr(flags["index_in_surface"])
             keep_train.append(tr)
             sc.train = C.pointer(tr)
-        need = lib.mp_render_workspace_bytes(C.byref(sc), R)
+        need = L.call("mp_render_workspace_bytes", sc, R)
         if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            self._ws = L.workspace(need, dev)
         if self._status is None:
             self._status = torch.zeros(1, dtype=torch.int32, device=dev)
         out = L.RenderOut()
@@ -545,34 +479,32 @@ class Renderer:
         if out_bufs is not None:
             res = {k: out_bufs[k] for k in shapes}
             for k, shp in shapes.items():
-                t = res[k]
-                assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shp, k
+                assert res[k].dtype == torch.float32 and tuple(res[k].shape) == shp, k
         else:
             res = {k: torch.empty(*shp, device=dev) for k, shp in shapes.items()}
         for k, v in res.items():
-            setattr(out, k, v.data_ptr())
-        out.status = self._status.data_ptr()
+            setattr(out, k, L.ptr(v))
+        out.status = L.ptr(self._status)
         taps = {}
         if debug or grad_on:       # per-sample taps: debug outputs and the compositor's inputs for RenderComposite
             n = self.n
             taps["bg_T"] = torch.empty(R, device=dev)
-            out.bg_T = taps["bg_T"].data_ptr()
+            out.bg_T = L.ptr(taps["bg_T"])
             for k in range(Pn):
                 Rp = hits[k][0].numel()
                 for name, shp in (("z_vals", (Rp, n + 1)), ("sdf", (Rp, n)), ("rgb", (Rp, n, 3)), ("normals", (Rp, n, 3))):
                     taps[f"{name}_{k}"] = torch.empty(*shp, device=dev)
-                    getattr(out, name)[k] = taps[f"{name}_{k}"].data_ptr()
+                    getattr(out, name)[k] = L.ptr(taps[f"{name}_{k}"])
         dbg = {}
         if debug:
             assert not dev_counts, "debug taps need host-side hit counts"
             dbg = {"trips": torch.zeros(Pn, dtype=torch.int32, device=dev), **taps}
-            out.trips = dbg["trips"].data_ptr()
+            out.trips = L.ptr(dbg["trips"])
         if grad_on and self.bg is not None:
             for name, shp in (("bg_rgb", (R, 3)), ("bg_sdf", (R, 32)), ("bg_rgb_samples", (R, 32, 3))):
                 taps[name] = torch.empty(*shp, device=dev)
-                setattr(out, name, taps[name].data_ptr())
-        L.check(lib.mp_render_rays(C.byref(sc), uv.data_ptr(), pose.data_ptr(), K.data_ptr(), R, C.byref(out),
-                                   self._ws.data_ptr(), self._ws.numel(), L.stream_ptr()), "mp_render_rays")
+                setattr(out, name, L.ptr(taps[name]))
+        L.call("mp_render_rays", sc, uv, pose, K, R, out, self._ws, self._ws.numel())
         self._keep = (uv, pose, K, hits, keep_train)
         for k, v in z_eik.items():
             dbg[f"z_eik_{k}"] = v
@@ -595,7 +527,7 @@ class Renderer:
         info = dict(n=self.n, R=R, P=Pn, beta=float(beta.detach()), hits=[h[0] for h in hits], z=[d["z_vals"] for d in samples],
                     bg_T=taps["bg_T"], bound=float(self.cfg["scene_bounding_sphere"]), device=dev, bg=None)
         if self.bg is not None:
-            t_rand = None if t_rand_bg is None else _dev(t_rand_bg, dev)
+            t_rand = L.dev(t_rand_bg, dev)
             bg = dict(sdf=taps["bg_sdf"].clone().requires_grad_(True),
                       rgb=taps["bg_rgb_samples"].clone().requires_grad_(True), t_rand=t_rand, bg_rgb=taps["bg_rgb"])
             leaves += [bg["sdf"], bg["rgb"]]
@@ -628,41 +560,31 @@ class RenderComposite(torch.autograd.Function):
         info = ctx.info
         leaves = ctx.saved_tensors
         dev, R, P, n = info["device"], info["R"], info["P"], info["n"]
-        lib = L.lib()
-
-        def g(t):
-            return None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous()
-        d_rgb, d_fgv, d_nrm, d_acc, d_accp = (g(t) for t in (d_rgb, d_fgv, d_nrm, d_acc, d_accp))
+        d_rgb, d_fgv, d_nrm, d_acc, d_accp = (L.dev(t, dev) for t in (d_rgb, d_fgv, d_nrm, d_acc, d_accp))
         with torch.cuda.device(dev):
-            st = L.stream_ptr()
             if d_rgb is None:
                 d_rgb = torch.zeros(R, 3, device=dev)
             bg = info["bg"]
             d_fg = torch.empty(R, 3, device=dev)
             d_bgT = torch.empty(R, device=dev)
             d_bg = torch.empty(R, 3, device=dev) if bg is not None else None
-            L.check(lib.mp_final_compose_backward(info["bg_T"].data_ptr(), L.ptr(bg["rgb"]) if bg else None, R,
-                                                  d_rgb.data_ptr(), L.ptr(d_fgv), d_fg.data_ptr(), d_bgT.data_ptr(),
-                                                  L.ptr(d_bg), st), "mp_final_compose_backward")
+            L.call("mp_final_compose_backward", info["bg_T"], bg["rgb"] if bg else None, R, d_rgb, d_fgv, d_fg, d_bgT, d_bg)
             arr = person_samples([(info["hits"][k], info["z"][k], *leaves[3 * k: 3 * k + 3], info["hits"][k].numel())
                                   for k in range(P)])
             gr = (L.PersonSampleGrads * P)()
             grads = []
             for k in range(P):
                 gk = tuple(torch.empty_like(t) for t in leaves[3 * k: 3 * k + 3])
-                gr[k].d_sdf, gr[k].d_rgb, gr[k].d_normal = (t.data_ptr() for t in gk)
+                gr[k].d_sdf, gr[k].d_rgb, gr[k].d_normal = (L.ptr(t) for t in gk)
                 grads += gk
             d_beta = torch.empty(1, device=dev)
-            ws = torch.empty(lib.mp_composite_backward_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
-            L.check(lib.mp_composite_backward(arr, P, R, n, info["beta"], d_fg.data_ptr(), L.ptr(d_nrm), L.ptr(d_acc),
-                                              L.ptr(d_accp), d_bgT.data_ptr(), gr, d_beta.data_ptr(), ws.data_ptr(),
-                                              ws.numel(), st), "mp_composite_backward")
+            ws = L.workspace(L.call("mp_composite_backward_workspace_bytes", R, P), dev)
+            L.call("mp_composite_backward", arr, P, R, n, info["beta"], d_fg, d_nrm, d_acc, d_accp, d_bgT, gr, d_beta, ws,
+                   ws.numel())
             if bg is not None:
                 b_sdf, b_rgb = leaves[3 * P], leaves[3 * P + 1]
                 d_bsdf, d_brgb = torch.empty_like(b_sdf), torch.empty_like(b_rgb)
-                L.check(lib.mp_bg_composite_backward(b_sdf.data_ptr(), b_rgb.data_ptr(), R, info["bound"],
-                                                     L.ptr(bg["t_rand"]), d_bg.data_ptr(), d_bsdf.data_ptr(),
-                                                     d_brgb.data_ptr(), st), "mp_bg_composite_backward")
+                L.call("mp_bg_composite_backward", b_sdf, b_rgb, R, info["bound"], bg["t_rand"], d_bg, d_bsdf, d_brgb)
                 grads += [d_bsdf, d_brgb]
         return (None, None, d_beta.reshape(ctx.beta_shape)) + tuple(grads)
 
@@ -672,7 +594,7 @@ def person_samples(persons):
     tensors alive while the array is in use."""
     arr = (L.PersonSamples * len(persons))()
     for a, (idx, z, sdf, rgb, nrm, n_rows) in zip(arr, persons):
-        a.ray_index, a.z_vals, a.sdf, a.rgb, a.normal = (t.data_ptr() for t in (idx, z, sdf, rgb, nrm))
+        a.ray_index, a.z_vals, a.sdf, a.rgb, a.normal = (L.ptr(t) for t in (idx, z, sdf, rgb, nrm))
         a.n_rows = n_rows
     return arr
 
@@ -680,14 +602,11 @@ def person_samples(persons):
 def sampler_rng_struct(rng, dev):
     """mp_sampler_rng_t from the tabled draws of ``ErrorBoundSampler.draw_training_rng`` (t_rand [R,E], u_final [R,S],
     extra_perm [T,T*E] int32, eik_idx [T,R] int32, t_rand_bg [T,R,32]); returns (struct, tensors to keep alive)."""
-    keep = {"t_rand": rng["t_rand"].to(device=dev, dtype=torch.float32).contiguous(),
-            "u_final": rng["u_final"].to(device=dev, dtype=torch.float32).contiguous(),
-            "extra_perm": rng["extra_perm"].to(device=dev, dtype=torch.int32).contiguous(),
-            "eik_idx": rng["eik_idx"].to(device=dev, dtype=torch.int32).contiguous(),
-            "t_rand_bg": rng["t_rand_bg"].to(device=dev, dtype=torch.float32).contiguous()}
+    keep = {k: L.dev(rng[k], dev, torch.int32 if k in ("extra_perm", "eik_idx") else torch.float32)
+            for k in ("t_rand", "u_final", "extra_perm", "eik_idx", "t_rand_bg")}
     r = L.SamplerRng()
     for k, v in keep.items():
-        setattr(r, k, v.data_ptr())
+        setattr(r, k, L.ptr(v))
     return r, keep
 
 
@@ -701,7 +620,7 @@ class GraphedRender:
     def __init__(self, renderer, inputs, hit_lists, persons=None):
         self.r = renderer
         dev = renderer.device
-        self.inputs = {k: _dev(inputs[k], dev).clone() for k in ("uv", "pose", "intrinsics")}
+        self.inputs = {k: L.dev(inputs[k], dev).clone() for k in ("uv", "pose", "intrinsics")}
         self.hits = [tuple(t.to(dev) for t in h) if isinstance(h, (tuple, list)) else h.to(dev).clone() for h in hit_lists]
         self.persons = persons
         with torch.cuda.device(dev):
@@ -725,18 +644,14 @@ def ray_aabb_hits(cam_loc, ray_dirs, verts, inflate=1.2):
     """Device-side culling against the x`inflate` axis-aligned box of `verts` [V,3] (multiply.py:208-214 uses trimesh's
     oriented box; see INTEGRATION.md): returns (ids [R] int64, count [1] int32), both on the device, the list already
     finalised (empty -> ray 0, multiply.py:262-263).  No host synchronisation: feed the pair to ``Renderer.render``."""
-    lib = L.lib()
     dev = cam_loc.device
-    cam = cam_loc.detach().contiguous().float()
-    d = ray_dirs.detach().contiguous().float()
-    v = verts.detach().reshape(-1, 3).contiguous().float()
+    cam, d, v = L.dev(cam_loc, dev), L.dev(ray_dirs, dev), L.dev(verts.reshape(-1, 3), dev)
     R = cam.shape[0]
     with torch.cuda.device(dev):
         idx = torch.empty(R, dtype=torch.int64, device=dev)
         cnt = torch.zeros(1, dtype=torch.int32, device=dev)
         box = torch.empty(8, dtype=torch.float64, device=dev)
-        L.check(lib.mp_ray_aabb_hits(cam.data_ptr(), d.data_ptr(), R, v.data_ptr(), v.shape[0], float(inflate),
-                                     idx.data_ptr(), cnt.data_ptr(), box.data_ptr(), L.stream_ptr()), "mp_ray_aabb_hits")
+        L.call("mp_ray_aabb_hits", cam, d, R, v, v.shape[0], float(inflate), idx, cnt, box)
     return idx, cnt
 
 
@@ -745,22 +660,15 @@ def ray_box_hits(cam_loc, ray_dirs, center, half_extent, rot=None, device_count=
     device->host read for the count — the reference pays a full `.cpu()` round trip plus trimesh here
     (multiply.py:256).  ``device_count=True`` returns (ids [R], count [1]) with the count left on the device and the
     list finalised (empty -> ray 0, mp_hit_list_finalize), the form ``Renderer.render`` takes without a host read."""
-    lib = L.lib()
     dev = cam_loc.device
-    cam = cam_loc.detach().contiguous().float()
-    d = ray_dirs.detach().contiguous().float()
+    cam, d = L.dev(cam_loc, dev), L.dev(ray_dirs, dev)
     R = cam.shape[0]
-    c = (C.c_double * 3)(*[float(v) for v in center])
-    h = (C.c_double * 3)(*[float(v) for v in half_extent])
     with torch.cuda.device(dev):
         idx = torch.empty(R, dtype=torch.int64, device=dev)
         cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        rot_d = None
-        if rot is not None:
-            rot_d = torch.as_tensor(rot, dtype=torch.float64).reshape(9).to(dev).contiguous()
-        L.check(lib.mp_ray_box_hits(cam.data_ptr(), d.data_ptr(), R, c, h, L.ptr(rot_d), idx.data_ptr(), cnt.data_ptr(),
-                                    L.stream_ptr()), "mp_ray_box_hits")
+        rot_d = None if rot is None else L.dev(torch.as_tensor(rot).reshape(9), dev, torch.float64)
+        L.call("mp_ray_box_hits", cam, d, R, L.vec3(C.c_double, center), L.vec3(C.c_double, half_extent), rot_d, idx, cnt)
         if device_count:
-            L.check(lib.mp_hit_list_finalize(idx.data_ptr(), cnt.data_ptr(), L.stream_ptr()), "mp_hit_list_finalize")
+            L.call("mp_hit_list_finalize", idx, cnt)
             return idx, cnt
     return idx[: int(cnt.item())]

@@ -34,9 +34,9 @@ class LaplaceDensity(Density):
         if torch.is_tensor(beta) and beta.numel() > 1:
             raise NotImplementedError("per-ray beta lives inside the fused sampler (mp_sample_rays)")
         b = float(beta.detach()) if torch.is_tensor(beta) else float(beta)
-        s = sdf.detach().contiguous().float()
+        s = L.dev(sdf, sdf.device)
         out = torch.empty_like(s)
-        L.check(L.lib().mp_laplace_density(L.ptr(s), s.numel(), b, L.ptr(out), L.stream_ptr()), "mp_laplace_density")
+        L.call("mp_laplace_density", s, s.numel(), b, out)
         return out.reshape(sdf.shape)
 
 

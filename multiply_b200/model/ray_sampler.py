@@ -1,5 +1,4 @@
 """Mirror of /root/reference/code/lib/model/ray_sampler.py (ErrorBoundSampler, eval mode)."""
-import ctypes as C
 import torch
 
 from .. import _lib as L
@@ -28,7 +27,6 @@ class ErrorBoundSampler:
         """model: object exposing ``density`` (LaplaceDensity), ``deformer_list`` and ``field_list`` —
         model.multiply.Multiply does."""
         training = bool(getattr(model, "training", False))
-        lib = L.lib()
         dev = ray_dirs.device
         R = ray_dirs.shape[0]
         c = engine.sampler_cfg(self.cfg, float(model.density.beta.detach()), float(model.density.beta_min))
@@ -39,16 +37,13 @@ class ErrorBoundSampler:
         z = torch.empty(R, engine.samples_per_ray(self.cfg) + 1, device=dev)
         z_bg = torch.empty(R, 32, device=dev)
         trips = torch.zeros(1, dtype=torch.int32, device=dev)
-        need = lib.mp_sampler_workspace_bytes(C.byref(c), R)
+        need = L.call("mp_sampler_workspace_bytes", c, R)
         if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        d = ray_dirs.detach().contiguous().float()
-        o = cam_loc.detach().contiguous().float()
+            self._ws = L.workspace(need, dev)
+        d, o = L.dev(ray_dirs, dev), L.dev(cam_loc, dev)
         if training:
-            return self._get_z_vals_training(lib, c, body, field, d, o, R, z, z_bg, trips, dev, rng=rng)
-        L.check(lib.mp_sample_rays(C.byref(c), body.handle, field.handle, d.data_ptr(), o.data_ptr(), R, z.data_ptr(),
-                                   z_bg.data_ptr(), trips.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                   L.stream_ptr()), "mp_sample_rays")
+            return self._get_z_vals_training(L.lib(), c, body, field, d, o, R, z, z_bg, trips, dev, rng=rng)
+        L.call("mp_sample_rays", c, body.handle, field.handle, d, o, R, z, z_bg, trips, self._ws, self._ws.numel())
         self.last_trips = trips
         # z_samples_eik only feeds the training-time eikonal term (ray_sampler.py:211-213)
         return (z, z_bg), z[:, :1]
@@ -85,9 +80,8 @@ class ErrorBoundSampler:
             rng = self.draw_training_rng(R)
         r, dv = engine.sampler_rng_struct(rng, dev)
         z_eik = torch.empty(R, device=dev)
-        L.check(lib.mp_sample_rays_train(C.byref(c), body.handle, field.handle, d.data_ptr(), o.data_ptr(), R, C.byref(r),
-                                         z.data_ptr(), z_bg.data_ptr(), z_eik.data_ptr(), trips.data_ptr(),
-                                         self._ws.data_ptr(), self._ws.numel(), L.stream_ptr()), "mp_sample_rays_train")
+        L.call("mp_sample_rays_train", c, body.handle, field.handle, d, o, R, r, z, z_bg, z_eik, trips, self._ws,
+               self._ws.numel())
         self.last_trips = trips
         if "states" in rng:
             # leave the generator where the reference would be: after the draws of the trip count the loop took

@@ -2,6 +2,8 @@
 import torch
 import torch.nn.functional as F
 
+from .. import _lib as L
+
 
 def get_camera_params_host(uv, pose, intrinsics):
     """Host (CPU) evaluation of get_camera_params (rend_util.py:45-87) used only to build
@@ -44,34 +46,34 @@ def pose_matrix(pose):
     return out
 
 
-def get_camera_params(uv, pose, intrinsics):
-    """rend_util.get_camera_params (rend_util.py:45-72) on the device: uv [1,R,2], pose [1,4,4] (or [1,7] quaternion
-    form), intrinsics [1,4,4] -> (ray_dirs [1,R,3], cam_loc [1,3])."""
-    from .. import _lib as L
+def camera_rays(uv, pose, intrinsics):
+    """mp_camera_rays on uv's device: uv [R,2] (or [1,R,2]), pose and intrinsics as ``get_camera_params`` takes them ->
+    (ray_dirs [R,3], cam_loc [R,3], the camera centre once per ray)."""
     dev = uv.device
-    pose = pose_matrix(pose)
-    f = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
-    u, p, k = f(uv.reshape(-1, 2)), f(pose.reshape(4, 4)), f(intrinsics.reshape(4, 4))
+    u, p, k = (L.dev(t, dev) for t in (uv.reshape(-1, 2), pose_matrix(pose).reshape(4, 4), intrinsics.reshape(4, 4)))
     R = u.shape[0]
     dirs = torch.empty(R, 3, device=dev)
     cam = torch.empty(R, 3, device=dev)
-    L.check(L.lib().mp_camera_rays(u.data_ptr(), p.data_ptr(), k.data_ptr(), R, dirs.data_ptr(), cam.data_ptr(),
-                                   L.stream_ptr()), "mp_camera_rays")
+    L.call("mp_camera_rays", u, p, k, R, dirs, cam)
+    return dirs, cam
+
+
+def get_camera_params(uv, pose, intrinsics):
+    """rend_util.get_camera_params (rend_util.py:45-72) on the device: uv [1,R,2], pose [1,4,4] (or [1,7] quaternion
+    form), intrinsics [1,4,4] -> (ray_dirs [1,R,3], cam_loc [1,3])."""
+    dirs, cam = camera_rays(uv, pose, intrinsics)
     return dirs[None], cam[:1]
 
 
 def get_sphere_intersections(cam_loc, ray_directions, r=1.0):
     """rend_util.get_sphere_intersections (rend_util.py:131-147): [R,3],[R,3] -> [R,2]; raises where the reference
     calls exit() (a ray missing the bounding sphere)."""
-    from .. import _lib as L
     dev = cam_loc.device
-    c = cam_loc.detach().contiguous().float()
-    d = ray_directions.detach().contiguous().float()
+    c, d = L.dev(cam_loc, dev), L.dev(ray_directions, dev)
     R = c.shape[0]
     out = torch.empty(R, 2, device=dev)
     flag = torch.zeros(1, dtype=torch.int32, device=dev)
-    L.check(L.lib().mp_sphere_intersections(c.data_ptr(), d.data_ptr(), R, float(r), out.data_ptr(), flag.data_ptr(),
-                                            L.stream_ptr()), "mp_sphere_intersections")
+    L.call("mp_sphere_intersections", c, d, R, float(r), out, flag)
     if int(flag.item()):
         raise RuntimeError("BOUNDING SPHERE PROBLEM!")
     return out

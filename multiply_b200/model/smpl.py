@@ -16,31 +16,26 @@ class SMPLServer(torch.nn.Module):
         super().__init__()
         if model is None:
             raise ValueError("SMPL model files are licence-gated: pass model=dict(v_template, shapedirs, ...)")
-        lib = L.lib()
         dev = torch.device(device)
-        f = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
-        self._arr = {k: f(model[k]) for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "lbs_weights")}
+        self._arr = {k: L.dev(model[k], dev) for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "lbs_weights")}
         if v_template is not None:
-            self._arr["v_template"] = f(torch.as_tensor(v_template))
+            self._arr["v_template"] = L.dev(torch.as_tensor(v_template), dev)
         self.V = self._arr["v_template"].shape[0]
         par = [int(p) for p in model["parents"]]
         par[0] = -1
         self.bone_parents = np.array(par)
-        self.betas = f(torch.as_tensor(betas)) if betas is not None else None
+        self.betas = L.dev(torch.as_tensor(betas), dev) if betas is not None else None
         pa = (C.c_int * 24)(*[max(p, 0) for p in par])
-        nbytes = lib.mp_smpl_bytes(self.V)
-        self._storage = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        h = C.c_void_p()
+        self._storage = L.workspace(L.call("mp_smpl_bytes", self.V), dev)
+        self.handle = L.Handle("mp_smpl_free")
         a = self._arr
-        L.check(lib.mp_smpl_create(a["v_template"].data_ptr(), a["shapedirs"].data_ptr(), a["posedirs"].data_ptr(),
-                                   a["J_regressor"].data_ptr(), pa, a["lbs_weights"].data_ptr(), self.V,
-                                   L.ptr(self.betas.reshape(-1)) if self.betas is not None and v_template is None else None,
-                                   self._storage.data_ptr(), nbytes, C.byref(h), L.stream_ptr()), "mp_smpl_create")
-        self.handle = h
+        L.call("mp_smpl_create", a["v_template"], a["shapedirs"], a["posedirs"], a["J_regressor"], pa, a["lbs_weights"],
+               self.V, self.betas.reshape(-1) if self.betas is not None and v_template is None else None,
+               self._storage, self._storage.numel(), C.byref(self.handle))
         self.device = dev
         vc = torch.empty(self.V, 3, device=dev)
         ti = torch.empty(24, 4, 4, device=dev)
-        L.check(lib.mp_smpl_canonical(h, vc.data_ptr(), ti.data_ptr(), L.stream_ptr()), "mp_smpl_canonical")
+        L.call("mp_smpl_canonical", self.handle, vc, ti)
         self.verts_c = vc[None]                      # smpl.py:45
         self.tfs_c_inv = ti                          # smpl.py:47
         self.weights = a["lbs_weights"][None]
@@ -50,14 +45,11 @@ class SMPLServer(torch.nn.Module):
 
     def forward(self, scale, transl, thetas, betas, absolute=False):
         """smpl.py:50-95: scale [1], transl [1,3], thetas [1,72], betas [1,10] -> dict."""
-        lib = L.lib()
         dev = self.device
-        f = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous().reshape(-1)
-        s, t, th, b = f(scale), f(transl), f(thetas), f(betas)
+        s, t, th, b = (L.dev(x.reshape(-1), dev) for x in (scale, transl, thetas, betas))
         verts = torch.empty(self.V, 3, device=dev)
         tfs = torch.empty(24, 4, 4, device=dev)
-        L.check(lib.mp_smpl_forward(self.handle, s.data_ptr(), t.data_ptr(), th.data_ptr(), b.data_ptr(), int(absolute),
-                                    verts.data_ptr(), tfs.data_ptr(), L.stream_ptr()), "mp_smpl_forward")
+        L.call("mp_smpl_forward", self.handle, s, t, th, b, int(absolute), verts, tfs)
         self._keep = (s, t, th, b)
         return {"smpl_verts": verts[None], "smpl_tfs": tfs[None], "smpl_weights": self.weights}
 
@@ -66,10 +58,3 @@ class SMPLServer(torch.nn.Module):
         th[0, 5], th[0, 8] = np.pi / 6, -np.pi / 6
         b = self.betas.reshape(1, 10) if self.betas is not None else torch.zeros(1, 10)
         return self(torch.ones(1), torch.zeros(1, 3), th, b)
-
-    def __del__(self):
-        try:
-            if getattr(self, "handle", None):
-                L.lib().mp_smpl_free(self.handle)
-        except Exception:
-            pass

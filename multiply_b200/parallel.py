@@ -8,6 +8,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L, engine
+from .model import rend_util
 
 PIXEL_KEYS = ("rgb_values", "fg_rgb_values", "normal_values", "acc_map", "acc_person_list")
 
@@ -181,7 +182,6 @@ class PersonShardedRenderer:
 
     def composite_block(self, inputs, hits, got, lo, hi):
         """Step 3 for the ray block [lo, hi)."""
-        lib = L.lib()
         dev = self.device
         n, Rb = self.n, hi - lo
         keep = []
@@ -206,27 +206,16 @@ class PersonShardedRenderer:
         bgT = torch.empty(Rb, device=dev)
         if Rb == 0:
             return out
-        ws = torch.empty(lib.mp_composite_workspace_bytes(Rb, self.P), dtype=torch.uint8, device=dev)
-        L.check(lib.mp_composite(persons, self.P, Rb, n, self.beta, fg.data_ptr(), out["normal_values"].data_ptr(),
-                                 out["acc_map"].data_ptr(), out["acc_person_list"].data_ptr(), bgT.data_ptr(),
-                                 ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_composite")
+        ws = L.workspace(L.call("mp_composite_workspace_bytes", Rb, self.P), dev)
+        L.call("mp_composite", persons, self.P, Rb, n, self.beta, fg, out["normal_values"], out["acc_map"],
+               out["acc_person_list"], bgT, ws, ws.numel())
         bg = None
         if self.bg is not None:
-            uv = inputs["uv"].reshape(-1, 2)[lo:hi].to(device=dev, dtype=torch.float32).contiguous()
-            pose = inputs["pose"].reshape(4, 4).to(device=dev, dtype=torch.float32).contiguous()
-            K = inputs["intrinsics"].reshape(4, 4).to(device=dev, dtype=torch.float32).contiguous()
-            dirs = torch.empty(Rb, 3, device=dev)
-            cam = torch.empty(Rb, 3, device=dev)
-            L.check(lib.mp_camera_rays(uv.data_ptr(), pose.data_ptr(), K.data_ptr(), Rb, dirs.data_ptr(), cam.data_ptr(),
-                                       L.stream_ptr()), "mp_camera_rays")
-            bg = torch.empty(Rb, 3, device=dev)
-            bws = torch.empty(lib.mp_background_workspace_bytes(Rb), dtype=torch.uint8, device=dev)
-            L.check(lib.mp_background(self.bg.handle, dirs.data_ptr(), cam.data_ptr(), Rb,
-                                      float(self.cfg["scene_bounding_sphere"]), bg.data_ptr(), bws.data_ptr(), bws.numel(),
-                                      L.stream_ptr()), "mp_background")
-            keep += [uv, pose, K, dirs, cam, bws]
-        L.check(lib.mp_final_compose(fg.data_ptr(), bgT.data_ptr(), L.ptr(bg), Rb, out["rgb_values"].data_ptr(),
-                                     out["fg_rgb_values"].data_ptr(), L.stream_ptr()), "mp_final_compose")
+            uv = L.dev(inputs["uv"].reshape(-1, 2)[lo:hi], dev)
+            dirs, cam = rend_util.camera_rays(uv, inputs["pose"], inputs["intrinsics"])
+            bg = self.bg.bg_pixels(dirs, cam, self.cfg["scene_bounding_sphere"])
+            keep += [uv, dirs, cam]
+        L.call("mp_final_compose", fg, bgT, bg, Rb, out["rgb_values"], out["fg_rgb_values"])
         self._keep = keep + [fg, bgT, bg, ws]
         return out
 

@@ -502,3 +502,17 @@ def test_abi_reports_errors():
     assert rc != 0 and b"null argument" in lib.mp_last_error()
     with pytest.raises(L.MpError):
         L.check(rc, "mp_sample_rays")
+
+
+def test_call_refuses_a_strided_tensor():
+    """``_lib.call`` checks every tensor before the library is entered: a transposed (non-contiguous) CUDA tensor raises
+    MpError naming the function and the argument, and nothing is enqueued."""
+    from multiply_b200 import _lib as L
+    s = torch.rand(4, 6, device="cuda").t()
+    out = torch.empty(24, device="cuda")
+    before = L.call("mp_launch_count", 0)
+    with pytest.raises(L.MpError, match="mp_laplace_density, argument 0: expected a contiguous tensor"):
+        L.call("mp_laplace_density", s, 24, 0.1, out)
+    assert L.call("mp_launch_count", 0) == before
+    L.call("mp_laplace_density", s.contiguous(), 24, 0.1, out)
+    assert L.call("mp_launch_count", 0) > before
