@@ -47,7 +47,6 @@ def _time(fn, steps):
 
 def workload(P, R, n, steps):
     from multiply_b200 import _lib as L, engine
-    lib = L.lib()
     g = torch.Generator(device="cuda").manual_seed(R + n)
     dev = "cuda"
     gr = (L.PersonSampleGrads * P)()
@@ -60,7 +59,7 @@ def workload(P, R, n, steps):
                  d_sdf=torch.empty(R, n, device=dev), d_rgb=torch.empty(R, n, 3, device=dev),
                  d_nrm=torch.empty(R, n, 3, device=dev))
         keep.append(t)
-        gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = t["d_sdf"].data_ptr(), t["d_rgb"].data_ptr(), t["d_nrm"].data_ptr()
+        gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = (L.ptr(t[k]) for k in ("d_sdf", "d_rgb", "d_nrm"))
     arr = engine.person_samples([(t["idx"], t["z"], t["sdf"], t["rgb"], t["nrm"], R) for t in keep])
     o = {k: torch.empty(*s, device=dev) for k, s in (("fg", (R, 3)), ("nrm", (R, 3)), ("acc", (R,)), ("accp", (R, P)),
                                                      ("bgT", (R,)))}
@@ -72,28 +71,22 @@ def workload(P, R, n, steps):
     d_bg_sdf, d_bg_rgb_s = torch.empty(R, 32, device=dev), torch.empty(R, 32, 3, device=dev)
     d_fg, d_bgT, d_bg = torch.empty(R, 3, device=dev), torch.empty(R, device=dev), torch.empty(R, 3, device=dev)
     d_beta = torch.empty(1, device=dev)
-    ws = torch.empty(lib.mp_composite_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
-    wsb = torch.empty(lib.mp_composite_backward_workspace_bytes(R, P), dtype=torch.uint8, device=dev)
-    st = L.stream_ptr()
+    ws = L.workspace(L.call("mp_composite_workspace_bytes", R, P), dev)
+    wsb = L.workspace(L.call("mp_composite_backward_workspace_bytes", R, P), dev)
     beta = 0.1
 
     def fwd():
-        L.check(lib.mp_composite(arr, P, R, n, beta, o["fg"].data_ptr(), o["nrm"].data_ptr(), o["acc"].data_ptr(),
-                                 o["accp"].data_ptr(), o["bgT"].data_ptr(), ws.data_ptr(), ws.numel(), st), "mp_composite")
+        L.call("mp_composite", arr, P, R, n, beta, o["fg"], o["nrm"], o["acc"], o["accp"], o["bgT"], ws, ws.numel())
 
     def blend_bwd():
-        L.check(lib.mp_final_compose_backward(o["bgT"].data_ptr(), bg_rgb.data_ptr(), R, u["rgb"].data_ptr(),
-                                              u["fg"].data_ptr(), d_fg.data_ptr(), d_bgT.data_ptr(), d_bg.data_ptr(), st),
-                "mp_final_compose_backward")
+        L.call("mp_final_compose_backward", o["bgT"], bg_rgb, R, u["rgb"], u["fg"], d_fg, d_bgT, d_bg)
 
     def comp_bwd():
-        L.check(lib.mp_composite_backward(arr, P, R, n, beta, d_fg.data_ptr(), u["nrm"].data_ptr(), u["acc"].data_ptr(),
-                                          u["accp"].data_ptr(), d_bgT.data_ptr(), gr, d_beta.data_ptr(), wsb.data_ptr(),
-                                          wsb.numel(), st), "mp_composite_backward")
+        L.call("mp_composite_backward", arr, P, R, n, beta, d_fg, u["nrm"], u["acc"], u["accp"], d_bgT, gr, d_beta, wsb,
+               wsb.numel())
 
     def bg_bwd():
-        L.check(lib.mp_bg_composite_backward(bg_sdf.data_ptr(), bg_rgb_s.data_ptr(), R, 3.0, None, d_bg.data_ptr(),
-                                             d_bg_sdf.data_ptr(), d_bg_rgb_s.data_ptr(), st), "mp_bg_composite_backward")
+        L.call("mp_bg_composite_backward", bg_sdf, bg_rgb_s, R, 3.0, None, d_bg, d_bg_sdf, d_bg_rgb_s)
 
     def all_bwd():
         blend_bwd()

@@ -38,10 +38,11 @@ def _card():
         return {"card": torch.cuda.get_device_name(), "power_limit_w": None, "sm_max_mhz": None}
 
 
-def _grid(lib):
+def _grid():
     """Persistent CTAs of a launch with at least as many tiles (csrc/mlp_tc.cu tc_launch): one per SM, capped by
     MP_TC_GRID.  A launch with fewer tiles than that runs one CTA per tile, which this figure does not account for."""
-    g = lib.mp_device_sm_count()
+    from multiply_b200 import _lib as L
+    g = L.call("mp_device_sm_count")
     env = int(os.environ.get("MP_TC_GRID", "0") or 0)
     return min(g, env) if env > 0 else g
 
@@ -50,7 +51,6 @@ def measure(steps):
     from multiply_b200 import engine, scene as S, _lib as L
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
-    lib = L.lib()
     engine.set_engine("tc")
     sc, _, _ = S.make_smpl_scene(P=2, S=128, seed=42, device=dev)
     inp = S.make_rays(sc, 4096, seed=1234, region="boxes")
@@ -59,19 +59,19 @@ def measure(steps):
     d_inp = {k: v.to(dev) for k, v in inp.items()}
     d_hits = [h.to(dev) for h in hits]
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    L.check(lib.mp_set_streams(0), "mp_set_streams")
+    L.call("mp_set_streams", 0)
     for _ in range(3):
         r.render(d_inp, d_hits)
     torch.cuda.synchronize()
-    L.check(lib.mp_profile_enable(1), "mp_profile_enable")
+    L.call("mp_profile_enable", 1)
     for i in range(steps):
         flush.fill_(i & 0xFF)
         r.render(d_inp, d_hits)
     torch.cuda.synchronize()
-    L.check(lib.mp_profile_enable(0), "mp_profile_enable")
+    L.call("mp_profile_enable", 0)
     pms, pl, pp = (C.c_double * 4)(), (C.c_longlong * 4)(), (C.c_double * 4)()
-    L.check(lib.mp_profile_read(pms, pl, pp, 1), "mp_profile_read")
-    grid = _grid(lib)
+    L.call("mp_profile_read", pms, pl, pp, 1)
+    grid = _grid()
     rec = {"MP_TC_GRID": os.environ.get("MP_TC_GRID"), "grid": grid, "steps": steps,
            "kernel_ms_per_step": sum(pms) / steps}
     for k, name in enumerate(KINDS):

@@ -21,7 +21,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-SENTINEL = -1234.5
+from _abi import SENTINEL, padded, take     # noqa: E402
+
 SMEM_CAP = 200 * 1024                   # launch_composite: dynamic shared memory of one block
 N_MAX_P8 = SMEM_CAP // (12 * 8)         # 2133: the largest n with 12 * P * n <= 200 KB at P = 8
 # fp64 comparison gate of every output (fg_rgb, normal, acc, acc_person, bg_T); the measured worst values are quoted in
@@ -156,54 +157,45 @@ def subset(persons, rays):
 
 
 # ---------------------------------------------------------------------------------------------
-# the C ABI with sentinel-padded outputs (as tests/test_gpu_networks.py)
+# the C ABI with sentinel-padded outputs
 # ---------------------------------------------------------------------------------------------
-
-def _out(N, width):
-    return torch.full(((N + 128) * width,), SENTINEL, device="cuda")
-
-
-def _take(buf, N, width, what):
-    tail = buf[N * width:]
-    assert bool((tail == SENTINEL).all()), "%s: %d values written past R = %d" % (what, int((tail != SENTINEL).sum()), N)
-    return buf[:N * width].reshape(N, width).cpu().numpy() if width > 1 else buf[:N].cpu().numpy()
-
 
 def wpc_of(P, n):
     """Rays per block of launch_composite."""
     return max(1, min(8, SMEM_CAP // (12 * P * n)))
 
 
-def call_composite(persons, R, n, beta, P_arg=None, ws_delta=0):
-    """(status, outputs or the untouched-check of the raw buffers)."""
-    from multiply_b200 import _lib as L
-    lib = L.lib()
-    P = len(persons)
-    arr = (L.PersonSamples * max(P, 1))()
+def person_samples(persons):
+    """(mp_person_samples_t array, the device tensors it points to); a person without rays gets one-element
+    placeholders, so that every pointer is valid."""
+    from multiply_b200 import engine
     keep = []
-    for p, d in enumerate(persons):
-        dev = {k: torch.from_numpy(d[k]).cuda() if d["idx"].size else torch.zeros(1, device="cuda")
-               for k in ("z", "sdf", "rgb", "nrm")}
-        dev["idx"] = torch.from_numpy(d["idx"]).cuda() if d["idx"].size else torch.zeros(1, dtype=torch.int64,
-                                                                                         device="cuda")
-        keep.append(dev)
-        arr[p].n_rows = int(d["idx"].size)
-        arr[p].ray_index = dev["idx"].data_ptr()
-        arr[p].z_vals = dev["z"].data_ptr()
-        arr[p].sdf = dev["sdf"].data_ptr()
-        arr[p].rgb = dev["rgb"].data_ptr()
-        arr[p].normal = dev["nrm"].data_ptr()
-    bufs = dict(fg=_out(R, 3), nrm=_out(R, 3), acc=_out(R, 1), accp=_out(R, P), bgT=_out(R, 1))
-    ws_bytes = lib.mp_composite_workspace_bytes(R, P) + ws_delta
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device="cuda")
-    rc = lib.mp_composite(arr, P if P_arg is None else P_arg, R, n, float(beta), bufs["fg"].data_ptr(),
-                          bufs["nrm"].data_ptr(), bufs["acc"].data_ptr(), bufs["accp"].data_ptr(), bufs["bgT"].data_ptr(),
-                          ws.data_ptr(), ws_bytes, L.stream_ptr())
+    for d in persons:
+        if d["idx"].size:
+            keep.append([torch.from_numpy(np.ascontiguousarray(d[k])).cuda() for k in ("idx", "z", "sdf", "rgb", "nrm")])
+        else:
+            keep.append([torch.zeros(1, dtype=torch.int64, device="cuda")] + [torch.zeros(1, device="cuda")] * 4)
+    return engine.person_samples([t + [int(d["idx"].size)] for t, d in zip(keep, persons)]), keep
+
+
+def outputs(R, P):
+    return dict(fg=padded((R, 3)), nrm=padded((R, 3)), acc=padded(R), accp=padded((R, P)), bgT=padded(R))
+
+
+def call_composite(persons, R, n, beta, P_arg=None, ws_delta=0, bufs=None):
+    """The five outputs on the host, read from ``bufs`` (fresh ``outputs`` by default)."""
+    from multiply_b200 import _lib as L
+    P = len(persons)
+    arr, keep = person_samples(persons)
+    bufs = outputs(R, P) if bufs is None else bufs
+    ws_bytes = L.call("mp_composite_workspace_bytes", R, P) + ws_delta
+    ws = L.workspace(ws_bytes, "cuda")
+    L.call("mp_composite", arr, P if P_arg is None else P_arg, R, n, float(beta), bufs["fg"], bufs["nrm"], bufs["acc"],
+           bufs["accp"], bufs["bgT"], ws, ws_bytes)
     torch.cuda.synchronize()
-    if rc != 0:
-        return rc, bufs
-    return rc, (_take(bufs["fg"], R, 3, "fg_rgb"), _take(bufs["nrm"], R, 3, "normal"), _take(bufs["acc"], R, 1, "acc"),
-                _take(bufs["accp"], R, P, "acc_person").reshape(R, P), _take(bufs["bgT"], R, 1, "bg_T"))
+    return tuple(take(bufs[k], shp, name).numpy() for k, shp, name in (
+        ("fg", (R, 3), "fg_rgb"), ("nrm", (R, 3), "normal"), ("acc", R, "acc"), ("accp", (R, P), "acc_person"),
+        ("bgT", R, "bg_T")))
 
 
 NAMES = ("fg_rgb", "normal", "acc", "acc_person", "bg_T")
@@ -232,8 +224,7 @@ def test_composite_vs_fp64(P, n, beta):
     Rs = sorted({1, max(1, wpc - 1), wpc, wpc + 1, 2 * wpc + 1, 3 * wpc + 5})
     for R in Rs:
         persons = make_inputs(1000 * P + n + R, P, R, n, substitute=(R % 2 == 1))
-        rc, got = call_composite(persons, R, n, beta)
-        assert rc == 0
+        got = call_composite(persons, R, n, beta)
         want = composite_ref(persons, R, n, np.float32(beta))
         e = _errs(got, want)
         key = (P, n, beta, R)
@@ -243,8 +234,7 @@ def test_composite_vs_fp64(P, n, beta):
         assert max(e.values()) < TOL, e
         if R >= 3:
             rays = np.arange(0, R, 2)
-            rc, part = call_composite(subset(persons, rays), rays.size, n, beta)
-            assert rc == 0
+            part = call_composite(subset(persons, rays), rays.size, n, beta)
             for k, a, b in zip(NAMES, part, got):
                 assert np.array_equal(a.view(np.uint32), b[rays].view(np.uint32)), k
 
@@ -262,8 +252,7 @@ def test_tie_order():
     rev = composite_ref(persons, R, n, np.float32(beta), reverse=True)
     gap = max(float(np.abs(a - b).max()) for a, b in zip(fwd, rev))
     assert gap > 1e-3
-    rc, got = call_composite(persons, R, n, beta)
-    assert rc == 0
+    got = call_composite(persons, R, n, beta)
     assert max(_errs(got, fwd).values()) < TOL
     assert max(_errs(got, rev).values()) > 1e-3 - TOL
     # in particular on bg_T, where the shared far with a negative sdf decides which sample is last
@@ -275,24 +264,21 @@ def test_rejected_calls_leave_outputs_untouched():
     """An over-cap P * n, a P outside [1, 8] and a short workspace each return a negative status with the expected
     mp_last_error() text, and no output is written (the checks run on the host before any kernel writes)."""
     from multiply_b200 import _lib as L
-    lib = L.lib()
 
-    def untouched(bufs):
-        return all(bool((b == SENTINEL).all()) for b in bufs.values())
+    def rejected(text, persons, R, n, **kw):
+        bufs = outputs(R, len(persons))
+        with pytest.raises(L.MpError, match=r"failed \(-\d+\): .*" + text):
+            call_composite(persons, R, n, 0.1, bufs=bufs, **kw)
+        assert all(bool((b == SENTINEL).all()) for b in bufs.values())
 
-    persons = make_inputs(3, 8, 5, N_MAX_P8 + 1, ties=False)
-    rc, bufs = call_composite(persons, 5, N_MAX_P8 + 1, 0.1)
-    assert rc < 0 and "too large for shared memory" in lib.mp_last_error().decode() and untouched(bufs)
+    rejected("too large for shared memory", make_inputs(3, 8, 5, N_MAX_P8 + 1, ties=False), 5, N_MAX_P8 + 1)
     persons = make_inputs(4, 2, 5, 8)
     for bad_P in (0, 9):
-        rc, bufs = call_composite(persons, 5, 8, 0.1, P_arg=bad_P)
-        assert rc < 0 and "bad person list" in lib.mp_last_error().decode() and untouched(bufs)
-    rc, bufs = call_composite(persons, 5, 8, 0.1, ws_delta=-1)
-    assert rc < 0 and "workspace too small" in lib.mp_last_error().decode() and untouched(bufs)
+        rejected("bad person list", persons, 5, 8, P_arg=bad_P)
+    rejected("workspace too small", persons, 5, 8, ws_delta=-1)
     # the largest n that fits still runs
     persons = make_inputs(5, 8, 2, N_MAX_P8, ties=False)
-    rc, _ = call_composite(persons, 2, N_MAX_P8, 0.1)
-    assert rc == 0
+    call_composite(persons, 2, N_MAX_P8, 0.1)
 
 
 @pytest.mark.parametrize("with_bg,with_fg_out", [(True, True), (False, True), (True, False), (False, False)])
@@ -307,14 +293,13 @@ def test_final_compose(with_bg, with_fg_out):
     bgT[::11] = 0.0
     bg = rng.random_sample((R, 3)).astype(np.float32)
     d_fg, d_T, d_bg = (torch.from_numpy(a).cuda() for a in (fg, bgT, bg))
-    rgb = _out(R, 3)
-    fgo = _out(R, 3) if with_fg_out else None
-    L.check(L.lib().mp_final_compose(d_fg.data_ptr(), d_T.data_ptr(), d_bg.data_ptr() if with_bg else None, R,
-                                     rgb.data_ptr(), L.ptr(fgo), L.stream_ptr()), "mp_final_compose")
+    rgb = padded((R, 3))
+    fgo = padded((R, 3)) if with_fg_out else None
+    L.call("mp_final_compose", d_fg, d_T, d_bg if with_bg else None, R, rgb, fgo)
     torch.cuda.synchronize()
     b = bg if with_bg else np.ones_like(bg)
     want = (fg + (bgT[:, None] * b).astype(np.float32)).astype(np.float32)
-    assert np.array_equal(_take(rgb, R, 3, "rgb").view(np.uint32), want.view(np.uint32))
+    assert np.array_equal(take(rgb, (R, 3), "rgb").numpy().view(np.uint32), want.view(np.uint32))
     if with_fg_out:
         want_fg = (fg + bgT[:, None]).astype(np.float32)
-        assert np.array_equal(_take(fgo, R, 3, "fg_rgb_values").view(np.uint32), want_fg.view(np.uint32))
+        assert np.array_equal(take(fgo, (R, 3), "fg_rgb_values").numpy().view(np.uint32), want_fg.view(np.uint32))

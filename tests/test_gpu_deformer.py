@@ -33,13 +33,12 @@ if ROOT not in sys.path:
 from multiply_b200 import scene as S          # noqa: E402
 from oracle import port                       # noqa: E402
 
+from _abi import padded, rows, take           # noqa: E402
+
 U = 2.0 ** -24
 POSED_CELL = np.float32(0.05005)   # mp_body_set_pose
 R0 = 2
 MAX_CELLS = 32768                  # kMaxCells (common.cuh)
-SENTINEL = -1234.5
-SENTINEL_U8 = 0xA5
-PAD_ROWS = 128
 SIZES = (0, 1, 127, 128, 129)
 # Gate on c of the kappa-scaled bound.  Measured on one H100 80GB HBM3 at a 400 W power limit: worst c = 3.6 on the
 # synthetic persons (kappa ~ 1.1) for x_c, x_d and Jinv; on the near-singular hand-built blends c grows with kappa
@@ -336,18 +335,6 @@ def c_of(err, kappa, scale):
 # calls through the C ABI into sentinel-padded buffers
 # ---------------------------------------------------------------------------------------------
 
-def _out(N, width, dtype=torch.float32):
-    fill = SENTINEL_U8 if dtype == torch.uint8 else SENTINEL
-    return torch.full(((N + PAD_ROWS) * width,), fill, dtype=dtype, device="cuda")
-
-
-def _take(buf, N, width, what):
-    fill = SENTINEL_U8 if buf.dtype == torch.uint8 else SENTINEL
-    tail = buf[N * width:]
-    assert bool((tail == fill).all()), "%s: %d values written past N = %d" % (what, int((tail != fill).sum()), N)
-    return buf[:N * width].reshape(N, width).cpu().numpy() if width > 1 else buf[:N].cpu().numpy()
-
-
 class DevBody:
     def __init__(self, body):
         from multiply_b200 import engine
@@ -360,21 +347,17 @@ class DevBody:
 
     def inverse(self, x, N, exact_far):
         from multiply_b200 import _lib as L
-        xd = torch.from_numpy(x[:N]).cuda() if N else torch.zeros(1, 3, device="cuda")
-        xc, out = _out(N, 3), _out(N, 1, torch.uint8)
-        L.check(L.lib().mp_deform_inverse(self.b.handle, xd.data_ptr(), N, xc.data_ptr(), out.data_ptr(),
-                                          int(exact_far), L.stream_ptr()), "mp_deform_inverse")
+        xc, out = padded((N, 3)), padded(N, torch.uint8)
+        L.call("mp_deform_inverse", self.b.handle, rows(torch.from_numpy(x), N), N, xc, out, int(exact_far))
         torch.cuda.synchronize()
-        return _take(xc, N, 3, "x_c"), _take(out, N, 1, "outlier").astype(bool)
+        return take(xc, (N, 3), "x_c").numpy(), take(out, N, "outlier").numpy().astype(bool)
 
     def forward_jac(self, x, N):
         from multiply_b200 import _lib as L
-        xd_in = torch.from_numpy(x[:N]).cuda() if N else torch.zeros(1, 3, device="cuda")
-        xd, J = _out(N, 3), _out(N, 9)
-        L.check(L.lib().mp_deform_forward_jac(self.b.handle, xd_in.data_ptr(), N, xd.data_ptr(), J.data_ptr(),
-                                              L.stream_ptr()), "mp_deform_forward_jac")
+        xd, J = padded((N, 3)), padded((N, 9))
+        L.call("mp_deform_forward_jac", self.b.handle, rows(torch.from_numpy(x), N), N, xd, J)
         torch.cuda.synchronize()
-        return _take(xd, N, 3, "x_d"), _take(J, N, 9, "Jinv")
+        return take(xd, (N, 3), "x_d").numpy(), take(J, (N, 9), "Jinv").numpy()
 
 
 _CASES = {}

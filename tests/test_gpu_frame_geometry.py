@@ -32,9 +32,9 @@ if ROOT not in sys.path:
 from multiply_b200 import scene as S          # noqa: E402  (CPU-only module)
 from oracle import render_grad as RG          # noqa: E402
 
+from _abi import SENTINEL_INT, padded, take     # noqa: E402
+
 EPS = 2.0 ** -24
-SENTINEL = -1234.5
-PAD = 128
 MEASURED = {}
 
 # gates in units of 2^-24 * M: 4x the worst measured on one H100 80GB HBM3 at a 400 W power limit (each test's docstring)
@@ -66,16 +66,6 @@ def _ratio(err, M):
     """err / (2^-24 M) elementwise, where M = 0 demands err = 0."""
     err, M = np.asarray(err, np.float64), np.asarray(M, np.float64)
     return np.where(M > 0, err / (EPS * np.where(M > 0, M, 1.0)), np.where(err == 0, 0.0, np.inf))
-
-
-def _padded(n, dtype=torch.float32, fill=SENTINEL):
-    return torch.full((n + PAD,), fill, dtype=dtype, device="cuda")
-
-
-def _take(buf, n, what, fill=SENTINEL):
-    tail = buf[n:]
-    assert bool((tail == fill).all()), "%s: %d values written past the end" % (what, int((tail != fill).sum()))
-    return buf[:n].cpu().numpy()
 
 
 # ---------------------------------------------------------------------------------------------
@@ -208,41 +198,30 @@ class SmplHandle:
 
     def __init__(self, model, betas_c=None):
         from multiply_b200 import _lib as L
-        self.L, self.lib = L, L.lib()
+        self.L = L
         self.V = model["v_template"].shape[0]
         self.d = {k: torch.from_numpy(np.ascontiguousarray(model[k], np.float32)).cuda()
                   for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "lbs_weights")}
         self.bc = None if betas_c is None else torch.from_numpy(np.asarray(betas_c, np.float32)).cuda()
         pa = (C.c_int * 24)(*[max(int(p), 0) for p in model["parents"]])
-        nbytes = self.lib.mp_smpl_bytes(self.V)
-        self.storage = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
-        h = C.c_void_p()
+        self.storage = L.workspace(L.call("mp_smpl_bytes", self.V), "cuda")
+        self.h = L.Handle("mp_smpl_free")
         d = self.d
-        L.check(self.lib.mp_smpl_create(d["v_template"].data_ptr(), d["shapedirs"].data_ptr(), d["posedirs"].data_ptr(),
-                                        d["J_regressor"].data_ptr(), pa, d["lbs_weights"].data_ptr(), self.V,
-                                        L.ptr(self.bc), self.storage.data_ptr(), nbytes, C.byref(h), L.stream_ptr()),
-                "mp_smpl_create")
-        self.h = h
+        L.call("mp_smpl_create", d["v_template"], d["shapedirs"], d["posedirs"], d["J_regressor"], pa, d["lbs_weights"],
+               self.V, self.bc, self.storage, self.storage.numel(), C.byref(self.h))
 
     def canonical(self):
-        vc, ti = _padded(self.V * 3), _padded(24 * 16)
-        self.L.check(self.lib.mp_smpl_canonical(self.h, vc.data_ptr(), ti.data_ptr(), self.L.stream_ptr()),
-                     "mp_smpl_canonical")
+        vc, ti = padded((self.V, 3)), padded((24, 4, 4))
+        self.L.call("mp_smpl_canonical", self.h, vc, ti)
         torch.cuda.synchronize()
-        return _take(vc, self.V * 3, "verts_c").reshape(self.V, 3), _take(ti, 24 * 16, "tfs_c_inv").reshape(24, 4, 4)
+        return take(vc, (self.V, 3), "verts_c").numpy(), take(ti, (24, 4, 4), "tfs_c_inv").numpy()
 
     def forward(self, scale, transl, theta, betas, absolute):
         args = [torch.from_numpy(np.asarray(a, np.float32).reshape(-1)).cuda() for a in ((scale,), transl, theta, betas)]
-        v, t = _padded(self.V * 3), _padded(24 * 16)
-        self.L.check(self.lib.mp_smpl_forward(self.h, *[a.data_ptr() for a in args], int(absolute), v.data_ptr(),
-                                              t.data_ptr(), self.L.stream_ptr()), "mp_smpl_forward")
+        v, t = padded((self.V, 3)), padded((24, 4, 4))
+        self.L.call("mp_smpl_forward", self.h, *args, int(absolute), v, t)
         torch.cuda.synchronize()
-        return _take(v, self.V * 3, "smpl_verts").reshape(self.V, 3), _take(t, 24 * 16, "smpl_tfs").reshape(24, 4, 4)
-
-    def free(self):
-        if self.h:
-            self.lib.mp_smpl_free(self.h)
-            self.h = None
+        return take(v, (self.V, 3), "smpl_verts").numpy(), take(t, (24, 4, 4), "smpl_tfs").numpy()
 
 
 _U = np.array([0.36, -0.48, 0.8])          # a unit axis with no zero component
@@ -307,20 +286,17 @@ def test_smpl_server_vs_fp64(name):
     bc_given = _betas(1.5, 11)
     for bc in (None, bc_given):
         hd = SmplHandle(model, bc)
-        try:
-            o, cano = canonical_ref(model, np.zeros(10, np.float32) if bc is None else bc)
-            vc, ti = hd.canonical()
-            c = max(_ratio(np.abs(vc - o["verts"]), o["M_verts"]).max(), _ratio(np.abs(ti - cano[0]), cano[1]).max())
-            _note("smpl_canonical/" + name, c)
-            assert c < C_SMPL, (name, bc is not None, c)
-            for pn, theta in poses.items():
-                for k, pl in enumerate(PLACEMENTS):
-                    c, parts = _smpl_case(hd, model, cano, theta, pl)
-                    _note("smpl/%s/%s" % (name, pn), c)
-                    _note("smpl/" + name, c)
-                    assert c < C_SMPL, (name, pn, k, bc is not None, parts)
-        finally:
-            hd.free()
+        o, cano = canonical_ref(model, np.zeros(10, np.float32) if bc is None else bc)
+        vc, ti = hd.canonical()
+        c = max(_ratio(np.abs(vc - o["verts"]), o["M_verts"]).max(), _ratio(np.abs(ti - cano[0]), cano[1]).max())
+        _note("smpl_canonical/" + name, c)
+        assert c < C_SMPL, (name, bc is not None, c)
+        for pn, theta in poses.items():
+            for k, pl in enumerate(PLACEMENTS):
+                c, parts = _smpl_case(hd, model, cano, theta, pl)
+                _note("smpl/%s/%s" % (name, pn), c)
+                _note("smpl/" + name, c)
+                assert c < C_SMPL, (name, pn, k, bc is not None, parts)
 
 
 def test_smpl_handle_state_does_not_leak():
@@ -329,17 +305,14 @@ def test_smpl_handle_state_does_not_leak():
     model = get_model("smpl6890")
     poses = smpl_poses()
     hd = SmplHandle(model)
-    try:
-        a = (0.5, (0.3, 0.1, -0.2), poses["random_a"], _betas(3.0, 7), 0)
-        b = (2.0, (-1.0, 0.4, 0.9), poses["large"], _betas(-5.0, 8), 1)
-        v1, t1 = hd.forward(*a)
-        v2, t2 = hd.forward(*b)
-        v3, t3 = hd.forward(*a)
-        assert not np.array_equal(v1, v2)
-        assert np.array_equal(v1.view(np.uint32), v3.view(np.uint32))
-        assert np.array_equal(t1.view(np.uint32), t3.view(np.uint32))
-    finally:
-        hd.free()
+    a = (0.5, (0.3, 0.1, -0.2), poses["random_a"], _betas(3.0, 7), 0)
+    b = (2.0, (-1.0, 0.4, 0.9), poses["large"], _betas(-5.0, 8), 1)
+    v1, t1 = hd.forward(*a)
+    v2, t2 = hd.forward(*b)
+    v3, t3 = hd.forward(*a)
+    assert not np.array_equal(v1, v2)
+    assert np.array_equal(v1.view(np.uint32), v3.view(np.uint32))
+    assert np.array_equal(t1.view(np.uint32), t3.view(np.uint32))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -395,23 +368,21 @@ def call_camera_rays(uv, pose, K):
     from multiply_b200 import _lib as L
     R = uv.shape[0]
     t = [torch.from_numpy(np.ascontiguousarray(a, np.float32).reshape(-1)).cuda() for a in (uv, pose, K)]
-    dirs, cam = _padded(R * 3), _padded(R * 3)
-    L.check(L.lib().mp_camera_rays(t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), R, dirs.data_ptr(),
-                                   cam.data_ptr(), L.stream_ptr()), "mp_camera_rays")
+    dirs, cam = padded((R, 3)), padded((R, 3))
+    L.call("mp_camera_rays", *t, R, dirs, cam)
     torch.cuda.synchronize()
-    return _take(dirs, R * 3, "ray_dirs").reshape(R, 3), _take(cam, R * 3, "cam_loc").reshape(R, 3)
+    return take(dirs, (R, 3), "ray_dirs").numpy(), take(cam, (R, 3), "cam_loc").numpy()
 
 
 def call_sphere(cam, dirs, r, flag0=0):
     from multiply_b200 import _lib as L
     R = cam.shape[0]
     c, d = (torch.from_numpy(np.ascontiguousarray(a, np.float32).reshape(-1)).cuda() for a in (cam, dirs))
-    nf = _padded(R * 2)
+    nf = padded((R, 2))
     flag = torch.full((1,), flag0, dtype=torch.int32, device="cuda")
-    L.check(L.lib().mp_sphere_intersections(c.data_ptr(), d.data_ptr(), R, float(r), nf.data_ptr(), flag.data_ptr(),
-                                            L.stream_ptr()), "mp_sphere_intersections")
+    L.call("mp_sphere_intersections", c, d, R, float(r), nf, flag)
     torch.cuda.synchronize()
-    return _take(nf, R * 2, "near_far").reshape(R, 2), int(flag.item())
+    return take(nf, (R, 2), "near_far").numpy(), int(flag.item())
 
 
 def _ordered(a):
@@ -532,14 +503,13 @@ def call_box_hits(cam, dirs, c, h, rot=None):
     R = cam.shape[0]
     cc, dd = (torch.from_numpy(np.ascontiguousarray(a, np.float32).reshape(-1)).cuda() for a in (cam, dirs))
     rot_d = None if rot is None else torch.from_numpy(np.asarray(rot, np.float64).reshape(9)).cuda()
-    idx = _padded(R, torch.int64, -7)
+    idx = padded(R, torch.int64)
     cnt = torch.full((1,), -1, dtype=torch.int32, device="cuda")
-    L.check(L.lib().mp_ray_box_hits(cc.data_ptr(), dd.data_ptr(), R, (C.c_double * 3)(*c), (C.c_double * 3)(*h),
-                                    L.ptr(rot_d), idx.data_ptr(), cnt.data_ptr(), L.stream_ptr()), "mp_ray_box_hits")
+    L.call("mp_ray_box_hits", cc, dd, R, L.vec3(C.c_double, c), L.vec3(C.c_double, h), rot_d, idx, cnt)
     torch.cuda.synchronize()
     n = int(cnt.item())
     assert 0 <= n <= R
-    return _take(idx, n, "hit ids", -7), idx, cnt
+    return take(idx, n, "hit ids").numpy(), idx, cnt
 
 
 BOX_C, BOX_H = (0.25, -0.5, 0.75), (0.5, 0.25, 0.375)     # exactly representable: faces at c +- h are float32
@@ -590,11 +560,11 @@ def test_ray_box_hits_patterns(R):
             assert np.array_equal(want, np.flatnonzero(mask)), (rname, pname)
             got, idx, cnt = call_box_hits(cam, dirs, BOX_C, BOX_H, rm)
             assert np.array_equal(got, want), (rname, pname, got[:8], want[:8])
-            L.check(L.lib().mp_hit_list_finalize(idx.data_ptr(), cnt.data_ptr(), L.stream_ptr()), "mp_hit_list_finalize")
+            L.call("mp_hit_list_finalize", idx, cnt)
             torch.cuda.synchronize()
             n = int(cnt.item())
             if want.size == 0:
-                assert n == 1 and int(idx[0].item()) == 0 and bool((idx[1:] == -7).all())
+                assert n == 1 and int(idx[0].item()) == 0 and bool((idx[1:] == SENTINEL_INT).all())
             else:
                 assert n == want.size and np.array_equal(idx[:n].cpu().numpy(), want)
 
@@ -653,22 +623,21 @@ def test_ray_aabb_hits(V):
         uv = rng.uniform(0, 64, (R, 2)).astype(np.float32)
         dirs, cam = call_camera_rays(uv, pose[0].numpy(), K[0].numpy())
         vd, cd, dd = (torch.from_numpy(np.ascontiguousarray(a).reshape(-1)).cuda() for a in (verts, cam, dirs))
-        idx = _padded(R, torch.int64, -7)
+        idx = padded(R, torch.int64)
         cnt = torch.full((1,), -1, dtype=torch.int32, device="cuda")
-        box = torch.full((6 + 16,), SENTINEL, dtype=torch.float64, device="cuda")
-        L.check(L.lib().mp_ray_aabb_hits(cd.data_ptr(), dd.data_ptr(), R, vd.data_ptr(), V, 1.2, idx.data_ptr(),
-                                         cnt.data_ptr(), box.data_ptr(), L.stream_ptr()), "mp_ray_aabb_hits")
+        box = padded(6, torch.float64)
+        L.call("mp_ray_aabb_hits", cd, dd, R, vd, V, 1.2, idx, cnt, box)
         torch.cuda.synchronize()
         lo, hi = verts.min(0).astype(np.float64), verts.max(0).astype(np.float64)
         ctr, half = (lo + hi) / 2.0, (hi - lo) / 2.0 * 1.2
-        b = box.cpu().numpy()
-        assert np.array_equal(b[:3], ctr) and np.array_equal(b[3:6], half) and (b[6:] == SENTINEL).all()
+        b = take(box, 6, "box_ws").numpy()
+        assert np.array_equal(b[:3], ctr) and np.array_equal(b[3:6], half)
         want = slab_hits_ref(cam, dirs, ctr, half)
         if want.size == 0:
             want = np.zeros(1, np.int64)
         n = int(cnt.item())
         assert n == want.size
-        assert np.array_equal(_take(idx, n, "aabb ids", -7), want)
+        assert np.array_equal(take(idx, n, "aabb ids").numpy(), want)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -763,15 +732,13 @@ def call_background(eng, cam, dirs, r=3.0):
     if key not in _SCENE:
         _SCENE[key] = engine.Field(sc["bg_implicit"], sc["bg_render"], background=True)
         _SCENE[key].set_cond(sc["frame_code"])
-    lib = L.lib()
     R = cam.shape[0]
     c, d = (torch.from_numpy(np.ascontiguousarray(a, np.float32).reshape(-1)).cuda() for a in (cam, dirs))
-    out = _padded(R * 3)
-    ws = torch.empty(lib.mp_background_workspace_bytes(R), dtype=torch.uint8, device="cuda")
-    L.check(lib.mp_background(_SCENE[key].handle, d.data_ptr(), c.data_ptr(), R, float(r), out.data_ptr(),
-                              ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_background")
+    out = padded((R, 3))
+    ws = L.workspace(L.call("mp_background_workspace_bytes", R), "cuda")
+    L.call("mp_background", _SCENE[key].handle, d, c, R, float(r), out, ws, ws.numel())
     torch.cuda.synchronize()
-    return _take(out, R * 3, "bg_rgb").reshape(R, 3)
+    return take(out, (R, 3), "bg_rgb").numpy()
 
 
 @pytest.mark.parametrize("eng", ["simt", "tc"])

@@ -33,13 +33,11 @@ import torch
 from multiply_b200 import scene as S
 from oracle import mesh_port as port
 
+from _abi import padded, take
+
 gpu = pytest.mark.gpu
 
 THRESHOLDS = (0.05, 0.0625, 0.0, -1e-3, -0.05)
-SENTINEL_F = -1234.5
-SENTINEL_I = -7
-SENTINEL_U8 = 0xA5
-PAD = 128
 
 
 # ---------------------------------------------------------------------------------------------
@@ -715,41 +713,33 @@ def _body():
 @gpu
 def test_abi_null_outputs_zero_n_and_padding():
     L = _L()
-    lib = L.lib()
     v, f = _body()
     m = _mesh(v, f)
     pts = _around(v, 300, 31).cuda()
     d2, fi, dt = m.distance(pts)
     ins = m.check_sign(pts)
     for N in (0, 1, 127, 128, 129):
-        o = torch.full((N + PAD,), SENTINEL_F, device="cuda")
-        oi = torch.full((N + PAD,), SENTINEL_I, dtype=torch.int64, device="cuda")
-        ot = torch.full((N + PAD,), SENTINEL_I, dtype=torch.int32, device="cuda")
-        ou = torch.full((N + PAD,), SENTINEL_U8, dtype=torch.uint8, device="cuda")
-        L.check(lib.mp_mesh_distance(m.handle, pts.data_ptr(), N, o.data_ptr(), oi.data_ptr(), ot.data_ptr(),
-                                     L.stream_ptr()), "mp_mesh_distance")
-        L.check(lib.mp_mesh_check_sign(m.handle, pts.data_ptr(), N, ou.data_ptr(), L.stream_ptr()), "check_sign")
+        o, oi, ot, ou = padded(N), padded(N, torch.int64), padded(N, torch.int32), padded(N, torch.uint8)
+        L.call("mp_mesh_distance", m.handle, pts, N, o, oi, ot)
+        L.call("mp_mesh_check_sign", m.handle, pts, N, ou)
         torch.cuda.synchronize()
-        assert torch.equal(o[:N], d2[:N]) and torch.equal(oi[:N], fi[:N]) and torch.equal(ot[:N], dt[:N])
-        assert torch.equal(ou[:N].bool(), ins[:N])
-        assert bool((o[N:] == SENTINEL_F).all()) and bool((oi[N:] == SENTINEL_I).all())
-        assert bool((ot[N:] == SENTINEL_I).all()) and bool((ou[N:] == SENTINEL_U8).all())
+        assert torch.equal(take(o, N, "sq_dist"), d2[:N].cpu()) and torch.equal(take(oi, N, "face_idx"), fi[:N].cpu())
+        assert torch.equal(take(ot, N, "dist_type"), dt[:N].cpu())
+        assert torch.equal(take(ou, N, "inside").bool(), ins[:N].cpu())
         # NULL face_idx / dist_type
-        o2 = torch.full((N + PAD,), SENTINEL_F, device="cuda")
-        L.check(lib.mp_mesh_distance(m.handle, pts.data_ptr(), N, o2.data_ptr(), None, None, L.stream_ptr()), "dist")
+        o2 = padded(N)
+        L.call("mp_mesh_distance", m.handle, pts, N, o2, None, None)
         torch.cuda.synchronize()
         assert torch.equal(o2, o)
         # flags: rows = N of 2 samples
         x = pts[:2].repeat(N + 1, 1)[: 2 * N].contiguous() if N else pts
-        fo = torch.full((N + PAD,), SENTINEL_U8, dtype=torch.uint8, device="cuda")
-        fn = torch.full((N + PAD,), SENTINEL_U8, dtype=torch.uint8, device="cuda")
-        L.check(lib.mp_mesh_surface_flags(m.handle, x.data_ptr(), N, 2, 0.05, fo.data_ptr(), fn.data_ptr(),
-                                          L.stream_ptr()), "flags")
+        fo, fn = padded(N, torch.uint8), padded(N, torch.uint8)
+        L.call("mp_mesh_surface_flags", m.handle, x, N, 2, 0.05, fo, fn)
         torch.cuda.synchronize()
-        assert bool((fo[N:] == SENTINEL_U8).all()) and bool((fn[N:] == SENTINEL_U8).all())
+        fo, fn = take(fo, N, "off_surface"), take(fn, N, "in_surface")
         if N:
             ro, ri = m.surface_flags(x, 2, 0.05)
-            assert torch.equal(fo[:N].bool(), ro) and torch.equal(fn[:N].bool(), ri)
+            assert torch.equal(fo.bool(), ro.cpu()) and torch.equal(fn.bool(), ri.cpu())
 
 
 @gpu
@@ -781,43 +771,31 @@ def test_abi_reruns_two_handles_and_rebuild():
 @gpu
 def test_abi_errors_leave_nothing_behind():
     L = _L()
-    lib = L.lib()
     v, f = voxel_mesh(_shape("box"), VOX_ORIGIN, VOX_STEP)
     V = v.shape[0]
-    vd = v.cuda()
-    scratch = torch.empty(L.MP_MESH_PLAN_SCRATCH_BYTES, dtype=torch.uint8, device="cuda")
+    vd, fd = v.cuda(), f.cuda()
+    scratch = L.workspace(L.MP_MESH_PLAN_SCRATCH_BYTES, "cuda")
 
-    def plan_of(verts, faces, Vn, Fn, margin):
+    def rejected(msg, faces, Vn, Fn, margin):
         p = L.MeshPlan()
         p.V, p.F, p.n_refs, p.storage_bytes = -5, -5, -5, 12345
-        rc = lib.mp_mesh_plan(verts.data_ptr(), Vn, faces.data_ptr(), Fn, margin, scratch.data_ptr(), C.byref(p),
-                              L.stream_ptr())
-        return rc, p
-
-    for bad, msg in ((-1, "outside"), (V, "outside")):
-        fb = f.clone()
-        fb[len(fb) // 2, 1] = bad
-        rc, p = plan_of(vd, fb.cuda(), V, f.shape[0], 0.01)
-        assert rc != 0 and msg in lib.mp_last_error().decode()
+        with pytest.raises(L.MpError, match=r"failed \(-\d+\): .*" + msg):
+            L.call("mp_mesh_plan", vd, Vn, faces, Fn, margin, scratch, p)
         assert (p.V, p.F, p.n_refs, p.storage_bytes) == (-5, -5, -5, 12345), "no plan is written"
-    fd = f.cuda()
-    for Vn, Fn, margin, msg in ((2, f.shape[0], 0.01, "V >= 3"), (V, 0, 0.01, "F >= 1"), (V, f.shape[0], -0.01, "margin")):
-        rc, p = plan_of(vd, fd, Vn, Fn, margin)
-        assert rc != 0 and msg in lib.mp_last_error().decode()
-        assert (p.V, p.F, p.n_refs, p.storage_bytes) == (-5, -5, -5, 12345)
-    with pytest.raises(L.MpError, match="outside"):
+
+    for (row, col), bad in (((len(f) // 2, 1), -1), ((len(f) // 2, 1), V), ((0, 0), V)):
         fb = f.clone()
-        fb[0, 0] = V
-        L.check(plan_of(vd, fb.cuda(), V, f.shape[0], 0.01)[0], "mp_mesh_plan")
+        fb[row, col] = bad
+        rejected("outside", fb.cuda(), V, f.shape[0], 0.01)
+    for Vn, Fn, margin, msg in ((2, f.shape[0], 0.01, "V >= 3"), (V, 0, 0.01, "F >= 1"), (V, f.shape[0], -0.01, "margin")):
+        rejected(msg, fd, Vn, Fn, margin)
     # storage one byte short: an error and no handle
-    rc, p = plan_of(vd, fd, V, f.shape[0], 0.01)
-    assert rc == 0
-    storage = torch.empty(p.storage_bytes, dtype=torch.uint8, device="cuda")
-    h = C.c_void_p()
-    rc = lib.mp_mesh_create(C.byref(p), vd.data_ptr(), fd.data_ptr(), storage.data_ptr(), p.storage_bytes - 1,
-                            C.byref(h), L.stream_ptr())
-    assert rc != 0 and "storage" in lib.mp_last_error().decode() and h.value is None
-    rc = lib.mp_mesh_create(C.byref(p), vd.data_ptr(), fd.data_ptr(), storage.data_ptr(), p.storage_bytes,
-                            C.byref(h), L.stream_ptr())
-    assert rc == 0 and h.value is not None
-    lib.mp_mesh_free(h)
+    p = L.MeshPlan()
+    L.call("mp_mesh_plan", vd, V, fd, f.shape[0], 0.01, scratch, p)
+    storage = L.workspace(p.storage_bytes, "cuda")
+    h = L.Handle("mp_mesh_free")
+    with pytest.raises(L.MpError, match=r"failed \(-\d+\): .*storage"):
+        L.call("mp_mesh_create", p, vd, fd, storage, p.storage_bytes - 1, C.byref(h))
+    assert h.value is None
+    L.call("mp_mesh_create", p, vd, fd, storage, p.storage_bytes, C.byref(h))
+    assert h.value is not None

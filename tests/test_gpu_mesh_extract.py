@@ -207,37 +207,33 @@ def test_generate_mesh_end_to_end_and_rerun(model):
 
 
 def test_rejected_inputs(model):
-    lib = L.lib()
     sc, m = model
     f = m._ensure_renderer(torch.device("cuda", torch.cuda.current_device())).fields[0]
-    c = (C.c_float * 3)(0.0, 0.0, 0.0)
+    c = L.vec3(C.c_float, (0.0, 0.0, 0.0))
     n = C.c_longlong(0)
     g = torch.zeros(9 ** 3, device="cuda")
-    ws = torch.empty(lib.mp_mise_workspace_bytes(4, 1), dtype=torch.uint8, device="cuda")
-    st = L.stream_ptr()
-    assert lib.mp_mise(f.handle, c, 1.0, 1.1, 4, 9, 0.0, g.data_ptr(), None, C.byref(n), ws.data_ptr(), ws.numel(), st) != 0
-    assert "res_init" in lib.mp_last_error().decode()
-    assert lib.mp_mise(f.handle, c, 1.0, 1.1, 4, 1, float("nan"), g.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
-                       st) != 0
-    assert lib.mp_mise(f.handle, c, 1.0, 1.1, 4, 1, 0.0, None, None, None, ws.data_ptr(), ws.numel(), st) != 0
-    assert lib.mp_mise(f.handle, c, 1.0, 1.1, 4, 1, 0.0, g.data_ptr(), None, None, ws.data_ptr(), 16, st) != 0
-    assert "workspace" in lib.mp_last_error().decode()
+
+    def rejected(text, name, *args):
+        with pytest.raises(L.MpError, match=r"failed \(-\d+\): .*" + text):
+            L.call(name, *args)
+
+    ws = L.workspace(L.call("mp_mise_workspace_bytes", 4, 1), "cuda")
+    rejected("res_init", "mp_mise", f.handle, c, 1.0, 1.1, 4, 9, 0.0, g, None, C.byref(n), ws, ws.numel())
+    rejected("", "mp_mise", f.handle, c, 1.0, 1.1, 4, 1, float("nan"), g, None, None, ws, ws.numel())
+    rejected("", "mp_mise", f.handle, c, 1.0, 1.1, 4, 1, 0.0, None, None, None, ws, ws.numel())
+    rejected("workspace", "mp_mise", f.handle, c, 1.0, 1.1, 4, 1, 0.0, g, None, None, ws, 16)
     V, F = C.c_longlong(0), C.c_longlong(0)
-    mws = torch.empty(lib.mp_marching_cubes_workspace_bytes(8), dtype=torch.uint8, device="cuda")
-    assert lib.mp_marching_cubes_count(g.data_ptr(), 0, 0.0, C.byref(V), C.byref(F), mws.data_ptr(), mws.numel(), st) != 0
-    assert lib.mp_marching_cubes_count(g.data_ptr(), 1025, 0.0, C.byref(V), C.byref(F), mws.data_ptr(), mws.numel(),
-                                       st) != 0
-    assert lib.mp_marching_cubes_count(g.data_ptr(), 8, float("nan"), C.byref(V), C.byref(F), mws.data_ptr(),
-                                       mws.numel(), st) != 0
-    assert lib.mp_marching_cubes_count(None, 8, 0.0, C.byref(V), C.byref(F), mws.data_ptr(), mws.numel(), st) != 0
-    assert lib.mp_marching_cubes_count(g.data_ptr(), 8, 0.0, C.byref(V), C.byref(F), mws.data_ptr(), 64, st) != 0
+    mws = L.workspace(L.call("mp_marching_cubes_workspace_bytes", 8), "cuda")
+    rejected("", "mp_marching_cubes_count", g, 0, 0.0, C.byref(V), C.byref(F), mws, mws.numel())
+    rejected("", "mp_marching_cubes_count", g, 1025, 0.0, C.byref(V), C.byref(F), mws, mws.numel())
+    rejected("", "mp_marching_cubes_count", g, 8, float("nan"), C.byref(V), C.byref(F), mws, mws.numel())
+    rejected("", "mp_marching_cubes_count", None, 8, 0.0, C.byref(V), C.byref(F), mws, mws.numel())
+    rejected("", "mp_marching_cubes_count", g, 8, 0.0, C.byref(V), C.byref(F), mws, 64)
     verts = torch.zeros(3, 3, device="cuda")
     faces = torch.tensor([[0, 1, 5]], dtype=torch.int64, device="cuda")
-    cws = torch.empty(lib.mp_largest_component_workspace_bytes(3, 1), dtype=torch.uint8, device="cuda")
+    cws = L.workspace(L.call("mp_largest_component_workspace_bytes", 3, 1), "cuda")
     Vo, Fo = C.c_int(0), C.c_int(0)
-    assert lib.mp_largest_component(verts.data_ptr(), 3, faces.data_ptr(), 1, verts.data_ptr(), faces.data_ptr(),
-                                    C.byref(Vo), C.byref(Fo), cws.data_ptr(), cws.numel(), st) != 0
-    assert "outside" in lib.mp_last_error().decode()
-    assert lib.mp_largest_component(verts.data_ptr(), 3, faces.data_ptr(), 1, verts.data_ptr(), faces.data_ptr(),
-                                    C.byref(Vo), C.byref(Fo), cws.data_ptr(), 8, st) != 0
+    rejected("outside", "mp_largest_component", verts, 3, faces, 1, verts, faces, C.byref(Vo), C.byref(Fo), cws,
+             cws.numel())
+    rejected("", "mp_largest_component", verts, 3, faces, 1, verts, faces, C.byref(Vo), C.byref(Fo), cws, 8)
     torch.cuda.synchronize()

@@ -166,7 +166,6 @@ def test_sampler_training_mode(golden_dir):
     (mp_sample_rays_train), (b) through the mirror with the same torch.manual_seed, which replays the reference's
     random stream."""
     import os
-    import ctypes as C
     from multiply_b200 import engine, _lib as L
     from multiply_b200.model.ray_sampler import ErrorBoundSampler
     from multiply_b200.model import rend_util
@@ -211,7 +210,7 @@ def test_sampler_training_mode(golden_dir):
         z = torch.empty(R, cfg["N_samples"] + cfg["N_samples_extra"] + 2, device="cuda")
         z_bg = torch.empty(R, 32, device="cuda")
         trips = torch.zeros(1, dtype=torch.int32, device="cuda")
-        smp._ws = torch.empty(lib.mp_sampler_workspace_bytes(C.byref(c), R), dtype=torch.uint8, device="cuda")
+        smp._ws = L.workspace(L.call("mp_sampler_workspace_bytes", c, R), "cuda")
         (z, z_bg), z_eik = smp._get_z_vals_training(lib, c, body, field, d.contiguous(), o.contiguous(), R, z, z_bg, trips,
                                                     d.device, rng=rng)
         torch.cuda.synchronize()

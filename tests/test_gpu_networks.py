@@ -30,13 +30,13 @@ if ROOT not in sys.path:
 from multiply_b200 import scene as S          # noqa: E402
 from oracle import port                       # noqa: E402
 
+from _abi import padded, rows, take           # noqa: E402
+
 ENGINES = ["simt", "tc"]
 WEIGHTS = ["geometric", "trained"]
 # the network tolerances of tests/test_gpu_parity.py (gradients get twice that), here measured against fp64
 TOL_NET = {"simt": 1e-5, "tc": 2e-5}
 TOL_GATE = 1e-4               # BASELINE.json north_star: RGB / SDF / normals
-SENTINEL = -1234.5
-PAD_ROWS = 128                # a write past N inside the last tile lands in this tail
 SHIFTS = (1, 8, 16, 64, 127)  # moves rows across warp (8 rows per quad group), warpgroup (64) and tile (128) boundaries
 
 
@@ -46,7 +46,7 @@ SHIFTS = (1, 8, 16, 64, 127)  # moves rows across warp (8 rows per quad group), 
 
 def _tile_points():
     from multiply_b200 import _lib as L
-    return 128 * int(L.lib().mp_device_sm_count())
+    return 128 * int(L.call("mp_device_sm_count"))
 
 
 def _sizes(T):
@@ -145,79 +145,50 @@ def cases(T):
 # the C ABI with sentinel-padded outputs
 # ---------------------------------------------------------------------------------------------
 
-def _in(t, N):
-    """Rows [0, N) as a fresh device buffer (at least one row, so that N = 0 still passes a valid pointer)."""
-    rows = max(N, 1)
-    buf = torch.zeros(rows, *t.shape[1:], device="cuda")
-    buf[:N] = t[:N].cuda()
-    return buf.contiguous()
-
-
-def _out(N, width):
-    return torch.full(((N + PAD_ROWS) * width,), SENTINEL, device="cuda")
-
-
-def _take(buf, N, width, what):
-    """Checks the tail past N is untouched and returns rows [0, N) on the host."""
-    tail = buf[N * width:]
-    assert bool((tail == SENTINEL).all()), "%s: %d values written past N = %d" % (
-        what, int((tail != SENTINEL).sum()), N)
-    return buf[:N * width].reshape(N, width).cpu() if width > 1 else buf[:N].cpu()
-
-
 def _ws(N):
     from multiply_b200 import _lib as L
-    return torch.empty(L.lib().mp_mlp_workspace_bytes(N), dtype=torch.uint8, device="cuda")
+    return L.workspace(L.call("mp_mlp_workspace_bytes", N), "cuda")
 
 
 def call_implicit(field, x, N, want_feat=True, want_grad=False):
     from multiply_b200 import _lib as L
-    lib = L.lib()
-    xd = _in(x, N)
-    sdf = _out(N, 1)
-    feat = _out(N, 256) if want_feat else None
+    xd = rows(x, N)
+    sdf = padded(N)
+    feat = padded((N, 256)) if want_feat else None
     ws = _ws(N)
     if want_grad:
-        grad = _out(N, 3)
-        rc = lib.mp_implicit_forward_grad(field.handle, xd.data_ptr(), N, sdf.data_ptr(), L.ptr(feat), grad.data_ptr(),
-                                          ws.data_ptr(), ws.numel(), L.stream_ptr())
+        grad = padded((N, 3))
+        L.call("mp_implicit_forward_grad", field.handle, xd, N, sdf, feat, grad, ws, ws.numel())
     else:
-        grad = None
-        rc = lib.mp_implicit_forward(field.handle, xd.data_ptr(), N, sdf.data_ptr(), L.ptr(feat), ws.data_ptr(),
-                                     ws.numel(), L.stream_ptr())
-    L.check(rc, "mp_implicit_forward%s" % ("_grad" if want_grad else ""))
+        L.call("mp_implicit_forward", field.handle, xd, N, sdf, feat, ws, ws.numel())
     torch.cuda.synchronize()
-    o = {"sdf": _take(sdf, N, 1, "sdf")}
+    o = {"sdf": take(sdf, N, "sdf")}
     if want_feat:
-        o["feat"] = _take(feat, N, 256, "feat")
+        o["feat"] = take(feat, (N, 256), "feat")
     if want_grad:
-        o["grad"] = _take(grad, N, 3, "grad")
+        o["grad"] = take(grad, (N, 3), "grad")
     return o
 
 
 def call_render(field, x, nrm, feat, N):
     from multiply_b200 import _lib as L
-    rgb = _out(N, 3)
-    xd, nd, fd = _in(x, N), _in(nrm, N), _in(feat, N)
+    rgb = padded((N, 3))
     ws = _ws(N)
-    L.check(L.lib().mp_render_forward(field.handle, xd.data_ptr(), nd.data_ptr(), fd.data_ptr(), N, rgb.data_ptr(),
-                                      ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_render_forward")
+    L.call("mp_render_forward", field.handle, rows(x, N), rows(nrm, N), rows(feat, N), N, rgb, ws, ws.numel())
     torch.cuda.synchronize()
-    return {"rgb": _take(rgb, N, 3, "rgb")}
+    return {"rgb": take(rgb, (N, 3), "rgb")}
 
 
 def call_bg(field, pts, view, N, want_sdf=True):
     from multiply_b200 import _lib as L
-    sdf = _out(N, 1) if want_sdf else None
-    rgb = _out(N, 3)
-    pd, vd = _in(pts, N), _in(view, N)
+    sdf = padded(N) if want_sdf else None
+    rgb = padded((N, 3))
     ws = _ws(N)
-    L.check(L.lib().mp_bg_nets_forward(field.handle, pd.data_ptr(), vd.data_ptr(), N, L.ptr(sdf), rgb.data_ptr(),
-                                       ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_bg_nets_forward")
+    L.call("mp_bg_nets_forward", field.handle, rows(pts, N), rows(view, N), N, sdf, rgb, ws, ws.numel())
     torch.cuda.synchronize()
-    o = {"rgb": _take(rgb, N, 3, "bg rgb")}
+    o = {"rgb": take(rgb, (N, 3), "bg rgb")}
     if want_sdf:
-        o["sdf"] = _take(sdf, N, 1, "bg sdf")
+        o["sdf"] = take(sdf, N, "bg sdf")
     return o
 
 
@@ -238,16 +209,13 @@ def _lattice(person, res, scale=1.1):
 
 def call_sdf_grid(field, person, res):
     from multiply_b200 import _lib as L
-    lib = L.lib()
     center, extent, _ = _lattice(person, res)
     n = (res + 1) ** 3
-    vals = _out(n, 1)
-    ws = torch.empty(lib.mp_sdf_grid_workspace_bytes(res), dtype=torch.uint8, device="cuda")
-    c = (C.c_float * 3)(*[float(v) for v in center])
-    L.check(lib.mp_sdf_grid(field.handle, c, float(extent), 1.1, int(res), vals.data_ptr(), ws.data_ptr(), ws.numel(),
-                            L.stream_ptr()), "mp_sdf_grid")
+    vals = padded(n)
+    ws = L.workspace(L.call("mp_sdf_grid_workspace_bytes", res), "cuda")
+    L.call("mp_sdf_grid", field.handle, L.vec3(C.c_float, center), float(extent), 1.1, int(res), vals, ws, ws.numel())
     torch.cuda.synchronize()
-    return _take(vals, n, 1, "sdf grid")
+    return take(vals, n, "sdf grid")
 
 
 # ---------------------------------------------------------------------------------------------

@@ -234,7 +234,7 @@ def test_density(golden_dir):
     g = _g(golden_dir, "density")
     s = torch.from_numpy(g["sdf"]).cuda()
     out = torch.empty_like(s)
-    L.check(L.lib().mp_laplace_density(s.data_ptr(), s.numel(), float(g["beta"]), out.data_ptr(), L.stream_ptr()))
+    L.call("mp_laplace_density", s, s.numel(), float(g["beta"]), out)
     assert _maxabs(out.cpu().numpy(), g["sigma"]) < 1e-6 * max(1.0, float(np.abs(g["sigma"]).max()))
 
 
@@ -441,19 +441,18 @@ def test_branch_streams_match_single_stream():
     inp = S.make_rays(sc, 300, seed=3, region="boxes")
     hits = S.make_hit_lists(sc, inp)
     r = engine.Renderer(sc)
-    lib = L.lib()
     try:
-        L.check(lib.mp_set_streams(0), "mp_set_streams")
+        L.call("mp_set_streams", 0)
         ref = {k: v.clone() for k, v in r.render(inp, hits).items()}
         torch.cuda.synchronize()
-        L.check(lib.mp_set_streams(1), "mp_set_streams")
+        L.call("mp_set_streams", 1)
         for _ in range(3):
             o = r.render(inp, hits)
             torch.cuda.synchronize()
             for k in ("rgb_values", "fg_rgb_values", "normal_values", "acc_map", "acc_person_list"):
                 assert torch.equal(o[k], ref[k]), k
     finally:
-        lib.mp_set_streams(1)
+        L.call("mp_set_streams", 1)
 
 
 def test_edge_cases_single_ray_and_no_hits():

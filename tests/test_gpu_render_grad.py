@@ -28,7 +28,8 @@ for p in (ROOT, HERE):
         sys.path.insert(0, p)
 
 from oracle import render_grad as RG                            # noqa: E402
-from test_gpu_composite import make_inputs, wpc_of, SENTINEL     # noqa: E402
+from _abi import SENTINEL, padded, take                         # noqa: E402
+from test_gpu_composite import make_inputs, person_samples, wpc_of     # noqa: E402
 
 EPS = 2.0 ** -24
 TINY = 2.0 ** -102
@@ -123,58 +124,39 @@ def worst_c(persons, got, want, wbeta, got_beta, sc):
 # the C ABI with sentinel-padded gradient buffers
 # ---------------------------------------------------------------------------------------------
 
-def _pad(shape):
-    N = int(np.prod(shape))
-    return torch.full((N + 257,), SENTINEL, device="cuda")
+def grad_outputs(persons, n):
+    """Per person padded d sdf / d rgb / d normal buffers, and d_beta."""
+    return [dict(sdf=padded((d["idx"].size, n)), rgb=padded((d["idx"].size, n, 3)), nrm=padded((d["idx"].size, n, 3)))
+            for d in persons], padded(1)
 
 
-def call_backward(persons, R, n, beta, ups, P_arg=None, ws_delta=0, null_grad=None):
+def call_backward(persons, R, n, beta, ups, P_arg=None, ws_delta=0, null_grad=None, out=None):
+    """(gradient buffers, d_beta) as ``grad_outputs`` makes them (or ``out``), after the call."""
     from multiply_b200 import _lib as L
-    lib = L.lib()
     P = len(persons)
-    arr = (L.PersonSamples * P)()
+    arr, keep = person_samples(persons)
+    bufs, d_beta = grad_outputs(persons, n) if out is None else out
     gr = (L.PersonSampleGrads * P)()
-    keep, bufs = [], []
-    for p, d in enumerate(persons):
-        dev = {k: torch.from_numpy(np.ascontiguousarray(d[k])).cuda() if d["idx"].size else torch.zeros(1, device="cuda")
-               for k in ("z", "sdf", "rgb", "nrm")}
-        dev["idx"] = torch.from_numpy(d["idx"]).cuda() if d["idx"].size else torch.zeros(1, dtype=torch.int64, device="cuda")
-        keep.append(dev)
-        arr[p].n_rows = int(d["idx"].size)
-        arr[p].ray_index, arr[p].z_vals, arr[p].sdf = dev["idx"].data_ptr(), dev["z"].data_ptr(), dev["sdf"].data_ptr()
-        arr[p].rgb, arr[p].normal = dev["rgb"].data_ptr(), dev["nrm"].data_ptr()
-        Rp = d["idx"].size
-        b = dict(sdf=_pad((Rp, n)), rgb=_pad((Rp, n, 3)), nrm=_pad((Rp, n, 3)))
-        bufs.append(b)
-        gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = b["sdf"].data_ptr(), b["rgb"].data_ptr(), b["nrm"].data_ptr()
+    for p, b in enumerate(bufs):
+        gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = (L.ptr(b[k]) for k in ("sdf", "rgb", "nrm"))
         if null_grad == p:
             gr[p].d_rgb = None
     up = {k: (torch.from_numpy(v).cuda() if v is not None else None) for k, v in ups.items()}
-    d_beta = torch.full((8,), SENTINEL, device="cuda")
-    ws_bytes = lib.mp_composite_backward_workspace_bytes(R, P) + ws_delta
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device="cuda")
-    rc = lib.mp_composite_backward(arr, P if P_arg is None else P_arg, R, n, float(beta), L.ptr(up["d_fg"]),
-                                   L.ptr(up["d_nrm"]), L.ptr(up["d_acc"]), L.ptr(up["d_accp"]), L.ptr(up["d_bgT"]), gr,
-                                   d_beta.data_ptr(), ws.data_ptr(), ws_bytes, L.stream_ptr())
+    ws_bytes = L.call("mp_composite_backward_workspace_bytes", R, P) + ws_delta
+    ws = L.workspace(ws_bytes, "cuda")
+    L.call("mp_composite_backward", arr, P if P_arg is None else P_arg, R, n, float(beta), up["d_fg"], up["d_nrm"],
+           up["d_acc"], up["d_accp"], up["d_bgT"], gr, d_beta, ws, ws_bytes)
     torch.cuda.synchronize()
-    return rc, bufs, d_beta
-
-
-def _unpad(buf, shape, what):
-    N = int(np.prod(shape))
-    tail = buf[N:]
-    assert bool((tail == SENTINEL).all()), "%s: written past [R_p, n]" % what
-    return buf[:N].reshape(shape).cpu().numpy()
+    return bufs, d_beta
 
 
 def check_against(persons, R, n, beta, ups, bufs, d_beta, reverse=False, assert_ok=True, tag=""):
     """Worst c of (sdf, rgb, normal, beta) against the fp64 reference (optionally the reversed tie order)."""
     want, wbeta, sc = ref_backward(persons, R, n, beta, ups, reverse=reverse)
-    got = [{k: _unpad(bufs[p][k], shp, "%s p%d" % (k, p)) for k, shp in
+    got = [{k: take(bufs[p][k], shp, "%s p%d" % (k, p)).numpy() for k, shp in
             (("sdf", (d["idx"].size, n)), ("rgb", (d["idx"].size, n, 3)), ("nrm", (d["idx"].size, n, 3)))}
            for p, d in enumerate(persons)]
-    assert bool((d_beta[1:] == SENTINEL).all())
-    worst = worst_c(persons, got, want, wbeta, float(d_beta[0].cpu()), sc)
+    worst = worst_c(persons, got, want, wbeta, float(take(d_beta, 1, "d_beta")[0]), sc)
     if assert_ok:
         _note(tag or "composite_backward", worst)
         assert worst < C_GATE, (worst, tag)
@@ -197,11 +179,9 @@ def test_composite_backward_vs_fp64(P, n, beta):
     for j, R in enumerate(sorted({1, max(1, wpc - 1), wpc, wpc + 1, 2 * wpc + 1})):
         persons = make_inputs(77 * P + n + R, P, R, n, substitute=(R % 2 == 1))
         ups = _ups(R + n, R, P, NULLS[(j + P) % len(NULLS)])
-        rc, bufs, d_beta = call_backward(persons, R, n, beta, ups)
-        assert rc == 0
+        bufs, d_beta = call_backward(persons, R, n, beta, ups)
         check_against(persons, R, n, beta, ups, bufs, d_beta, tag="composite P=%d n=%d b=%g R=%d" % (P, n, beta, R))
-        rc, bufs2, d_beta2 = call_backward(persons, R, n, beta, ups)
-        assert rc == 0
+        bufs2, d_beta2 = call_backward(persons, R, n, beta, ups)
         for a, b in zip(bufs, bufs2):
             for k in a:
                 assert torch.equal(a[k].view(torch.int32), b[k].view(torch.int32)), k
@@ -214,10 +194,9 @@ def test_zero_sdf_gives_zero_gradient():
     persons = make_inputs(5, P, R, n, ties=False)
     for d in persons:
         d["sdf"][:, ::3] = 0.0
-    rc, bufs, _ = call_backward(persons, R, n, beta, _ups(1, R, P))
-    assert rc == 0
+    bufs, _ = call_backward(persons, R, n, beta, _ups(1, R, P))
     for p, d in enumerate(persons):
-        g = _unpad(bufs[p]["sdf"], d["sdf"].shape, "sdf")
+        g = take(bufs[p]["sdf"], d["sdf"].shape, "sdf").numpy()
         assert np.all(g[:, ::3] == 0) and np.any(g[:, 1::3] != 0)
 
 
@@ -231,8 +210,7 @@ def test_tie_order_backward():
         d["sdf"][row] = 1.0
         d["sdf"][row, -1] = -0.1 - 0.3 * p
     ups = _ups(3, R, P)
-    rc, bufs, d_beta = call_backward(persons, R, n, beta, ups)
-    assert rc == 0
+    bufs, d_beta = call_backward(persons, R, n, beta, ups)
     check_against(persons, R, n, beta, ups, bufs, d_beta, tag="tie order")
     c_rev = check_against(persons, R, n, beta, ups, bufs, d_beta, reverse=True, assert_ok=False)
     print("reversed order c=%.3g" % c_rev)
@@ -243,19 +221,20 @@ def test_rejected_calls_leave_outputs_untouched():
     """Bad P, a short workspace and a NULL required gradient buffer: negative status, mp_last_error text, nothing
     written."""
     from multiply_b200 import _lib as L
-    lib = L.lib()
     persons = make_inputs(4, 2, 5, 8)
     ups = _ups(2, 5, 2)
 
-    def untouched(bufs, d_beta):
-        return all(bool((b == SENTINEL).all()) for bb in bufs for b in bb.values()) and bool((d_beta == SENTINEL).all())
+    def rejected(text, **kw):
+        bufs, d_beta = out = grad_outputs(persons, 8)
+        with pytest.raises(L.MpError, match=r"failed \(-\d+\): .*" + text):
+            call_backward(persons, 5, 8, 0.1, ups, out=out, **kw)
+        assert all(bool((b == SENTINEL).all()) for bb in bufs for b in bb.values())
+        assert bool((d_beta == SENTINEL).all())
+
     for bad_P in (0, 9):
-        rc, bufs, d_beta = call_backward(persons, 5, 8, 0.1, ups, P_arg=bad_P)
-        assert rc < 0 and "bad person list" in lib.mp_last_error().decode() and untouched(bufs, d_beta)
-    rc, bufs, d_beta = call_backward(persons, 5, 8, 0.1, ups, ws_delta=-1)
-    assert rc < 0 and "workspace too small" in lib.mp_last_error().decode() and untouched(bufs, d_beta)
-    rc, bufs, d_beta = call_backward(persons, 5, 8, 0.1, ups, null_grad=1)
-    assert rc < 0 and "null argument" in lib.mp_last_error().decode() and untouched(bufs, d_beta)
+        rejected("bad person list", P_arg=bad_P)
+    rejected("workspace too small", ws_delta=-1)
+    rejected("null argument", null_grad=1)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -279,12 +258,10 @@ def test_bg_composite_backward(mode):
     d_out = rng.randn(R, 3).astype(np.float32)
     dv = {k: torch.from_numpy(v).cuda() for k, v in (("sdf", sdf), ("rgb", rgb), ("d", d_out))}
     tr = torch.from_numpy(t_rand).cuda() if t_rand is not None else None
-    g_sdf, g_rgb = _pad((R, 32)), _pad((R, 32, 3))
-    L.check(L.lib().mp_bg_composite_backward(dv["sdf"].data_ptr(), dv["rgb"].data_ptr(), R, bound, L.ptr(tr),
-                                             dv["d"].data_ptr(), g_sdf.data_ptr(), g_rgb.data_ptr(), L.stream_ptr()),
-            "mp_bg_composite_backward")
+    g_sdf, g_rgb = padded((R, 32)), padded((R, 32, 3))
+    L.call("mp_bg_composite_backward", dv["sdf"], dv["rgb"], R, bound, tr, dv["d"], g_sdf, g_rgb)
     torch.cuda.synchronize()
-    got_s, got_c = _unpad(g_sdf, (R, 32), "d_bg_sdf"), _unpad(g_rgb, (R, 32, 3), "d_bg_rgb")
+    got_s, got_c = take(g_sdf, (R, 32), "d_bg_sdf").numpy(), take(g_rgb, (R, 32, 3), "d_bg_rgb").numpy()
     z = torch.from_numpy(RG.bg_depths(R, bound, t_rand)).double()
     s = torch.from_numpy(sdf).double().requires_grad_(True)
     c = torch.from_numpy(rgb).double().requires_grad_(True)
@@ -311,11 +288,9 @@ def test_final_compose_backward(with_bg, with_fgv):
     bgT, bg = rng.random_sample(R).astype(np.float32), rng.random_sample((R, 3)).astype(np.float32)
     d_rgb, d_fgv = rng.randn(R, 3).astype(np.float32), rng.randn(R, 3).astype(np.float32)
     t = {k: torch.from_numpy(v).cuda() for k, v in (("bgT", bgT), ("bg", bg), ("d_rgb", d_rgb), ("d_fgv", d_fgv))}
-    o_fg, o_T, o_bg = _pad((R, 3)), _pad((R,)), _pad((R, 3))
-    L.check(L.lib().mp_final_compose_backward(t["bgT"].data_ptr(), t["bg"].data_ptr() if with_bg else None, R,
-                                              t["d_rgb"].data_ptr(), t["d_fgv"].data_ptr() if with_fgv else None,
-                                              o_fg.data_ptr(), o_T.data_ptr(), o_bg.data_ptr(), L.stream_ptr()),
-            "mp_final_compose_backward")
+    o_fg, o_T, o_bg = padded((R, 3)), padded(R), padded((R, 3))
+    L.call("mp_final_compose_backward", t["bgT"], t["bg"] if with_bg else None, R, t["d_rgb"],
+           t["d_fgv"] if with_fgv else None, o_fg, o_T, o_bg)
     torch.cuda.synchronize()
     dv = d_fgv if with_fgv else np.zeros_like(d_fgv)
     b = bg if with_bg else np.ones_like(bg)
@@ -324,9 +299,9 @@ def test_final_compose_backward(with_bg, with_fgv):
     for c in range(3):
         acc = (acc + ((d_rgb[:, c] * b[:, c]).astype(np.float32) + dv[:, c]).astype(np.float32)).astype(np.float32)
     want_bg = (bgT[:, None] * d_rgb).astype(np.float32)
-    assert np.array_equal(_unpad(o_fg, (R, 3), "d_fg").view(np.uint32), want_fg.view(np.uint32))
-    assert np.array_equal(_unpad(o_T, (R,), "d_bgT").view(np.uint32), acc.view(np.uint32))
-    assert np.array_equal(_unpad(o_bg, (R, 3), "d_bg").view(np.uint32), want_bg.view(np.uint32))
+    assert np.array_equal(take(o_fg, (R, 3), "d_fg").numpy().view(np.uint32), want_fg.view(np.uint32))
+    assert np.array_equal(take(o_T, (R,), "d_bgT").numpy().view(np.uint32), acc.view(np.uint32))
+    assert np.array_equal(take(o_bg, (R, 3), "d_bg").numpy().view(np.uint32), want_bg.view(np.uint32))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -336,7 +311,8 @@ def test_final_compose_backward(with_bg, with_fgv):
 def test_render_taps_leave_pixels_unchanged():
     """mp_render_rays with the background taps requested gives bit-identical pixels; the bg_rgb tap equals
     mp_background's output on the same rays, and the per-sample taps reproduce it through the restated blend."""
-    from multiply_b200 import engine, scene as S, _lib as L
+    from multiply_b200 import engine, scene as S
+    from multiply_b200.model import rend_util
     sc = S.make_scene(P=2, S=16, seed=42, weights="trained")
     inp = S.make_rays(sc, 96, seed=5, region="image")
     hits = S.make_hit_lists(sc, inp)
@@ -357,17 +333,10 @@ def test_render_taps_leave_pixels_unchanged():
         assert torch.equal(off[k].view(torch.int32), on[k].detach().view(torch.int32)), k
         assert not off[k].requires_grad and on[k].requires_grad
     # bg_rgb tap == mp_background on the eval depths
-    lib = L.lib()
     R = inp["uv"].shape[1]
-    uv, pose, K = (inp[k].reshape(-1).cuda().contiguous() for k in ("uv", "pose", "intrinsics"))
-    dirs, cam = torch.empty(R, 3, device="cuda"), torch.empty(R, 3, device="cuda")
-    L.check(lib.mp_camera_rays(uv.data_ptr(), pose.data_ptr(), K.data_ptr(), R, dirs.data_ptr(), cam.data_ptr(),
-                               L.stream_ptr()), "mp_camera_rays")
-    bg = torch.empty(R, 3, device="cuda")
+    dirs, cam = rend_util.camera_rays(inp["uv"].cuda(), inp["pose"], inp["intrinsics"])
     r.bg.set_cond(sc["frame_code"])
-    ws = torch.empty(lib.mp_background_workspace_bytes(R), dtype=torch.uint8, device="cuda")
-    L.check(lib.mp_background(r.bg.handle, dirs.data_ptr(), cam.data_ptr(), R, 3.0, bg.data_ptr(), ws.data_ptr(),
-                              ws.numel(), L.stream_ptr()), "mp_background")
+    bg = r.bg.bg_pixels(dirs, cam, 3.0)
     ev = r.render(inp, hits, train=dict(rng=rngs, t_rand_bg=None, beta=beta))
     torch.cuda.synchronize()
     assert torch.equal(ev["samples_bg"]["bg_rgb"].view(torch.int32), bg.view(torch.int32))
@@ -403,7 +372,7 @@ def _mirror_case(P, seed=33):
 
 def _run_mirror(m, inputs, pid, grad_on, streams=1):
     from multiply_b200 import _lib as L
-    L.check(L.lib().mp_set_streams(streams), "mp_set_streams")
+    L.call("mp_set_streams", streams)
     m.set_render_grad(grad_on)
     m.train()
     try:
@@ -411,7 +380,7 @@ def _run_mirror(m, inputs, pid, grad_on, streams=1):
         out = m(inputs, id=pid)
     finally:
         m.eval()
-        L.lib().mp_set_streams(1)
+        L.call("mp_set_streams", 1)
     return out
 
 

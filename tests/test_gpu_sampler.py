@@ -13,8 +13,8 @@ Exact checks, no tolerance, wherever the algorithm is deterministic:
 Float64 comparisons elsewhere (tests/_sampler_ref.py states the bound, the widenings and the masks):
 oracle/port.error_bound_get_z_vals in float64 with the draws of the GPU run, its SDF callback the GPU's own deformer and
 field at the fp32 points the kernels form, so both sides sample one function."""
-import ctypes as C
 import os
+import re
 import sys
 
 import pytest
@@ -29,9 +29,8 @@ if ROOT not in sys.path:
 from multiply_b200 import scene as S          # noqa: E402  (CPU-only module)
 from oracle import port                       # noqa: E402
 
+from _abi import SENTINEL, SENTINEL_INT, padded, take                                            # noqa: E402
 from _sampler_ref import EPS, MASK_MAX_M4096, MASK_MAX_TRIPS, cfg_of, compare, far_of, report      # noqa: E402
-
-SENTINEL = -1234.5
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -110,42 +109,40 @@ def train_rng(cfg, R, seed=0, edges=False):
     return dict(t_rand=t_rand, u_final=u_final, extra_perm=perm, eik_idx=eik, t_rand_bg=bg)
 
 
-def run(cfg, body, field, d, o, rng=None, ws=None, fill=None, out_fill=SENTINEL):
-    """One sampler call through the ABI.  Returns dict(z, z_bg, z_eik, trips) on the host (or the error text) and the
-    workspace it used; fill: byte value written into the workspace first."""
+def run(cfg, body, field, d, o, rng=None, ws=None, fill=None):
+    """One sampler call through the ABI.  Returns dict(err, z, z_bg, z_eik, trips) on the host -- err: the error text of
+    a rejected call, else None -- and the workspace it used; fill: byte value written into the workspace first."""
     from multiply_b200 import _lib as L, engine
-    lib = L.lib()
     c = c_cfg(cfg)
     R = d.shape[0]
     n = cfg["N_samples"] + cfg["N_samples_extra"] + 2
-    need = lib.mp_sampler_workspace_bytes(C.byref(c), R)
+    need = L.call("mp_sampler_workspace_bytes", c, R)
     if ws is None or ws.numel() < need:
-        ws = torch.empty(need, dtype=torch.uint8, device="cuda")
+        ws = L.workspace(need, "cuda")
     if fill is not None:
         ws.fill_(fill)
     dd, oo = d.cuda().contiguous(), o.cuda().contiguous()
-    z = torch.full((R, n), out_fill, device="cuda")
-    z_bg = torch.full((R, 32), out_fill, device="cuda")
-    z_eik = torch.full((R,), out_fill, device="cuda")
-    trips = torch.full((1,), -7, dtype=torch.int32, device="cuda")
-    if rng is None:
-        rc = lib.mp_sample_rays(C.byref(c), body.handle, field.handle, dd.data_ptr(), oo.data_ptr(), R, z.data_ptr(),
-                                z_bg.data_ptr(), trips.data_ptr(), ws.data_ptr(), ws.numel(), L.stream_ptr())
-    else:
-        r, keep = engine.sampler_rng_struct(rng, torch.device("cuda"))
-        rc = lib.mp_sample_rays_train(C.byref(c), body.handle, field.handle, dd.data_ptr(), oo.data_ptr(), R,
-                                      C.byref(r), z.data_ptr(), z_bg.data_ptr(), z_eik.data_ptr(), trips.data_ptr(),
-                                      ws.data_ptr(), ws.numel(), L.stream_ptr())
+    z, z_bg, z_eik, trips = padded((R, n)), padded((R, 32)), padded(R), padded(1, torch.int32)
+    err = None
+    try:
+        if rng is None:
+            L.call("mp_sample_rays", c, body.handle, field.handle, dd, oo, R, z, z_bg, trips, ws, ws.numel())
+        else:
+            r, keep = engine.sampler_rng_struct(rng, torch.device("cuda"))
+            L.call("mp_sample_rays_train", c, body.handle, field.handle, dd, oo, R, r, z, z_bg, z_eik, trips, ws,
+                   ws.numel())
+    except L.MpError as e:
+        err = str(e)
     torch.cuda.synchronize()
-    out = dict(rc=rc, err=lib.mp_last_error().decode() if rc else "", z=z.cpu(), z_bg=z_bg.cpu(), z_eik=z_eik.cpu(),
-               trips=int(trips.item()))
+    out = dict(err=err, z=take(z, (R, n), "z_vals"), z_bg=take(z_bg, (R, 32), "z_bg"), z_eik=take(z_eik, R, "z_eik"),
+               trips=int(take(trips, 1, "trips")[0]))
     return out, ws
 
 
 def check_rows(out, cfg, d, o, train=False):
     """Exact invariants of every output row: no sentinel, finite, sorted, inside [near, far], near and far present."""
     z = out["z"]
-    assert out["rc"] == 0, out["err"]
+    assert out["err"] is None, out["err"]
     assert not bool((z == SENTINEL).any()), "%d slots of z_vals unwritten" % int((z == SENTINEL).sum())
     assert not bool((out["z_bg"] == SENTINEL).any())
     assert bool(torch.isfinite(z).all())
@@ -169,7 +166,6 @@ def gpu_callback(body, field, verts_p):
     deform_rays_kernel does), evaluated by mp_sdf_with_deformer (outliers -> 4); the float64 nearest-vertex distance of
     each point is kept per call, to know the points near the 0.1 outlier radius."""
     from multiply_b200 import _lib as L
-    lib = L.lib()
     dist = []
     v64 = verts_p.double()
 
@@ -180,9 +176,8 @@ def gpu_callback(body, field, verts_p):
         xg = x.cuda()
         sdf = torch.empty(N, device="cuda")
         xc = torch.empty(N, 3, device="cuda")
-        ws = torch.empty(lib.mp_mlp_workspace_bytes(N) + N + 4096, dtype=torch.uint8, device="cuda")
-        L.check(lib.mp_sdf_with_deformer(body.handle, field.handle, xg.data_ptr(), N, sdf.data_ptr(), xc.data_ptr(),
-                                         None, ws.data_ptr(), ws.numel(), L.stream_ptr()), "mp_sdf_with_deformer")
+        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N) + N + 4096, "cuda")
+        L.call("mp_sdf_with_deformer", body.handle, field.handle, xg, N, sdf, xc, None, ws, ws.numel())
         d2, _, _ = port.knn_points(x.double()[None], v64[None], return_nn=False)
         dist.append(d2[0, :, 0].sqrt().reshape(z.shape))
         return sdf.cpu().double()[:, None]
@@ -217,11 +212,11 @@ def test_rejects_invalid_configs(scene, person):
             r = train_rng(dict(cfg, N_samples=max(cfg["N_samples"], 1), N_samples_extra=max(cfg["N_samples_extra"], 0),
                                max_total_iters=min(max(cfg["max_total_iters"], 1), 8)), 8) if rng else None
             out, _ = run(cfg, person["body"], person["field"], d, o, rng=r)
-            assert out["rc"] != 0 and "sampler" in out["err"], (cfg, out["err"])
-            assert bool((out["z"] == SENTINEL).all()) and out["trips"] == -7
+            assert re.search(r"failed \(-\d+\): .*sampler", out["err"] or ""), (cfg, out["err"])
+            assert bool((out["z"] == SENTINEL).all()) and out["trips"] == SENTINEL_INT
     cfg = cfg_of(16, 8, 17, 2)
     out, _ = run(cfg, person["body"], person["field"], d, o, rng=train_rng(cfg, 8))
-    assert out["rc"] != 0 and "N_samples_extra" in out["err"], out["err"]
+    assert re.search(r"failed \(-\d+\): .*N_samples_extra", out["err"] or ""), out["err"]
     assert bool((out["z"] == SENTINEL).all()) and bool((out["z_eik"] == SENTINEL).all())
     # the same configuration is valid in eval mode (the extras come from linspace(0, M-1, X))
     out, _ = run(cfg, person["body"], person["field"], d, o)
@@ -415,7 +410,7 @@ def test_geometry_edges(scene, person):
     dd2 = torch.tensor([[0.0, 0.0, 1.0], [0.0, 0.1, 0.995], [0.1, 0.0, 0.995]])
     dd2 = dd2 / dd2.norm(dim=1, keepdim=True)
     out, _ = run(cfg, person["body"], person["field"], dd2, oo2)
-    assert out["rc"] == 0 and not bool((out["z"] == SENTINEL).any())
+    assert out["err"] is None and not bool((out["z"] == SENTINEL).any())
     assert bool((out["z"] == 0).all()), "far clamped to 0 must give a row of zeros"
 
 
