@@ -160,6 +160,30 @@ int mp_deform_inverse(mp_body_t* b, const float* x, int N, float* x_c, uint8_t* 
  * the upper-left 3x3 of sum_j w_j tfs_j with w from the nearest CANONICAL vertex. */
 int mp_deform_forward_jac(mp_body_t* b, const float* x_c, int N, float* x_d, float* Jinv, void* stream);
 
+/* Backward of the two deformer calls (VJPs; the weights are detached, deformer.py:47, so gradients reach the points and
+ * the bone transforms only).  Both use the body's current pose (mp_body_set_pose), recompute the nearest vertex with the
+ * forward's own search, and write every element of d_tfs [24,4,4] (= dL/d smpl_tfs; N = 0 gives zeros).  Sums over
+ * points are per-CTA partials added in a fixed order (no float atomics): reruns are bit-identical.  Workspace:
+ * mp_deform_backward_workspace_bytes(N); its contents on entry do not matter.
+ *
+ * mp_deform_inverse_backward: of mp_deform_inverse (skinning(inverse=True), deformer.py:72-89, weights of the nearest
+ * POSED vertex).  d_x_c [N,3] required; with A = sum_j w_j tfs_j, u = A[:3,:3]^-T d_x_c: dL/dA = -[u ; -t.u/s] [x_c ; 1]^T
+ * (all four rows, as torch's inverse backward gives them), d_x [N,3] = u (NULL: not written), x_c [N,3] = the recomputed
+ * canonical point, bit-equal to mp_deform_inverse's (NULL: not written).  A point with no vertex within reach
+ * (exact_far == 0) has x_c = x: d_x = d_x_c, nothing to the bones.  Refused while the body's root finder is on (the
+ * reference has none, so that gradient has no definition to match).
+ *
+ * mp_deform_forward_jac_backward: of mp_deform_forward_jac (forward skinning with the weights of the nearest CANONICAL
+ * vertex, deformer.py:31-35, and the inverse Jacobian of multiply.py:625-641).  d_x_d [N,3] and d_Jinv [N,9] may be NULL
+ * (zero).  dL/dJ = -Jinv^T d_Jinv Jinv^T and d_x_d [x_c;1]^T go to tfs_j[:3,:]; the bottom row of d_tfs is 0.
+ * d_x_c [N,3] = J^T d_x_d (NULL: not written). */
+size_t mp_deform_backward_workspace_bytes(int N);
+int mp_deform_inverse_backward(mp_body_t* b, const float* x, int N, int exact_far, const float* d_x_c,
+                               float* d_tfs, float* d_x, float* x_c, void* workspace, size_t workspace_bytes,
+                               void* stream);
+int mp_deform_forward_jac_backward(mp_body_t* b, const float* x_c, int N, const float* d_x_d, const float* d_Jinv,
+                                   float* d_tfs, float* d_x_c, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Optional root finder (SURVEY.md §8 row f4; BASELINE.json north_star: "Broyden-root-finds canonical points").  The
  * reference has NO such step (SURVEY.md fact 0-1: its deformer is KNN + closed-form inverse LBS, deformer.py:19-50), so
  * this is non-default and checked against its own CPU restatement (oracle/port.py:deform_broyden), not against MultiPly.
@@ -221,6 +245,19 @@ int mp_smpl_canonical(mp_smpl_t* s, float* verts_c, float* tfs_c_inv, void* stre
 /* scale [1], transl [3], thetas [72], betas [10] (device) -> smpl_verts [V,3], smpl_tfs [24,4,4] */
 int mp_smpl_forward(mp_smpl_t* s, const float* scale, const float* transl, const float* thetas, const float* betas,
                     int absolute, float* smpl_verts, float* smpl_tfs, void* stream);
+/* Backward (VJP) of mp_smpl_forward with the same inputs: d_verts [V,3] and d_tfs [24,4,4] are the upstream gradients
+ * (either may be NULL: zero; the bottom row of d_tfs reaches no parameter and is ignored) -> d_scale [1], d_transl [3],
+ * d_thetas [72], d_betas [10], every element written.  Reverses skinning, the pose blend (posedirs), the shape blend
+ * (shapedirs), J = J_t + J_s betas, the kinematic chain, the rel_transforms correction (lbs.py:371-376), Rodrigues as
+ * lbs.py:276-307 writes it (angle = |theta + 1e-8|; theta = 0 gets the finite skew-basis derivative), scale /
+ * translation (smpl.py:86-88) and the tfs_c_inv product when absolute == 0.  Everything is recomputed from the inputs
+ * (the handle's per-call scratch is not read); the per-joint part runs in fp64.  Sums over vertices are per-CTA partials
+ * added in a fixed order: reruns are bit-identical.  A server built with v_template ignores betas (smpl.py:65-66): its
+ * caller passes zero betas and discards d_betas.  Workspace: mp_smpl_backward_workspace_bytes(V), any contents. */
+size_t mp_smpl_backward_workspace_bytes(int V);
+int mp_smpl_backward(mp_smpl_t* s, const float* scale, const float* transl, const float* thetas, const float* betas,
+                     int absolute, const float* d_verts, const float* d_tfs, float* d_scale, float* d_transl,
+                     float* d_thetas, float* d_betas, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * sampler: ErrorBoundSampler (lib/model/ray_sampler.py:45-230), eval mode

@@ -134,6 +134,9 @@ SIGNATURES = {
     "mp_body_set_pose": (STATUS, [_VP, _VP, _VP, STREAM]),
     "mp_deform_inverse": (STATUS, [_VP, _VP, _I, _VP, _VP, _I, STREAM]),
     "mp_deform_forward_jac": (STATUS, [_VP, _VP, _I, _VP, _VP, STREAM]),
+    "mp_deform_backward_workspace_bytes": (_SZ, [_I]),
+    "mp_deform_inverse_backward": (STATUS, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_deform_forward_jac_backward": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_deform_broyden": (STATUS, [_VP, _VP, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, STREAM]),
     "mp_body_set_root_finder": (STATUS, [_VP, _I, _F]),
     "mp_laplace_density": (STATUS, [_VP, _I, _F, _VP, STREAM]),
@@ -148,6 +151,8 @@ SIGNATURES = {
     "mp_smpl_free": (None, [_VP]),
     "mp_smpl_canonical": (STATUS, [_VP, _VP, _VP, STREAM]),
     "mp_smpl_forward": (STATUS, [_VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, STREAM]),
+    "mp_smpl_backward_workspace_bytes": (_SZ, [_I]),
+    "mp_smpl_backward": (STATUS, [_VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_sampler_workspace_bytes": (_SZ, [C.POINTER(SamplerCfg), _I]),
     "mp_sample_rays": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_sample_rays_train": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, C.POINTER(SamplerRng), _VP, _VP, _VP,

@@ -352,8 +352,9 @@ __device__ __noinline__ void broyden_refine(const Body& b, float px, float py, f
 
 // Shared per-point routine of the inverse deformer.  ROOT = false is the reference's path; the ROOT = true
 // instantiations exist so that the optional refinement costs the default kernels neither registers nor stack.
+// Returns the vertex whose weights were used (0x7fffffff: none within reach, x_c = x).
 template <bool ROOT = false>
-__device__ __forceinline__ void deform_inverse_point(const Body& b, const GridHeader& g, float px, float py, float pz,
+__device__ __forceinline__ int deform_inverse_point(const Body& b, const GridHeader& g, float px, float py, float pz,
                                                      bool exact_far, float xc[3], bool& outlier) {
   float d2;
   int vi;
@@ -366,7 +367,7 @@ __device__ __forceinline__ void deform_inverse_point(const Body& b, const GridHe
     xc[0] = px;
     xc[1] = py;
     xc[2] = pz;
-    return;
+    return vi;
   }
   // [A t; 0 s]^-1 [x;1] = A^-1 (x - t/s), from the per-vertex table
   const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
@@ -380,6 +381,7 @@ __device__ __forceinline__ void deform_inverse_point(const Body& b, const GridHe
     int steps;
     broyden_refine(b, px, py, pz, b.root_steps, b.root_thr, xc, resid, steps);
   }
+  return vi;
 }
 
 __global__ void deform_broyden_kernel(Body b, const float* __restrict__ x, int N, int max_steps, float thr,
@@ -504,6 +506,175 @@ __global__ void deform_forward_jac_kernel(Body b, const float* __restrict__ x_c,
       o[0] = r0.x; o[1] = r0.y; o[2] = r0.z; o[3] = r1.x; o[4] = r1.y; o[5] = r1.z; o[6] = r2.x; o[7] = r2.y; o[8] = r2.z;
     }
   }
+}
+
+// ---- backward (VJPs of mp_deform_inverse and mp_deform_forward_jac) ------------------------------------------------
+// Every point's dL/d(blended transform) goes to the bones with its (detached) vertex weights: d_tfs_j = sum_i w_ij dA_i.
+// A fixed grid of CTAs walks the points in a fixed order; per warp the 32 points' terms are added by shuffles and lane 0
+// accumulates them in fp64 shared memory; each CTA leaves one partial [24,16] and bone_grad_final_kernel adds the
+// partials in CTA order.  No atomics: reruns are bit-identical.
+constexpr int kBgThreads = 256, kBgMaxBlocks = 1024, kBoneGrad = MP_NUM_JOINTS * 16;
+
+static int bone_grad_blocks(int N) { return N > 0 ? std::min(div_up(N, kBgThreads), kBgMaxBlocks) : 0; }
+
+// acc[16 j + 4 r + c] += sum over the warp's lanes of w_j dA[4 r + c], rows r < NROW; w == nullptr: the lane adds nothing.
+// Every lane of the warp must call it.
+template <int NROW>
+__device__ __forceinline__ void bone_grad_warp(const float* __restrict__ w, const float dA[16], double* acc, int lane) {
+  const float4* w4 = reinterpret_cast<const float4*>(w);
+#pragma unroll 1
+  for (int j4 = 0; j4 < MP_NUM_JOINTS / 4; ++j4) {
+    float4 ww = w ? __ldg(w4 + j4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float wv[4] = {ww.x, ww.y, ww.z, ww.w};
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const float wj = wv[u];
+      if (!__any_sync(0xffffffffu, wj != 0.f)) continue;
+      double* a = acc + 16 * (4 * j4 + u);
+#pragma unroll
+      for (int k = 0; k < 4 * NROW; ++k) {
+        const float t = warp_sum(wj * dA[k]);
+        if (lane == 0) a[k] += (double)t;
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ void bone_grad_zero(double (*acc)[kBoneGrad]) {
+  for (int i = threadIdx.x; i < (kBgThreads / 32) * kBoneGrad; i += blockDim.x) acc[i / kBoneGrad][i % kBoneGrad] = 0.0;
+  __syncthreads();
+}
+
+__device__ __forceinline__ void bone_grad_store(double (*acc)[kBoneGrad], double* __restrict__ partials) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < kBoneGrad; i += blockDim.x) {
+    double t = acc[0][i];
+    for (int q = 1; q < kBgThreads / 32; ++q) t += acc[q][i];
+    partials[(size_t)blockIdx.x * kBoneGrad + i] = t;
+  }
+}
+
+__global__ void __launch_bounds__(kBoneGrad) bone_grad_final_kernel(const double* __restrict__ partials, int nblk,
+                                                                    float* __restrict__ d_tfs) {
+  const int i = threadIdx.x;
+  double t = 0.0;
+  for (int q = 0; q < nblk; ++q) t += partials[(size_t)q * kBoneGrad + i];
+  d_tfs[i] = (float)t;
+}
+
+// x_c = (A^-1 [x;1])[:3] with A = sum_j w_j tfs_j = [M t; 0 s]: with u = M^-T g and tau = t / s (the forward's table),
+// dL/dA = -[u ; -tau.u] [x_c ; 1]^T and dL/dx = u.  All four rows go to the bones, as torch's inverse backward gives them.
+__global__ void __launch_bounds__(kBgThreads) deform_inverse_backward_kernel(Body b, const float* __restrict__ x, int N,
+                                                                             int exact_far, const float* __restrict__ d_xc,
+                                                                             float* __restrict__ d_x,
+                                                                             float* __restrict__ x_c_out,
+                                                                             double* __restrict__ partials) {
+  __shared__ double acc[kBgThreads / 32][kBoneGrad];
+  bone_grad_zero(acc);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const GridHeader g = *b.posed_hdr;
+  for (int base = blockIdx.x * kBgThreads; base < N; base += gridDim.x * kBgThreads) {
+    const int i = base + threadIdx.x;
+    float dA[16];                       // zero for lanes without a point or a vertex: bone_grad_warp multiplies by w = 0
+#pragma unroll
+    for (int k = 0; k < 16; ++k) dA[k] = 0.f;
+    const float* w = nullptr;
+    if (i < N) {
+      const float px = x[3 * i], py = x[3 * i + 1], pz = x[3 * i + 2];
+      float xc[3];
+      bool o;
+      const int vi = deform_inverse_point<false>(b, g, px, py, pz, exact_far != 0, xc, o);
+      const float gx = d_xc[3 * i], gy = d_xc[3 * i + 1], gz = d_xc[3 * i + 2];
+      float u[3] = {gx, gy, gz};        // no vertex within reach: x_c = x
+      if (vi != 0x7fffffff) {
+        const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
+                     r2 = __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
+        u[0] = r0.x * gx + r1.x * gy + r2.x * gz;
+        u[1] = r0.y * gx + r1.y * gy + r2.y * gz;
+        u[2] = r0.z * gx + r1.z * gy + r2.z * gz;
+        const float tu = r0.w * u[0] + r1.w * u[1] + r2.w * u[2];
+        const float a[4] = {-u[0], -u[1], -u[2], tu}, bb[4] = {xc[0], xc[1], xc[2], 1.f};
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) dA[4 * r + c] = a[r] * bb[c];
+        w = b.weights + (size_t)vi * MP_NUM_JOINTS;
+      }
+      if (d_x) {
+        d_x[3 * i] = u[0];
+        d_x[3 * i + 1] = u[1];
+        d_x[3 * i + 2] = u[2];
+      }
+      if (x_c_out) {
+        x_c_out[3 * i] = xc[0];
+        x_c_out[3 * i + 1] = xc[1];
+        x_c_out[3 * i + 2] = xc[2];
+      }
+    }
+    bone_grad_warp<4>(w, dA, acc[warp], lane);
+  }
+  bone_grad_store(acc, partials);
+}
+
+// x_d = M x_c + t and Jinv = M^-1 with M, t blended with the weights of the nearest CANONICAL vertex (the forward's
+// search and table): dL/dM = -Jinv^T d_Jinv Jinv^T, dL/dT[:3,:] += d_x_d [x_c;1]^T, dL/dx_c = M^T d_x_d (the weights are
+// piecewise constant, so Jinv contributes nothing to it).  The bottom row of d_tfs is 0.
+__global__ void __launch_bounds__(kBgThreads) deform_forward_jac_backward_kernel(
+    Body b, const float* __restrict__ x_c, int N, const float* __restrict__ d_xd, const float* __restrict__ d_Jinv,
+    float* __restrict__ d_xc, double* __restrict__ partials) {
+  __shared__ double acc[kBgThreads / 32][kBoneGrad];
+  bone_grad_zero(acc);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const GridHeader g = *b.cano_hdr;
+  for (int base = blockIdx.x * kBgThreads; base < N; base += gridDim.x * kBgThreads) {
+    const int i = base + threadIdx.x;
+    float dA[16];                       // zero for lanes without a point or a vertex: bone_grad_warp multiplies by w = 0
+#pragma unroll
+    for (int k = 0; k < 16; ++k) dA[k] = 0.f;
+    const float* w = nullptr;
+    if (i < N) {
+      const float px = x_c[3 * i], py = x_c[3 * i + 1], pz = x_c[3 * i + 2];
+      float d2;
+      int vi;
+      nearest_vertex(g, b.cano_cell_start, b.cano_sorted, b.V, px, py, pz, true, d2, vi);
+      w = b.weights + (size_t)vi * MP_NUM_JOINTS;
+      float dxc[3] = {0.f, 0.f, 0.f};
+      if (d_xd) {
+        const float gx = d_xd[3 * i], gy = d_xd[3 * i + 1], gz = d_xd[3 * i + 2];
+        const float gg[3] = {gx, gy, gz}, xh[4] = {px, py, pz, 1.f};
+        float T[12], s;
+        blend_tf(w, b.tfs, T, s);
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) dA[4 * r + c] = gg[r] * xh[c];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) dxc[c] = T[c] * gx + T[4 + c] * gy + T[8 + c] * gz;
+      }
+      if (d_Jinv) {
+        const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
+                     r2 = __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
+        const float I[9] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z};
+        const float* dJ = d_Jinv + 9 * (size_t)i;
+        float H[9];   // d_Jinv Jinv^T
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) H[3 * r + c] = dJ[3 * r] * I[3 * c] + dJ[3 * r + 1] * I[3 * c + 1] + dJ[3 * r + 2] * I[3 * c + 2];
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) dA[4 * r + c] -= I[r] * H[c] + I[3 + r] * H[3 + c] + I[6 + r] * H[6 + c];
+      }
+      if (d_xc) {
+        d_xc[3 * i] = dxc[0];
+        d_xc[3 * i + 1] = dxc[1];
+        d_xc[3 * i + 2] = dxc[2];
+      }
+    }
+    bone_grad_warp<3>(w, dA, acc[warp], lane);
+  }
+  bone_grad_store(acc, partials);
 }
 
 int body_build_grid(const float* verts, int V, float cell, int R0, GridHeader* hdr, int* cell_start, float4* sorted,
@@ -647,5 +818,50 @@ int mp_deform_broyden(mp_body_t* h, const float* x, int N, int max_steps, float 
 int mp_deform_forward_jac(mp_body_t* h, const float* x_c, int N, float* x_d, float* Jinv, void* stream) {
   MP_REQUIRE(h && h->b.tfs, "mp_deform_forward_jac: body has no pose (call mp_body_set_pose)");
   return mp::launch_forward_jac(h->b, x_c, N, nullptr, x_d, Jinv, 9, (cudaStream_t)stream);
+}
+
+size_t mp_deform_backward_workspace_bytes(int N) {
+  return mp::align_up((size_t)mp::bone_grad_blocks(N) * mp::kBoneGrad * sizeof(double), 256) + 256;
+}
+
+int mp_deform_inverse_backward(mp_body_t* h, const float* x, int N, int exact_far, const float* d_x_c, float* d_tfs,
+                               float* d_x, float* x_c, void* workspace, size_t workspace_bytes, void* stream) {
+  MP_REQUIRE(h && h->b.tfs, "mp_deform_inverse_backward: body has no pose (call mp_body_set_pose)");
+  MP_REQUIRE(h->b.root_steps == 0,
+             "mp_deform_inverse_backward: the body's root finder is on; only the closed-form inverse has a backward");
+  MP_REQUIRE(d_tfs && N >= 0 && (N == 0 || (x && d_x_c)), "mp_deform_inverse_backward: null argument");
+  MP_REQUIRE(workspace && workspace_bytes >= mp_deform_backward_workspace_bytes(N),
+             "mp_deform_inverse_backward: workspace too small (%zu < %zu)", workspace_bytes,
+             mp_deform_backward_workspace_bytes(N));
+  cudaStream_t st = (cudaStream_t)stream;
+  double* partials = (double*)mp::align_up((size_t)workspace, 256);
+  const int nblk = mp::bone_grad_blocks(N);
+  if (nblk) {
+    mp::deform_inverse_backward_kernel<<<nblk, mp::kBgThreads, 0, st>>>(h->b, x, N, exact_far, d_x_c, d_x, x_c,
+                                                                       partials);
+    MP_LAUNCH_CHECK();
+  }
+  mp::bone_grad_final_kernel<<<1, mp::kBoneGrad, 0, st>>>(partials, nblk, d_tfs);
+  MP_LAUNCH_CHECK();
+  return 0;
+}
+
+int mp_deform_forward_jac_backward(mp_body_t* h, const float* x_c, int N, const float* d_x_d, const float* d_Jinv,
+                                   float* d_tfs, float* d_x_c, void* workspace, size_t workspace_bytes, void* stream) {
+  MP_REQUIRE(h && h->b.tfs, "mp_deform_forward_jac_backward: body has no pose (call mp_body_set_pose)");
+  MP_REQUIRE(d_tfs && N >= 0 && (N == 0 || x_c), "mp_deform_forward_jac_backward: null argument");
+  MP_REQUIRE(workspace && workspace_bytes >= mp_deform_backward_workspace_bytes(N),
+             "mp_deform_forward_jac_backward: workspace too small (%zu < %zu)", workspace_bytes,
+             mp_deform_backward_workspace_bytes(N));
+  cudaStream_t st = (cudaStream_t)stream;
+  double* partials = (double*)mp::align_up((size_t)workspace, 256);
+  const int nblk = mp::bone_grad_blocks(N);
+  if (nblk) {
+    mp::deform_forward_jac_backward_kernel<<<nblk, mp::kBgThreads, 0, st>>>(h->b, x_c, N, d_x_d, d_Jinv, d_x_c, partials);
+    MP_LAUNCH_CHECK();
+  }
+  mp::bone_grad_final_kernel<<<1, mp::kBoneGrad, 0, st>>>(partials, nblk, d_tfs);
+  MP_LAUNCH_CHECK();
+  return 0;
 }
 }

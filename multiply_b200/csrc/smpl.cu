@@ -162,16 +162,9 @@ __global__ void __launch_bounds__(1024) smpl_pose_kernel(Smpl m, const float* __
 // per vertex: pose blend shapes + skinning + SMPLServer's scale/translation
 //   v_posed = v_shaped + pose_feature @ posedirs ; T = W @ A ; verts = T v_posed      lbs.py:201-227, smpl.py:78
 // A_abs already carries the scale and translation: (s*A_rot) v + (s*A_t + t*s) = s*(A v) + t*s.
-__global__ void smpl_skin_kernel(Smpl m, const float* __restrict__ betas, float* __restrict__ verts_out) {
-  __shared__ float spf[207];
-  __shared__ float sA[MP_NUM_JOINTS * 16];
-  __shared__ float sb[10];
-  if (threadIdx.x < 10) sb[threadIdx.x] = betas[threadIdx.x];
-  for (int i = threadIdx.x; i < 207; i += blockDim.x) spf[i] = m.pose_feature[i];
-  for (int i = threadIdx.x; i < MP_NUM_JOINTS * 16; i += blockDim.x) sA[i] = m.A_abs[i];
-  __syncthreads();
-  int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= m.V) return;
+// smpl_vertex is the per-vertex part, shared with the backward so that both see the same x = v_posed and T.
+__device__ __forceinline__ void smpl_vertex(const Smpl& m, const float* spf, const float* sA, const float* sb, int v,
+                                            float xo[3], float T[12]) {
   const size_t ld = (size_t)m.V * 3;
   float p0 = 0.f, p1 = 0.f, p2 = 0.f;
   for (int k = 0; k < 207; ++k) {
@@ -191,8 +184,9 @@ __global__ void smpl_skin_kernel(Smpl m, const float* __restrict__ betas, float*
     for (int l = 0; l < 10; ++l) sacc = fmaf(sb[l], sd[l], sacc);
     vs[a] = m.v_template[3 * v + a] + sacc;
   }
-  float x = vs[0] + p0, y = vs[1] + p1, z = vs[2] + p2;
-  float T[12];
+  xo[0] = vs[0] + p0;
+  xo[1] = vs[1] + p1;
+  xo[2] = vs[2] + p2;
 #pragma unroll
   for (int k = 0; k < 12; ++k) T[k] = 0.f;
   const float* w = m.lbs_weights + (size_t)v * MP_NUM_JOINTS;
@@ -202,9 +196,27 @@ __global__ void smpl_skin_kernel(Smpl m, const float* __restrict__ betas, float*
 #pragma unroll
     for (int k = 0; k < 12; ++k) T[k] = fmaf(wj, sA[16 * j + k], T[k]);
   }
-  verts_out[3 * v] = T[0] * x + T[1] * y + T[2] * z + T[3];
-  verts_out[3 * v + 1] = T[4] * x + T[5] * y + T[6] * z + T[7];
-  verts_out[3 * v + 2] = T[8] * x + T[9] * y + T[10] * z + T[11];
+}
+
+__device__ __forceinline__ void smpl_load_shared(const Smpl& m, const float* betas, float* spf, float* sA, float* sb) {
+  if (threadIdx.x < 10) sb[threadIdx.x] = betas[threadIdx.x];
+  for (int i = threadIdx.x; i < 207; i += blockDim.x) spf[i] = m.pose_feature[i];
+  for (int i = threadIdx.x; i < MP_NUM_JOINTS * 16; i += blockDim.x) sA[i] = m.A_abs[i];
+}
+
+__global__ void smpl_skin_kernel(Smpl m, const float* __restrict__ betas, float* __restrict__ verts_out) {
+  __shared__ float spf[207];
+  __shared__ float sA[MP_NUM_JOINTS * 16];
+  __shared__ float sb[10];
+  smpl_load_shared(m, betas, spf, sA, sb);
+  __syncthreads();
+  int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= m.V) return;
+  float x[3], T[12];
+  smpl_vertex(m, spf, sA, sb, v, x, T);
+  verts_out[3 * v] = T[0] * x[0] + T[1] * x[1] + T[2] * x[2] + T[3];
+  verts_out[3 * v + 1] = T[4] * x[0] + T[5] * x[1] + T[6] * x[2] + T[7];
+  verts_out[3 * v + 2] = T[8] * x[0] + T[9] * x[1] + T[10] * x[2] + T[11];
 }
 
 // tfs_c_inv = inverse of 24 affine 4x4 matrices (bottom row 0 0 0 1)      smpl.py:47
@@ -226,6 +238,283 @@ __global__ void affine_inverse_kernel(const float* __restrict__ T, float* __rest
   o[12] = o[13] = o[14] = 0.f;
   o[15] = 1.f;
 }
+
+// ---- backward (VJP of mp_smpl_forward) ----------------------------------------------------------------------------
+// The per-vertex pass reverses the skinning, the pose blend and the shape blend of every vertex and leaves per-block
+// partial sums of dL/dA_j (rows 0..2), dL/dpose_feature and dL/dbetas; one CTA adds them in block order and reverses the
+// 24-joint part in fp64.  pose_feature / A_abs are recomputed into the workspace by smpl_pose_kernel itself, so the
+// handle's per-call scratch (which a later forward overwrites) is never read.
+constexpr int kSmplBwdThreads = 128;
+constexpr int kSmplNA = MP_NUM_JOINTS * 12, kSmplNP = kSmplNA + 207 + 10;   // dA rows 0..2 | d pose_feature | d betas
+
+__global__ void __launch_bounds__(kSmplBwdThreads) smpl_skin_backward_kernel(Smpl m, const float* __restrict__ betas,
+                                                                             const float* __restrict__ d_verts,
+                                                                             float* __restrict__ partials) {
+  __shared__ float spf[207];
+  __shared__ float sA[MP_NUM_JOINTS * 16];
+  __shared__ float sb[10];
+  __shared__ float red[kSmplBwdThreads / 32][kSmplNP];
+  smpl_load_shared(m, betas, spf, sA, sb);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = v < m.V;
+  float x[3] = {0.f, 0.f, 0.f}, T[12], g[3] = {0.f, 0.f, 0.f};
+  if (valid) {
+    smpl_vertex(m, spf, sA, sb, v, x, T);
+    g[0] = d_verts[3 * v];
+    g[1] = d_verts[3 * v + 1];
+    g[2] = d_verts[3 * v + 2];
+  } else {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) T[k] = 0.f;
+  }
+  const float xh[4] = {x[0], x[1], x[2], 1.f};
+  // verts = T[:3,:] [x;1]:  dT = g [x;1]^T (dA_j = w_j dT), dx = T[:3,:3]^T g
+  float dx[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) dx[c] = T[c] * g[0] + T[4 + c] * g[1] + T[8 + c] * g[2];
+  const float* w = m.lbs_weights + (size_t)(valid ? v : 0) * MP_NUM_JOINTS;
+  for (int j = 0; j < MP_NUM_JOINTS; ++j) {
+    const float wj = valid ? w[j] : 0.f;
+    const bool any = __any_sync(0xffffffffu, wj != 0.f);
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const float t = any ? warp_sum(wj * g[r] * xh[c]) : 0.f;
+        if (lane == 0) red[warp][12 * j + 4 * r + c] = t;
+      }
+  }
+  // v_posed = v_shaped + pose_feature @ posedirs:  d pose_feature[k] = sum_v posedirs[k, v] . dx_v
+  const size_t ld = (size_t)m.V * 3;
+  for (int k = 0; k < 207; ++k) {
+    float t = 0.f;
+    if (valid) {
+      const float* pd = m.posedirs + (size_t)k * ld + 3 * (size_t)v;
+      t = pd[0] * dx[0] + pd[1] * dx[1] + pd[2] * dx[2];
+    }
+    t = warp_sum(t);
+    if (lane == 0) red[warp][kSmplNA + k] = t;
+  }
+  // v_shaped = v_template + shapedirs . betas:  d betas[l] = sum_v shapedirs[v, :, l] . dx_v
+  for (int l = 0; l < 10; ++l) {
+    float t = 0.f;
+    if (valid) {
+      const float* sd = m.shapedirs + (size_t)3 * v * 10 + l;
+      t = sd[0] * dx[0] + sd[10] * dx[1] + sd[20] * dx[2];
+    }
+    t = warp_sum(t);
+    if (lane == 0) red[warp][kSmplNA + 207 + l] = t;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kSmplNP; i += blockDim.x) {
+    float t = red[0][i];
+    for (int q = 1; q < kSmplBwdThreads / 32; ++q) t += red[q][i];
+    partials[(size_t)blockIdx.x * kSmplNP + i] = t;
+  }
+}
+
+// Rodrigues exactly as lbs.py:276-307 writes it (angle = |theta + 1e-8|, axis = theta / angle), in fp64:
+// R = I + sin(a) K + (1 - cos(a)) K K with K = skew(axis).  At theta = 0 the axis is 0 and sin(a) / a -> 1, so dR
+// reaches theta through the skew basis, as torch autograd's derivative of the same expression does.
+__device__ void rodrigues64(const float* th, double R[9], double K[9], double& ang, double a[3], double& c, double& s) {
+  double t2 = 0.0;
+  for (int q = 0; q < 3; ++q) {
+    a[q] = (double)th[q] + 1e-8;
+    t2 += a[q] * a[q];
+  }
+  ang = sqrt(t2);
+  const double dx = th[0] / ang, dy = th[1] / ang, dz = th[2] / ang;
+  c = cos(ang);
+  s = sin(ang);
+  const double Kv[9] = {0.0, -dz, dy, dz, 0.0, -dx, -dy, dx, 0.0};
+  for (int i = 0; i < 9; ++i) K[i] = Kv[i];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      double kk = 0.0;
+      for (int k = 0; k < 3; ++k) kk += K[3 * i + k] * K[3 * k + j];
+      R[3 * i + j] = (i == j ? 1.0 : 0.0) + s * K[3 * i + j] + (1.0 - c) * kk;
+    }
+}
+
+__global__ void __launch_bounds__(512) smpl_backward_final_kernel(
+    Smpl m, const float* __restrict__ scale_p, const float* __restrict__ transl, const float* __restrict__ thetas,
+    const float* __restrict__ betas, int absolute, const float* __restrict__ partials, int nblk,
+    const float* __restrict__ d_tfs, float* __restrict__ d_scale, float* __restrict__ d_transl,
+    float* __restrict__ d_thetas, float* __restrict__ d_betas) {
+  __shared__ double sP[kSmplNP];
+  __shared__ double sJ[MP_NUM_JOINTS][3], sR[MP_NUM_JOINTS][9], sG[MP_NUM_JOINTS][16];
+  __shared__ double sdG[MP_NUM_JOINTS][12], sdJ[MP_NUM_JOINTS][3], sdR[MP_NUM_JOINTS][9];
+  __shared__ double sds[MP_NUM_JOINTS], sdt[MP_NUM_JOINTS][3];
+  const int tid = threadIdx.x;
+  // fixed-order sum of the per-block partials
+  for (int i = tid; i < kSmplNP; i += blockDim.x) {
+    double t = 0.0;
+    for (int q = 0; q < nblk; ++q) t += (double)partials[(size_t)q * kSmplNP + i];
+    sP[i] = t;
+  }
+  // J = J_t + J_s . betas (lbs.py:188) and Rodrigues, recomputed in fp64
+  if (tid < MP_NUM_JOINTS * 3) {
+    double j = m.J_t[tid];
+    for (int l = 0; l < 10; ++l) j += (double)betas[l] * (double)m.J_s[tid * 10 + l];
+    sJ[tid / 3][tid % 3] = j;
+  }
+  if (tid < MP_NUM_JOINTS) {
+    double K[9], ang, a[3], c, s;
+    rodrigues64(thetas + 3 * tid, sR[tid], K, ang, a, c, s);
+  }
+  __syncthreads();
+  // kinematic chain G_i = G_parent T_i (lbs.py:323-370)
+  if (tid == 0) {
+    for (int i = 0; i < MP_NUM_JOINTS; ++i) {
+      double T[16];
+      const int p = m.parents[i];
+      for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) T[4 * r + c] = sR[i][3 * r + c];
+        T[4 * r + 3] = i == 0 ? sJ[0][r] : sJ[i][r] - sJ[p][r];
+      }
+      T[12] = T[13] = T[14] = 0.0;
+      T[15] = 1.0;
+      for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) {
+          if (i == 0) {
+            sG[0][4 * r + c] = T[4 * r + c];
+          } else {
+            double t = 0.0;
+            for (int k = 0; k < 4; ++k) t += sG[p][4 * r + k] * T[4 * k + c];
+            sG[i][4 * r + c] = t;
+          }
+        }
+    }
+  }
+  __syncthreads();
+  if (tid < MP_NUM_JOINTS) {
+    const int j = tid;
+    const double sc = scale_p[0];
+    // dA (rows 0..2) from the vertices and from smpl_tfs = A (absolute) or A @ tfs_c_inv (smpl.py:91); the bottom row of
+    // d_tfs reaches nothing (row 3 of A is constant)
+    double dA[12];
+    for (int k = 0; k < 12; ++k) dA[k] = sP[12 * j + k];
+    if (d_tfs) {
+      const float* dt = d_tfs + 16 * j;
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 4; ++c) {
+          if (absolute) {
+            dA[4 * r + c] += dt[4 * r + c];
+          } else {
+            const float* ci = m.tfs_c_inv + 16 * j;
+            double t = 0.0;
+            for (int k = 0; k < 4; ++k) t += (double)dt[4 * r + k] * (double)ci[4 * c + k];
+            dA[4 * r + c] += t;
+          }
+        }
+    }
+    // A0 = G - pad(G [J;0]) (lbs.py:371-376); A[:3] = s A0[:3] + [0 | t s] (smpl.py:86-88)
+    double A0[12];
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 4; ++c) A0[4 * r + c] = sG[j][4 * r + c];
+      A0[4 * r + 3] -= sG[j][4 * r] * sJ[j][0] + sG[j][4 * r + 1] * sJ[j][1] + sG[j][4 * r + 2] * sJ[j][2];
+    }
+    double ds = 0.0;
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 4; ++c) ds += dA[4 * r + c] * A0[4 * r + c];
+      ds += dA[4 * r + 3] * (double)transl[r];
+      sdt[j][r] = sc * dA[4 * r + 3];
+    }
+    sds[j] = ds;
+    double dJ[3] = {0.0, 0.0, 0.0};
+    for (int r = 0; r < 3; ++r) {
+      const double d3 = sc * dA[4 * r + 3];
+      for (int c = 0; c < 4; ++c) sdG[j][4 * r + c] = sc * dA[4 * r + c];
+      for (int c = 0; c < 3; ++c) {
+        sdG[j][4 * r + c] -= d3 * sJ[j][c];
+        dJ[c] -= d3 * sG[j][4 * r + c];
+      }
+    }
+    for (int c = 0; c < 3; ++c) sdJ[j][c] = dJ[c];
+  }
+  __syncthreads();
+  // the chain in reverse: children (higher indices) first
+  if (tid == 0) {
+    for (int j = MP_NUM_JOINTS - 1; j >= 0; --j) {
+      const double* dG = sdG[j];
+      if (j == 0) {
+        for (int r = 0; r < 3; ++r) {
+          for (int c = 0; c < 3; ++c) sdR[0][3 * r + c] = dG[4 * r + c];
+          sdJ[0][r] += dG[4 * r + 3];
+        }
+        continue;
+      }
+      const int p = m.parents[j];
+      // dT_j = G_p^T dG_j (row 3 of dG_j is 0)
+      for (int a = 0; a < 3; ++a) {
+        for (int b = 0; b < 4; ++b) {
+          double t = 0.0;
+          for (int r = 0; r < 3; ++r) t += sG[p][4 * r + a] * dG[4 * r + b];
+          if (b < 3) {
+            sdR[j][3 * a + b] = t;
+          } else {
+            sdJ[j][a] += t;
+            sdJ[p][a] -= t;
+          }
+        }
+      }
+      // dG_p += dG_j T_j^T
+      for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) {
+          double t = 0.0;
+          for (int k = 0; k < 3; ++k) t += dG[4 * r + k] * sR[j][3 * c + k];
+          t += dG[4 * r + 3] * (sJ[j][c] - sJ[p][c]);
+          sdG[p][4 * r + c] += t;
+        }
+        sdG[p][4 * r + 3] += dG[4 * r + 3];
+      }
+    }
+    double ds = 0.0, dt[3] = {0.0, 0.0, 0.0};
+    for (int j = 0; j < MP_NUM_JOINTS; ++j) {
+      ds += sds[j];
+      for (int r = 0; r < 3; ++r) dt[r] += sdt[j][r];
+    }
+    d_scale[0] = (float)ds;
+    for (int r = 0; r < 3; ++r) d_transl[r] = (float)dt[r];
+  }
+  __syncthreads();
+  if (tid < MP_NUM_JOINTS) {
+    const int j = tid;
+    double dR[9];
+    for (int i = 0; i < 9; ++i) dR[i] = sdR[j][i] + (j >= 1 ? sP[kSmplNA + 9 * (j - 1) + i] : 0.0);  // lbs.py:199
+    double R[9], K[9], ang, a[3], c, s;
+    rodrigues64(thetas + 3 * j, R, K, ang, a, c, s);
+    // R = I + s K + (1 - c) K K
+    double dang = 0.0, dK[9];
+    for (int p = 0; p < 3; ++p)
+      for (int q = 0; q < 3; ++q) {
+        double kk = 0.0, dkk = 0.0;
+        for (int k = 0; k < 3; ++k) {
+          kk += K[3 * p + k] * K[3 * k + q];
+          dkk += dR[3 * p + k] * K[3 * q + k] + K[3 * k + p] * dR[3 * k + q];   // dL/dK of K K: dR K^T + K^T dR
+        }
+        dang += dR[3 * p + q] * (c * K[3 * p + q] + s * kk);
+        dK[3 * p + q] = s * dR[3 * p + q] + (1.0 - c) * dkk;
+      }
+    // K = skew(axis), axis = theta / angle, angle = |theta + 1e-8|
+    const double dd[3] = {dK[7] - dK[5], dK[2] - dK[6], dK[3] - dK[1]};
+    double dth[3];
+    for (int q = 0; q < 3; ++q) {
+      dth[q] = dd[q] / ang;
+      dang -= dd[q] * (double)thetas[3 * j + q] / (ang * ang);
+    }
+    for (int q = 0; q < 3; ++q) d_thetas[3 * j + q] = (float)(dth[q] + dang * a[q] / ang);
+  }
+  if (tid < 10) {
+    double t = sP[kSmplNA + 207 + tid];
+    for (int k = 0; k < MP_NUM_JOINTS * 3; ++k) t += sdJ[k / 3][k % 3] * (double)m.J_s[k * 10 + tid];
+    d_betas[tid] = (float)t;
+  }
+}
+
+static int smpl_backward_blocks(int V) { return div_up(V, kSmplBwdThreads); }
 
 static int smpl_run(const Smpl& m, const float* scale, const float* transl, const float* thetas, const float* betas,
                     int absolute, float* verts, float* tfs, cudaStream_t st) {
@@ -327,5 +616,41 @@ int mp_smpl_forward(mp_smpl_t* h, const float* scale, const float* transl, const
                     int absolute, float* smpl_verts, float* smpl_tfs, void* stream) {
   MP_REQUIRE(h && scale && transl && thetas && betas && smpl_verts && smpl_tfs, "mp_smpl_forward: null argument");
   return mp::smpl_run(h->m, scale, transl, thetas, betas, absolute, smpl_verts, smpl_tfs, (cudaStream_t)stream);
+}
+
+size_t mp_smpl_backward_workspace_bytes(int V) {
+  using namespace mp;
+  return align_up(207 * 4, 256) + 2 * align_up(24 * 16 * 4, 256) +
+         align_up((size_t)smpl_backward_blocks(V > 0 ? V : 0) * kSmplNP * 4, 256) + 256;
+}
+
+int mp_smpl_backward(mp_smpl_t* h, const float* scale, const float* transl, const float* thetas, const float* betas,
+                     int absolute, const float* d_verts, const float* d_tfs, float* d_scale, float* d_transl,
+                     float* d_thetas, float* d_betas, void* workspace, size_t workspace_bytes, void* stream) {
+  using namespace mp;
+  MP_REQUIRE(h && scale && transl && thetas && betas && d_scale && d_transl && d_thetas && d_betas,
+             "mp_smpl_backward: null argument");
+  MP_REQUIRE(workspace && workspace_bytes >= mp_smpl_backward_workspace_bytes(h->m.V),
+             "mp_smpl_backward: workspace too small (%zu < %zu)", workspace_bytes,
+             mp_smpl_backward_workspace_bytes(h->m.V));
+  cudaStream_t st = (cudaStream_t)stream;
+  Smpl m = h->m;   // a copy whose per-call scratch lives in the workspace
+  Arena a(workspace, workspace_bytes);
+  m.pose_feature = a.take<float>(207);
+  m.A_abs = a.take<float>(24 * 16);
+  float* tfs_scratch = a.take<float>(24 * 16);
+  int nblk = d_verts ? smpl_backward_blocks(m.V) : 0;
+  float* partials = a.take<float>((size_t)smpl_backward_blocks(m.V) * kSmplNP);
+  MP_REQUIRE(a.ok, "mp_smpl_backward: workspace overflow");
+  if (nblk) {
+    smpl_pose_kernel<<<1, 1024, 0, st>>>(m, scale, transl, thetas, betas, absolute, tfs_scratch);
+    MP_LAUNCH_CHECK();
+    smpl_skin_backward_kernel<<<nblk, kSmplBwdThreads, 0, st>>>(m, betas, d_verts, partials);
+    MP_LAUNCH_CHECK();
+  }
+  smpl_backward_final_kernel<<<1, 512, 0, st>>>(m, scale, transl, thetas, betas, absolute, partials, nblk, d_tfs, d_scale,
+                                                d_transl, d_thetas, d_betas);
+  MP_LAUNCH_CHECK();
+  return 0;
 }
 }

@@ -199,6 +199,55 @@ class Body:
         L.call("mp_deform_forward_jac", self.handle, xc, N, xd, J)
         return xd, J
 
+    def deform_inverse_backward(self, x, d_xc, exact_far=True, want_x_c=False):
+        """VJP of ``deform_inverse`` at the current pose (mp_deform_inverse_backward): x [N,3], d_xc [N,3] ->
+        (d_x [N,3], d_tfs [24,4,4]) and, with ``want_x_c``, the recomputed canonical points."""
+        x, d = L.dev(x, self.device), L.dev(d_xc, self.device)
+        N = x.shape[0]
+        d_x = torch.empty(N, 3, device=self.device)
+        d_tfs = torch.empty(24, 4, 4, device=self.device)
+        xc = torch.empty(N, 3, device=self.device) if want_x_c else None
+        ws = L.workspace(L.call("mp_deform_backward_workspace_bytes", N), self.device)
+        L.call("mp_deform_inverse_backward", self.handle, x, N, int(exact_far), d, d_tfs, d_x, xc, ws, ws.numel())
+        return (d_x, d_tfs, xc) if want_x_c else (d_x, d_tfs)
+
+    def forward_jac_backward(self, xc, d_xd=None, d_Jinv=None):
+        """VJP of ``forward_jac`` at the current pose (mp_deform_forward_jac_backward): xc [N,3], d_xd [N,3] and
+        d_Jinv [N,9] (None: zero) -> (d_xc [N,3], d_tfs [24,4,4])."""
+        xc = L.dev(xc, self.device)
+        N = xc.shape[0]
+        d_xd = L.dev(d_xd, self.device)
+        d_J = None if d_Jinv is None else L.dev(d_Jinv.reshape(N, 9), self.device)
+        d_xc = torch.empty(N, 3, device=self.device)
+        d_tfs = torch.empty(24, 4, 4, device=self.device)
+        ws = L.workspace(L.call("mp_deform_backward_workspace_bytes", N), self.device)
+        L.call("mp_deform_forward_jac_backward", self.handle, xc, N, d_xd, d_J, d_tfs, d_xc, ws, ws.numel())
+        return d_xc, d_tfs
+
+    def posed_as(self, pose):
+        """Context for a backward: the body posed with ``pose`` = (verts_p, tfs) as a forward saw it, the pose it had
+        before restored afterwards (a later frame may have re-posed it in between)."""
+        return _Posed(self, pose)
+
+
+class _Posed:
+    def __init__(self, body, pose):
+        self.body, self.pose = body, pose
+
+    def __enter__(self):
+        b = self.body
+        self.prev = (b.verts_p, b.tfs)
+        if self.prev[0] is not self.pose[0] or self.prev[1] is not self.pose[1]:
+            b.set_pose(*self.pose)
+        else:
+            self.prev = None
+        return b
+
+    def __exit__(self, *exc):
+        if self.prev is not None:
+            self.body.set_pose(*self.prev)
+        return False
+
 
 class CanonicalMesh:
     """A triangle mesh on the device with its grid of face references (mp_mesh_plan / mp_mesh_create): the canonical
@@ -587,6 +636,78 @@ class RenderComposite(torch.autograd.Function):
                 L.call("mp_bg_composite_backward", b_sdf, b_rgb, R, info["bound"], bg["t_rand"], d_bg, d_bsdf, d_brgb)
                 grads += [d_bsdf, d_brgb]
         return (None, None, d_beta.reshape(ctx.beta_shape)) + tuple(grads)
+
+
+def _grad_like(g, t):
+    """A gradient computed on the device, in the shape, dtype and device of the input ``t`` it belongs to."""
+    return g.reshape(t.shape).to(device=t.device, dtype=t.dtype)
+
+
+class SmplFunction(torch.autograd.Function):
+    """SMPLServer.forward (mp_smpl_forward) as one autograd node: inputs scale [1], transl [3], thetas [72], betas [10]
+    (any shapes with those sizes, on any device), outputs smpl_verts [V,3], smpl_tfs [24,4,4].  ``server`` provides
+    ``_run(s, t, th, b, absolute)`` -> (verts, tfs, device inputs) and ``_backward(inputs, absolute, d_verts, d_tfs)``
+    -> (d_scale, d_transl, d_thetas, d_betas), the latter mp_smpl_backward on the current stream."""
+
+    @staticmethod
+    def forward(ctx, server, absolute, scale, transl, thetas, betas):
+        verts, tfs, dev_inputs = server._run(scale, transl, thetas, betas, absolute)
+        ctx.server, ctx.absolute = server, absolute
+        ctx.inputs = (scale, transl, thetas, betas)
+        ctx.save_for_backward(*dev_inputs)
+        return verts, tfs
+
+    @staticmethod
+    def backward(ctx, d_verts, d_tfs):
+        grads = ctx.server._backward(ctx.saved_tensors, ctx.absolute, d_verts, d_tfs)
+        return (None, None) + tuple(None if g is None else _grad_like(g, t) for g, t in zip(grads, ctx.inputs))
+
+
+class DeformInverse(torch.autograd.Function):
+    """SMPLDeformer.forward(x, smpl_tfs, inverse=True) on a posed ``Body`` (mp_deform_inverse) as an autograd node:
+    inputs x [N,3] and the smpl_tfs [24,4,4] the body is posed with; outputs x_c [N,3] and the outlier mask (not
+    differentiable).  The backward runs mp_deform_inverse_backward on the current stream, at the pose of the forward."""
+
+    @staticmethod
+    def forward(ctx, body, exact_far, x, tfs):
+        xc, outlier = body.deform_inverse(x, exact_far=exact_far)
+        ctx.body, ctx.exact_far, ctx.pose = body, exact_far, (body.verts_p, body.tfs)
+        ctx.inputs = (x, tfs)
+        ctx.save_for_backward(L.dev(x, body.device))
+        ctx.mark_non_differentiable(outlier)
+        return xc, outlier
+
+    @staticmethod
+    def backward(ctx, d_xc, _d_outlier):
+        x_in, tfs_in = ctx.inputs
+        if d_xc is None:
+            return None, None, None, None
+        (x,) = ctx.saved_tensors
+        with ctx.body.posed_as(ctx.pose) as b:
+            d_x, d_tfs = b.deform_inverse_backward(x, d_xc, exact_far=ctx.exact_far)
+        return None, None, _grad_like(d_x, x_in), _grad_like(d_tfs, tfs_in)
+
+
+class ForwardJac(torch.autograd.Function):
+    """SMPLDeformer.forward_skinning and the inverse Jacobian of Multiply.forward_gradient on a posed ``Body``
+    (mp_deform_forward_jac) as one autograd node: inputs x_c [N,3] and the smpl_tfs [24,4,4] the body is posed with;
+    outputs x_d [N,3] and Jinv [N,9].  The backward runs mp_deform_forward_jac_backward on the current stream."""
+
+    @staticmethod
+    def forward(ctx, body, xc, tfs):
+        xd, J = body.forward_jac(xc)
+        ctx.body, ctx.pose = body, (body.verts_p, body.tfs)
+        ctx.inputs = (xc, tfs)
+        ctx.save_for_backward(L.dev(xc, body.device))
+        return xd, J
+
+    @staticmethod
+    def backward(ctx, d_xd, d_J):
+        xc_in, tfs_in = ctx.inputs
+        (xc,) = ctx.saved_tensors
+        with ctx.body.posed_as(ctx.pose) as b:
+            d_xc, d_tfs = b.forward_jac_backward(xc, d_xd, d_J)
+        return None, _grad_like(d_xc, xc_in), _grad_like(d_tfs, tfs_in)
 
 
 def person_samples(persons):

@@ -44,17 +44,39 @@ class SMPLDeformer(torch.nn.Module):
             raise NotImplementedError("only the hot-path call forward(x, tfs, return_weights=False, inverse=True, "
                                       "smpl_verts=posed) is provided (multiply.py:139)")
         b = self.body(x.device)
-        b.set_pose(smpl_verts[0], smpl_tfs[0] if smpl_tfs.ndim == 4 else smpl_tfs)
+        tfs = smpl_tfs[0] if smpl_tfs.ndim == 4 else smpl_tfs
+        b.set_pose(smpl_verts[0], tfs)
+        if torch.is_grad_enabled() and (x.requires_grad or smpl_tfs.requires_grad):
+            # gradients to x and smpl_tfs; none to smpl_verts (the weights are detached, deformer.py:47)
+            return engine.DeformInverse.apply(b, True, x, tfs)
         return b.deform_inverse(x, exact_far=True)
 
+    def _posed_tfs(self, b, smpl_tfs):
+        """The [24,4,4] view of ``smpl_tfs``, which must be the transforms the body is posed with: the gradient goes to
+        exactly that tensor, never to other transforms."""
+        tfs = smpl_tfs.reshape(24, 4, 4)
+        if not torch.equal(b.tfs, tfs.detach().to(device=b.tfs.device, dtype=b.tfs.dtype)):
+            raise ValueError("smpl_tfs differs from the transforms the body is posed with (forward(...) of this frame)")
+        return tfs
+
     def forward_skinning(self, xc, cond, smpl_tfs):
-        """deformer.py:31-35 — returns x_d [1,N,3]; the Jacobian used for normals comes from ``jacobian_inverse``."""
+        """deformer.py:31-35 — returns x_d [1,N,3]; the Jacobian used for normals comes from ``jacobian_inverse``.
+        With grad mode on, gradients go to ``xc`` and ``smpl_tfs`` when either requires grad."""
         b = self.body(xc.device)
         if getattr(b, "tfs", None) is None:
             raise RuntimeError("call forward(...) (which sets the frame's pose) first")
+        if torch.is_grad_enabled() and (xc.requires_grad or torch.is_tensor(smpl_tfs) and smpl_tfs.requires_grad):
+            xd, _ = engine.ForwardJac.apply(b, xc.reshape(-1, 3), self._posed_tfs(b, smpl_tfs))
+            return xd[None]
         xd, _ = b.forward_jac(xc.reshape(-1, 3))
         return xd[None]
 
-    def jacobian_inverse(self, xc):
-        _, J = self.body(xc.device).forward_jac(xc.reshape(-1, 3))
+    def jacobian_inverse(self, xc, smpl_tfs=None):
+        """Inverse Jacobian of forward skinning at xc (multiply.py:625-641) -> [N,3,3].  Given ``smpl_tfs`` (the
+        transforms the body is posed with) and grad mode on, gradients go to it; Jinv is piecewise constant in xc."""
+        b = self.body(xc.device)
+        if smpl_tfs is not None and torch.is_grad_enabled() and smpl_tfs.requires_grad:
+            _, J = engine.ForwardJac.apply(b, xc.reshape(-1, 3), self._posed_tfs(b, smpl_tfs))
+            return J.reshape(-1, 3, 3)
+        _, J = b.forward_jac(xc.reshape(-1, 3))
         return J.reshape(-1, 3, 3)

@@ -132,7 +132,11 @@ class Multiply(nn.Module):
         canonical SMPL vertex and smpl_tfs [24,4,4] (or [1,24,4,4]) -> [1,V,3] (SMPLDeformer.forward_skinning)."""
         b = self.deformer_list[person_id].body(verts.device)
         # forward skinning reads only the canonical vertices; the posed ones keep the body's current frame
-        b.set_pose(getattr(b, "verts_p", b.verts_c), smpl_tfs.reshape(24, 4, 4))
+        tfs = smpl_tfs.reshape(24, 4, 4)
+        b.set_pose(getattr(b, "verts_p", b.verts_c), tfs)
+        if torch.is_grad_enabled() and (smpl_tfs.requires_grad or verts.requires_grad):
+            xd, _ = engine.ForwardJac.apply(b, verts.reshape(-1, 3), tfs)     # differentiable in smpl_tfs (opt_depth)
+            return xd[None]
         xd, _ = b.forward_jac(verts.reshape(-1, 3))
         return xd[None]
 
