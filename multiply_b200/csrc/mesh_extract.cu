@@ -519,9 +519,12 @@ __global__ void cc_union_kernel(const int64_t* __restrict__ faces, int F, int* p
   uf_union(parent, a, c);
 }
 
-__global__ void cc_label_kernel(int* parent, int V) {
+// The labels go to their own array: a concurrent uf_find compresses a path by writing a grandparent it read earlier,
+// which may land on parent[v] after v's own thread stored the root there, leaving v labelled with a non-root ancestor
+// (and dropped from its component).  Compression only ever stores ancestors, so every find still ends at the root.
+__global__ void cc_label_kernel(int* parent, int V, int* __restrict__ label) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v < V) parent[v] = uf_find(parent, v);
+  if (v < V) label[v] = uf_find(parent, v);
 }
 
 __global__ void cc_face_key_kernel(const int64_t* __restrict__ faces, int F, const int* __restrict__ label,
@@ -619,7 +622,7 @@ __global__ void cc_totals_kernel(const int* __restrict__ vflag, const int* __res
 }
 
 struct CcWs {
-  int *parent, *key, *idx, *key_s, *idx_s, *fflag, *frank, *vflag, *vrank, *winner, *totals, *bad;
+  int *parent, *label, *key, *idx, *key_s, *idx_s, *fflag, *frank, *vflag, *vrank, *winner, *totals, *bad;
   double* csum;
   void* cub_tmp;
   size_t cub_bytes;
@@ -642,6 +645,7 @@ static size_t cc_cub_bytes(int V, int F) {
 
 static bool cc_carve(Arena& a, int V, int F, CcWs& w) {
   w.parent = a.take<int>(V);
+  w.label = a.take<int>(V);
   w.key = a.take<int>(F);
   w.idx = a.take<int>(F);
   w.key_s = a.take<int>(F);
@@ -839,9 +843,9 @@ int mp_largest_component(const float* verts, int V, const int64_t* faces, int F,
   MP_LAUNCH_CHECK();
   cc_union_kernel<<<div_up(F, 256), 256, 0, st>>>(faces, F, w.parent);
   MP_LAUNCH_CHECK();
-  cc_label_kernel<<<div_up(V, 256), 256, 0, st>>>(w.parent, V);
+  cc_label_kernel<<<div_up(V, 256), 256, 0, st>>>(w.parent, V, w.label);
   MP_LAUNCH_CHECK();
-  cc_face_key_kernel<<<div_up(F, 256), 256, 0, st>>>(faces, F, w.parent, w.key, w.idx);
+  cc_face_key_kernel<<<div_up(F, 256), 256, 0, st>>>(faces, F, w.label, w.key, w.idx);
   MP_LAUNCH_CHECK();
   size_t cb = w.cub_bytes;
   MP_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, cb, w.key, w.key_s, w.idx, w.idx_s, F, 0, key_bits(V), st));
@@ -849,7 +853,7 @@ int mp_largest_component(const float* verts, int V, const int64_t* faces, int F,
   MP_LAUNCH_CHECK();
   cc_pick_kernel<<<1, 1024, 0, st>>>(w.key_s, w.idx_s, w.csum, F, w.winner);
   MP_LAUNCH_CHECK();
-  cc_flag_kernel<<<div_up(V, 256), 256, 0, st>>>(w.parent, V, w.winner, w.vflag);
+  cc_flag_kernel<<<div_up(V, 256), 256, 0, st>>>(w.label, V, w.winner, w.vflag);
   MP_LAUNCH_CHECK();
   cc_flag_kernel<<<div_up(F, 256), 256, 0, st>>>(w.key, F, w.winner, w.fflag);
   MP_LAUNCH_CHECK();
