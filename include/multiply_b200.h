@@ -15,7 +15,12 @@
  *   - return 0 on success, negative on error; mp_last_error() gives the (thread-local) text.
  *   - fp32 row-major contiguous tensors; B = 1 (the reference indexes [0] everywhere,
  *     multiply.py:208, deformer.py:22-24).
- *   - scratch memory comes from caller-provided workspaces sized by the *_workspace_bytes calls.
+ *   - scratch memory comes from caller-provided workspaces sized by the *_workspace_bytes calls, and persistent
+ *     handles live in caller storage sized by the *_bytes calls (mp_mesh_plan's storage_bytes).  Exactly the query's
+ *     bytes suffice and a call writes none beyond them (mp_field_pack_bytes, which takes no shapes, is an upper
+ *     bound); where a query answers 0 the call also takes a NULL buffer.  Every workspace, storage and scratch base
+ *     (mp_mesh_plan's MP_MESH_PLAN_SCRATCH_BYTES included) must be 256-byte aligned, as every cudaMalloc and torch
+ *     allocation is.  A call refuses a smaller or misaligned buffer before it enqueues anything.
  */
 #ifndef MULTIPLY_B200_H
 #define MULTIPLY_B200_H
@@ -308,6 +313,7 @@ int mp_sample_rays_train(const mp_sampler_cfg_t* cfg, mp_body_t* body, mp_net_t*
 
 /* Multiply.sdf_func_with_smpl_deformer (multiply.py:137-151, eval): x [N,3] -> sdf [N] (4.0 on outliers),
  * x_c [N,3], feat [N,256] (may be NULL). */
+size_t mp_sdf_with_deformer_workspace_bytes(int N);
 int mp_sdf_with_deformer(mp_body_t* body, mp_net_t* field, const float* x, int N,
                          float* sdf, float* x_c, float* feat,
                          void* workspace, size_t workspace_bytes, void* stream);

@@ -157,6 +157,7 @@ SIGNATURES = {
     "mp_sample_rays": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_sample_rays_train": (STATUS, [C.POINTER(SamplerCfg), _VP, _VP, _VP, _VP, _I, C.POINTER(SamplerRng), _VP, _VP, _VP,
                                       _VP, _VP, _SZ, STREAM]),
+    "mp_sdf_with_deformer_workspace_bytes": (_SZ, [_I]),
     "mp_sdf_with_deformer": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_composite_workspace_bytes": (_SZ, [_I, _I]),
     "mp_composite": (STATUS, [C.POINTER(PersonSamples), _I, _I, _I, _F, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),

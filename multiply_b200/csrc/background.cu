@@ -127,37 +127,51 @@ __global__ void bg_composite_backward_kernel(const float* __restrict__ sdf, cons
   d_rgb[3 * i + 2] = wgt * d2;
 }
 
+// 32 samples per ray: points, view directions, colour, SDF, then the MLP's workspace
+struct BgWs {
+  float *pts, *dexp, *rgb, *sdf;
+  void* mlp;
+  size_t mlp_bytes;
+};
+static void bg_carve(Arena& a, int R, BgWs& w) {
+  const int N = R * 32;
+  w.pts = a.take<float>((size_t)N * 4);
+  w.dexp = a.take<float>((size_t)N * 3);
+  w.rgb = a.take<float>((size_t)N * 3);
+  w.sdf = a.take<float>(N);
+  w.mlp_bytes = field_ws_bytes(N);
+  w.mlp = a.take<char>(w.mlp_bytes);
+}
+
 size_t bg_ws_bytes(int R) {
-  size_t N = (size_t)(R > 0 ? R : 1) * 32;
-  return align_up(N * 4 * 4, 256) + align_up(N * 3 * 4, 256) * 2 + align_up(N * 4, 256) + field_ws_bytes((int)N) +
-         4096;
+  Arena a;
+  BgWs w;
+  bg_carve(a, R > 0 ? R : 0, w);
+  return a.off;
 }
 
 int render_background(const Field& f, const float* dirs, const float* cam, int R, float bound, float* bg_rgb,
                       void* ws, size_t ws_bytes, cudaStream_t st, const float* t_rand, float* tap_sdf, float* tap_rgb) {
   if (R <= 0) return 0;
   Arena a(ws, ws_bytes);
-  int N = R * 32;
-  float* pts = a.take<float>((size_t)N * 4);
-  float* dexp = a.take<float>((size_t)N * 3);
-  float* rgb = a.take<float>((size_t)N * 3);
-  float* sdf = a.take<float>(N);
-  size_t mb = field_ws_bytes(N);
-  void* mws = a.take<char>(mb);
-  MP_REQUIRE(a.ok, "background: workspace too small (%zu needed, %zu given)", a.off, ws_bytes);
+  BgWs w;
+  bg_carve(a, R, w);
+  MP_TRY(a.fits("background"));
+  const int N = R * 32;
   float inv_bound = (float)(1.0 / bound);
-  bg_points_kernel<<<div_up(N, 256), 256, 0, st>>>(dirs, cam, R, bound, inv_bound, pts, dexp, t_rand);
+  bg_points_kernel<<<div_up(N, 256), 256, 0, st>>>(dirs, cam, R, bound, inv_bound, w.pts, w.dexp, t_rand);
   MP_LAUNCH_CHECK();
   MlpCall c{};
-  c.x = pts;
+  c.x = w.pts;
   c.cap = N;
-  c.dirs = dexp;
-  c.sdf = sdf;
-  c.rgb = rgb;
-  MP_TRY(field_run(f, c, mws, mb, st));
-  if (tap_sdf) MP_CHECK_CUDA(cudaMemcpyAsync(tap_sdf, sdf, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  if (tap_rgb) MP_CHECK_CUDA(cudaMemcpyAsync(tap_rgb, rgb, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  bg_composite_kernel<<<div_up(N, 256), 256, 0, st>>>(sdf, rgb, R, inv_bound, bg_rgb, t_rand);
+  c.dirs = w.dexp;
+  c.sdf = w.sdf;
+  c.rgb = w.rgb;
+  MP_TRY(field_run(f, c, w.mlp, w.mlp_bytes, st));
+  if (tap_sdf) MP_CHECK_CUDA(cudaMemcpyAsync(tap_sdf, w.sdf, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (tap_rgb)
+    MP_CHECK_CUDA(cudaMemcpyAsync(tap_rgb, w.rgb, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  bg_composite_kernel<<<div_up(N, 256), 256, 0, st>>>(w.sdf, w.rgb, R, inv_bound, bg_rgb, t_rand);
   MP_LAUNCH_CHECK();
   return 0;
 }

@@ -53,17 +53,24 @@ extern std::atomic<long long> g_launches;
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// bump allocator over a caller-provided workspace
+// Bump allocator over a caller-provided workspace or storage.  Each call's buffers come from one carve function: the
+// call's size query runs it on a sizing Arena (no base) and returns `off`, and the call runs it on the caller's buffer
+// and refuses that buffer through fits() before it enqueues anything.  A base is 256-byte aligned (as cudaMalloc and
+// torch allocations are), so every take is.
 struct Arena {
   char* base;
   size_t cap;
   size_t off;
   bool ok;
+  Arena() : Arena(nullptr, 0) {}
   Arena(void* p, size_t n) : base((char*)p), cap(n), off(0), ok(true) {}
+  // A zero-element take always fits and moves nothing, so a layout's size is where its last non-empty take ends and a
+  // call whose layout is empty accepts a null base.
   template <typename T>
   T* take(size_t n) {
-    off = align_up(off, 256);
     size_t bytes = n * sizeof(T);
+    if (bytes == 0) return base ? (T*)(base + off) : nullptr;
+    off = align_up(off, 256);
     if (base == nullptr || off + bytes > cap) {
       ok = false;
       off += bytes;
@@ -73,6 +80,8 @@ struct Arena {
     off += bytes;
     return r;
   }
+  // 0 when the carve fitted an aligned base; else -1 with "<who>: <what> too small (<off> needed, <cap> given)"
+  int fits(const char* who, const char* what = "workspace") const;
 };
 
 int sm_count();

@@ -372,18 +372,33 @@ int launch_row_of_ray(const int64_t* idx, int n_rows, int R, int* row_of_ray, cu
   return 0;
 }
 
-// cp from the caller's person records: each person's row_of_ray map is carved from the arena (`who` names the entry
-// point in the error text) and filled from its hit list on st.
-static int composite_persons(Arena& a, const mp_person_samples_t* persons, int P, int R, const char* who,
+// The backward's per-ray d beta terms, then each person's row_of_ray map.
+struct CompositeWs {
+  float* dbeta_ray;
+  int* row_of_ray[MP_MAX_PERSONS];
+};
+static void composite_carve(Arena& a, int R, int P, bool backward, CompositeWs& w) {
+  w.dbeta_ray = backward ? a.take<float>(R) : nullptr;
+  for (int p = 0; p < P; ++p) w.row_of_ray[p] = a.take<int>(R);
+}
+
+// cp from the caller's person records: each person's row_of_ray map is filled from its hit list on st.
+static int composite_persons(const CompositeWs& w, const mp_person_samples_t* persons, int P, int R,
                              CompositePersons& cp, cudaStream_t st) {
   cp.P = P;
   for (int p = 0; p < P; ++p) {
-    int* ror = a.take<int>(R);
-    MP_REQUIRE(a.ok, "%s: workspace too small", who);
-    MP_TRY(launch_row_of_ray(persons[p].ray_index, persons[p].n_rows, R, ror, st, nullptr));
-    set_person(cp, p, persons[p], ror);
+    MP_TRY(launch_row_of_ray(persons[p].ray_index, persons[p].n_rows, R, w.row_of_ray[p], st, nullptr));
+    set_person(cp, p, persons[p], w.row_of_ray[p]);
   }
   return 0;
+}
+
+static size_t composite_ws_bytes(int R, int P, bool backward) {
+  if (P < 1 || P > MP_MAX_PERSONS) return 0;
+  Arena a;
+  CompositeWs w;
+  composite_carve(a, R > 0 ? R : 0, P, backward, w);
+  return a.off;
 }
 
 int launch_final_compose(const float* fg, const float* bgT, const float* bg, int R, float* rgb, float* fg_out,
@@ -397,22 +412,22 @@ int launch_final_compose(const float* fg, const float* bgT, const float* bg, int
 
 extern "C" {
 
-size_t mp_composite_workspace_bytes(int R, int P) { return (size_t)P * (mp::align_up((size_t)R * 4, 256)) + 4096; }
+size_t mp_composite_workspace_bytes(int R, int P) { return mp::composite_ws_bytes(R, P, false); }
 
 int mp_composite(const mp_person_samples_t* persons, int P, int R, int n, float beta, float* fg_rgb, float* normal,
                  float* acc, float* acc_person, float* bg_T, void* workspace, size_t workspace_bytes, void* stream) {
   MP_REQUIRE(persons && P >= 1 && P <= MP_MAX_PERSONS, "mp_composite: bad person list");
-  MP_REQUIRE(workspace_bytes >= mp_composite_workspace_bytes(R, P), "mp_composite: workspace too small");
   mp::Arena a(workspace, workspace_bytes);
+  mp::CompositeWs w;
+  mp::composite_carve(a, R, P, false, w);
+  MP_TRY(a.fits("mp_composite"));
   mp::CompositePersons cp;
   cudaStream_t st = (cudaStream_t)stream;
-  MP_TRY(mp::composite_persons(a, persons, P, R, "mp_composite", cp, st));
+  MP_TRY(mp::composite_persons(w, persons, P, R, cp, st));
   return mp::launch_composite(cp, R, n, beta, fg_rgb, normal, acc, acc_person, bg_T, st);
 }
 
-size_t mp_composite_backward_workspace_bytes(int R, int P) {
-  return (size_t)(P + 1) * (mp::align_up((size_t)(R > 0 ? R : 1) * 4, 256)) + 4096;
-}
+size_t mp_composite_backward_workspace_bytes(int R, int P) { return mp::composite_ws_bytes(R, P, true); }
 
 int mp_composite_backward(const mp_person_samples_t* persons, int P, int R, int n, float beta, const float* d_fg_rgb,
                           const float* d_normal, const float* d_acc, const float* d_acc_person, const float* d_bg_T,
@@ -426,9 +441,10 @@ int mp_composite_backward(const mp_person_samples_t* persons, int P, int R, int 
                "mp_composite_backward: null argument for person %d", p);
   int wpc;
   MP_REQUIRE(mp::composite_smem(P, n, &wpc) <= 200 * 1024, "mp_composite_backward: P*n too large for shared memory");
-  MP_REQUIRE(workspace_bytes >= mp_composite_backward_workspace_bytes(R, P),
-             "mp_composite_backward: workspace too small");
   mp::Arena a(workspace, workspace_bytes);
+  mp::CompositeWs w;
+  mp::composite_carve(a, R, P, true, w);
+  MP_TRY(a.fits("mp_composite_backward"));
   mp::CompositePersons cp;
   mp::CompositeGrads g;
   g.d_fg = d_fg_rgb;
@@ -437,14 +453,13 @@ int mp_composite_backward(const mp_person_samples_t* persons, int P, int R, int 
   g.d_accp = d_acc_person;
   g.d_bgT = d_bg_T;
   cudaStream_t st = (cudaStream_t)stream;
-  float* dbeta_ray = a.take<float>(R);
-  MP_TRY(mp::composite_persons(a, persons, P, R, "mp_composite_backward", cp, st));
+  MP_TRY(mp::composite_persons(w, persons, P, R, cp, st));
   for (int p = 0; p < P; ++p) {
     g.d_sdf[p] = grads[p].d_sdf;
     g.d_rgb[p] = grads[p].d_rgb;
     g.d_nrm_s[p] = grads[p].d_normal;
   }
-  return mp::launch_composite_backward(cp, g, R, n, beta, dbeta_ray, d_beta, st);
+  return mp::launch_composite_backward(cp, g, R, n, beta, w.dbeta_ray, d_beta, st);
 }
 
 int mp_final_compose_backward(const float* bg_T, const float* bg_rgb, int R, const float* d_rgb_values,

@@ -710,29 +710,42 @@ int launch_forward_jac(const Body& b, const float* x_c, int N, const int* n_dev,
   return 0;
 }
 
+// The body's two vertex grids and per-vertex transforms, in its caller's storage.
+static void body_carve(Arena& a, int V, Body& b) {
+  b.cano_hdr = a.take<GridHeader>(1);
+  b.posed_hdr = a.take<GridHeader>(1);
+  b.cano_cell_start = a.take<int>(kMaxCells + 1);
+  b.posed_cell_start = a.take<int>(kMaxCells + 1);
+  b.cano_sorted = a.take<float4>(V);
+  b.posed_sorted = a.take<float4>(V);
+  b.scratch = a.take<int>(kMaxCells + 8);
+  b.vert_tf = a.take<float4>((size_t)V * 3);
+}
+
+// per-CTA fp64 partials of the bone gradient
+static double* deform_backward_carve(Arena& a, int N) {
+  return a.take<double>((size_t)bone_grad_blocks(N) * kBoneGrad);
+}
+
 }  // namespace mp
 
 extern "C" {
 
 size_t mp_body_bytes(int V) {
-  size_t n = 0;
-  n += mp::align_up(sizeof(mp::GridHeader), 256) * 2;
-  n += mp::align_up((mp::kMaxCells + 1) * sizeof(int), 256) * 2;
-  n += mp::align_up((size_t)V * sizeof(float4), 256) * 2;
-  n += mp::align_up((mp::kMaxCells + 8) * sizeof(int), 256);
-  n += mp::align_up((size_t)V * 3 * sizeof(float4), 256);
-  return n + 1024;
+  mp::Arena a;
+  mp::Body b{};
+  mp::body_carve(a, V > 0 ? V : 0, b);
+  return a.off;
 }
 
 int mp_body_create(const float* verts_cano, const float* weights, int V, float cano_cell, void* storage,
                    size_t storage_bytes, mp_body_t** out, void* stream) {
   MP_REQUIRE(verts_cano && weights && storage && out, "mp_body_create: null argument");
   MP_REQUIRE(V > 0, "mp_body_create: V must be positive");
-  MP_REQUIRE(storage_bytes >= mp_body_bytes(V), "mp_body_create: storage too small (%zu < %zu)", storage_bytes,
-             mp_body_bytes(V));
-  mp_body* h = new mp_body();
   mp::Arena a(storage, storage_bytes);
-  mp::Body& b = h->b;
+  mp::Body b{};
+  mp::body_carve(a, V, b);
+  MP_TRY(a.fits("mp_body_create", "storage"));
   b.V = V;
   b.weights = weights;
   b.verts_cano = verts_cano;
@@ -741,19 +754,8 @@ int mp_body_create(const float* verts_cano, const float* weights, int V, float c
   b.root_steps = 0;
   b.root_thr = 1e-5f;
   b.cano_cell = cano_cell;
-  b.cano_hdr = a.take<mp::GridHeader>(1);
-  b.posed_hdr = a.take<mp::GridHeader>(1);
-  b.cano_cell_start = a.take<int>(mp::kMaxCells + 1);
-  b.posed_cell_start = a.take<int>(mp::kMaxCells + 1);
-  b.cano_sorted = a.take<float4>(V);
-  b.posed_sorted = a.take<float4>(V);
-  b.scratch = a.take<int>(mp::kMaxCells + 8);
-  b.vert_tf = a.take<float4>((size_t)V * 3);
-  if (!a.ok) {
-    delete h;
-    mp::set_error("mp_body_create: arena overflow");
-    return -1;
-  }
+  mp_body* h = new mp_body();
+  h->b = b;
   int r = mp::body_build_grid(verts_cano, V, cano_cell * 0.5f, 2, b.cano_hdr, b.cano_cell_start, b.cano_sorted, b.scratch,
                               (cudaStream_t)stream);
   if (r) {
@@ -821,7 +823,9 @@ int mp_deform_forward_jac(mp_body_t* h, const float* x_c, int N, float* x_d, flo
 }
 
 size_t mp_deform_backward_workspace_bytes(int N) {
-  return mp::align_up((size_t)mp::bone_grad_blocks(N) * mp::kBoneGrad * sizeof(double), 256) + 256;
+  mp::Arena a;
+  mp::deform_backward_carve(a, N);
+  return a.off;
 }
 
 int mp_deform_inverse_backward(mp_body_t* h, const float* x, int N, int exact_far, const float* d_x_c, float* d_tfs,
@@ -830,11 +834,10 @@ int mp_deform_inverse_backward(mp_body_t* h, const float* x, int N, int exact_fa
   MP_REQUIRE(h->b.root_steps == 0,
              "mp_deform_inverse_backward: the body's root finder is on; only the closed-form inverse has a backward");
   MP_REQUIRE(d_tfs && N >= 0 && (N == 0 || (x && d_x_c)), "mp_deform_inverse_backward: null argument");
-  MP_REQUIRE(workspace && workspace_bytes >= mp_deform_backward_workspace_bytes(N),
-             "mp_deform_inverse_backward: workspace too small (%zu < %zu)", workspace_bytes,
-             mp_deform_backward_workspace_bytes(N));
+  mp::Arena a(workspace, workspace_bytes);
+  double* partials = mp::deform_backward_carve(a, N);
+  MP_TRY(a.fits("mp_deform_inverse_backward"));
   cudaStream_t st = (cudaStream_t)stream;
-  double* partials = (double*)mp::align_up((size_t)workspace, 256);
   const int nblk = mp::bone_grad_blocks(N);
   if (nblk) {
     mp::deform_inverse_backward_kernel<<<nblk, mp::kBgThreads, 0, st>>>(h->b, x, N, exact_far, d_x_c, d_x, x_c,
@@ -850,11 +853,10 @@ int mp_deform_forward_jac_backward(mp_body_t* h, const float* x_c, int N, const 
                                    float* d_tfs, float* d_x_c, void* workspace, size_t workspace_bytes, void* stream) {
   MP_REQUIRE(h && h->b.tfs, "mp_deform_forward_jac_backward: body has no pose (call mp_body_set_pose)");
   MP_REQUIRE(d_tfs && N >= 0 && (N == 0 || x_c), "mp_deform_forward_jac_backward: null argument");
-  MP_REQUIRE(workspace && workspace_bytes >= mp_deform_backward_workspace_bytes(N),
-             "mp_deform_forward_jac_backward: workspace too small (%zu < %zu)", workspace_bytes,
-             mp_deform_backward_workspace_bytes(N));
+  mp::Arena a(workspace, workspace_bytes);
+  double* partials = mp::deform_backward_carve(a, N);
+  MP_TRY(a.fits("mp_deform_forward_jac_backward"));
   cudaStream_t st = (cudaStream_t)stream;
-  double* partials = (double*)mp::align_up((size_t)workspace, 256);
   const int nblk = mp::bone_grad_blocks(N);
   if (nblk) {
     mp::deform_forward_jac_backward_kernel<<<nblk, mp::kBgThreads, 0, st>>>(h->b, x_c, N, d_x_d, d_Jinv, d_x_c, partials);

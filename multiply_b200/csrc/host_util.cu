@@ -13,6 +13,12 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int Arena::fits(const char* who, const char* what) const {
+  MP_REQUIRE(((uintptr_t)base & 255) == 0, "%s: %s base %p is not 256-byte aligned", who, what, (void*)base);
+  MP_REQUIRE(ok, "%s: %s too small (%zu needed, %zu given)", who, what, off, cap);
+  return 0;
+}
+
 // SM count of the CURRENT device (cached per device ordinal)
 int sm_count() {
   static std::atomic<int> cache[64];
@@ -29,7 +35,7 @@ int sm_count() {
 
 extern "C" {
 
-int mp_version(void) { return 101; }
+int mp_version(void) { return 102; }
 
 const char* mp_last_error(void) { return mp::g_err; }
 

@@ -479,6 +479,28 @@ int launch_merge_flags(const int64_t* idx, int rows, const int* rows_dev, const 
 
 const Mesh& mesh_of(const mp_mesh_t* h) { return h->m; }
 
+// A mesh as its plan describes it, and the grid's buffers in the caller's storage.
+static Mesh mesh_of_plan(const mp_mesh_plan_t& plan) {
+  Mesh m{};
+  m.V = plan.V;
+  m.F = plan.F;
+  for (int k = 0; k < 3; ++k) {
+    m.g.lo[k] = plan.lo[k];
+    m.g.dim[k] = plan.dim[k];
+  }
+  m.g.h = plan.h;
+  m.g.inv_h = 1.0 / plan.h;
+  m.g.ncell = plan.dim[0] * plan.dim[1] * plan.dim[2];
+  m.n_refs = plan.n_refs;
+  return m;
+}
+static void mesh_carve(Arena& a, Mesh& m) {
+  m.cell_start = a.take<int>((size_t)m.g.ncell + 1);
+  m.cell_cursor = a.take<int>((size_t)m.g.ncell);
+  m.cell_faces = a.take<int>((size_t)m.n_refs);
+  m.tri = a.take<float4>((size_t)m.F * 3);
+}
+
 }  // namespace mp
 
 extern "C" {
@@ -493,7 +515,7 @@ int mp_mesh_plan(const float* verts, int V, const int64_t* faces, int F, float m
   mp::MeshGrid* g = a.take<mp::MeshGrid>(1);
   unsigned long long* total = a.take<unsigned long long>(1);
   int* bad = a.take<int>(1);
-  MP_REQUIRE(a.ok, "mp_mesh_plan: scratch layout exceeds %d bytes", MP_MESH_PLAN_SCRATCH_BYTES);
+  MP_TRY(a.fits("mp_mesh_plan", "scratch"));
   MP_CHECK_CUDA(cudaMemsetAsync(total, 0, sizeof(unsigned long long), st));
   MP_CHECK_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
   mp::mesh_header_kernel<<<1, 1024, 0, st>>>(verts, V, F, margin, g);
@@ -518,38 +540,21 @@ int mp_mesh_plan(const float* verts, int V, const int64_t* faces, int F, float m
   }
   plan->h = hg.h;
   plan->n_refs = (long long)ht;
-  mp::Arena s(nullptr, 0);
-  s.take<int>((size_t)hg.ncell + 1);
-  s.take<int>((size_t)hg.ncell);
-  s.take<int>((size_t)ht);
-  s.take<float4>((size_t)F * 3);
-  plan->storage_bytes = s.off + 1024;
+  mp::Arena s;
+  mp::Mesh m = mp::mesh_of_plan(*plan);
+  mp::mesh_carve(s, m);
+  plan->storage_bytes = s.off;
   return 0;
 }
 
 int mp_mesh_create(const mp_mesh_plan_t* plan, const float* verts, const int64_t* faces, void* storage,
                    size_t storage_bytes, mp_mesh_t** out, void* stream) {
   MP_REQUIRE(plan && verts && faces && storage && out, "mp_mesh_create: null argument");
-  MP_REQUIRE(storage_bytes >= plan->storage_bytes, "mp_mesh_create: storage too small (%zu < %zu)", storage_bytes,
-             plan->storage_bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  mp::Mesh m;
-  m.V = plan->V;
-  m.F = plan->F;
-  for (int k = 0; k < 3; ++k) {
-    m.g.lo[k] = plan->lo[k];
-    m.g.dim[k] = plan->dim[k];
-  }
-  m.g.h = plan->h;
-  m.g.inv_h = 1.0 / plan->h;
-  m.g.ncell = plan->dim[0] * plan->dim[1] * plan->dim[2];
-  m.n_refs = plan->n_refs;
+  mp::Mesh m = mp::mesh_of_plan(*plan);
   mp::Arena a(storage, storage_bytes);
-  m.cell_start = a.take<int>((size_t)m.g.ncell + 1);
-  m.cell_cursor = a.take<int>((size_t)m.g.ncell);
-  m.cell_faces = a.take<int>((size_t)m.n_refs);
-  m.tri = a.take<float4>((size_t)m.F * 3);
-  MP_REQUIRE(a.ok, "mp_mesh_create: storage too small (%zu needed)", a.off);
+  mp::mesh_carve(a, m);
+  MP_TRY(a.fits("mp_mesh_create", "storage"));
   MP_CHECK_CUDA(cudaMemsetAsync(m.cell_cursor, 0, (size_t)m.g.ncell * sizeof(int), st));
   mp::mesh_count_kernel<<<mp::div_up(m.F, 256), 256, 0, st>>>(m.g, verts, faces, m.F, m.cell_cursor, m.tri);
   MP_LAUNCH_CHECK();

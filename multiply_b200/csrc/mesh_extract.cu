@@ -172,7 +172,7 @@ static size_t mise_cub_bytes(int nb) {
   return b;
 }
 
-static bool mise_carve(Arena& a, int res_init, int depth, MiseWs& w) {
+static void mise_carve(Arena& a, int res_init, int depth, MiseWs& w) {
   const long long R = (long long)res_init << depth, n1 = R + 1, n = n1 * n1 * n1;
   const long long Rh = R >> 1, nh = depth > 0 ? Rh * Rh * Rh : 1;
   const int nb = (int)((n + kMiseBlock - 1) / kMiseBlock);
@@ -190,7 +190,6 @@ static bool mise_carve(Arena& a, int res_init, int depth, MiseWs& w) {
   w.cub_tmp = a.take<char>(w.cub_bytes);
   w.mlp_bytes = field_ws_bytes(slab);
   w.mlp = a.take<char>(w.mlp_bytes);
-  return a.ok;
 }
 
 static int grid_stride_blocks(long long n) {
@@ -450,7 +449,7 @@ static size_t mc_cub_bytes(int n) {
   return b;
 }
 
-static bool mc_carve(Arena& a, int R, McWs& w) {
+static void mc_carve(Arena& a, int R, McWs& w) {
   const int nl = (R + 1) * (R + 1), nr = R * R;
   w.vcnt = a.take<long long>(nl);
   w.voff = a.take<long long>(nl);
@@ -459,7 +458,6 @@ static bool mc_carve(Arena& a, int R, McWs& w) {
   w.totals = a.take<long long>(2);
   w.cub_bytes = mc_cub_bytes(nl);
   w.cub_tmp = a.take<char>(w.cub_bytes);
-  return a.ok;
 }
 
 // ---- 3. largest connected component --------------------------------------------------------------------------------
@@ -643,7 +641,7 @@ static size_t cc_cub_bytes(int V, int F) {
   return a > b ? (a > c ? a : c) : (b > c ? b : c);
 }
 
-static bool cc_carve(Arena& a, int V, int F, CcWs& w) {
+static void cc_carve(Arena& a, int V, int F, CcWs& w) {
   w.parent = a.take<int>(V);
   w.label = a.take<int>(V);
   w.key = a.take<int>(F);
@@ -660,7 +658,6 @@ static bool cc_carve(Arena& a, int V, int F, CcWs& w) {
   w.csum = a.take<double>(F);
   w.cub_bytes = cc_cub_bytes(V, F);
   w.cub_tmp = a.take<char>(w.cub_bytes);
-  return a.ok;
 }
 
 }  // namespace mp
@@ -669,10 +666,10 @@ extern "C" {
 
 size_t mp_mise_workspace_bytes(int res_init, int depth) {
   if (res_init < 1 || depth < 0 || depth > 10 || ((long long)res_init << depth) > 1024) return 0;
-  mp::Arena a(nullptr, 0);
+  mp::Arena a;
   mp::MiseWs w;
   mp::mise_carve(a, res_init, depth, w);
-  return a.off + 4096;
+  return a.off;
 }
 
 int mp_mise(mp_net_t* field, const float* center_host, float extent, float pad, int res_init, int depth, double level,
@@ -690,8 +687,8 @@ int mp_mise(mp_net_t* field, const float* center_host, float extent, float pad, 
   const int nb = (int)((n + kMiseBlock - 1) / kMiseBlock);
   Arena a(workspace, workspace_bytes);
   MiseWs w;
-  MP_REQUIRE(mise_carve(a, res_init, depth, w), "mp_mise: workspace too small (%zu needed, %zu given)", a.off,
-             workspace_bytes);
+  mise_carve(a, res_init, depth, w);
+  MP_TRY(a.fits("mp_mise"));
   const int gs = grid_stride_blocks(n);
   mise_init_kernel<<<gs, 256, 0, st>>>(w.state, R, 1 << depth);
   MP_LAUNCH_CHECK();
@@ -747,10 +744,10 @@ int mp_mise(mp_net_t* field, const float* center_host, float extent, float pad, 
 
 size_t mp_marching_cubes_workspace_bytes(int res) {
   if (res < 1 || res > 1024) return 0;
-  mp::Arena a(nullptr, 0);
+  mp::Arena a;
   mp::McWs w;
   mp::mc_carve(a, res, w);
-  return a.off + 4096;
+  return a.off;
 }
 
 int mp_marching_cubes_count(const float* grid, int res, double level, long long* V_host, long long* F_host,
@@ -762,8 +759,8 @@ int mp_marching_cubes_count(const float* grid, int res, double level, long long*
   cudaStream_t st = (cudaStream_t)stream;
   Arena a(workspace, workspace_bytes);
   McWs w;
-  MP_REQUIRE(mc_carve(a, res, w), "mp_marching_cubes_count: workspace too small (%zu needed, %zu given)", a.off,
-             workspace_bytes);
+  mc_carve(a, res, w);
+  MP_TRY(a.fits("mp_marching_cubes_count"));
   const int nl = (res + 1) * (res + 1), nr = res * res;
   mc_line_count_kernel<<<nl, kMcBlock, 0, st>>>(grid, res, level, w.vcnt);
   MP_LAUNCH_CHECK();
@@ -795,8 +792,8 @@ int mp_marching_cubes_emit(const float* grid, int res, double level, const doubl
   cudaStream_t st = (cudaStream_t)stream;
   Arena a(workspace, workspace_bytes);
   McWs w;
-  MP_REQUIRE(mc_carve(a, res, w), "mp_marching_cubes_emit: workspace too small (%zu needed, %zu given)", a.off,
-             workspace_bytes);
+  mc_carve(a, res, w);
+  MP_TRY(a.fits("mp_marching_cubes_emit"));
   const int nl = (res + 1) * (res + 1), nr = res * res;
   if (verts) {
     mc_vert_kernel<<<nl, kMcBlock, 0, st>>>(grid, res, level, w.voff, center_host[0], center_host[1], center_host[2],
@@ -812,10 +809,10 @@ int mp_marching_cubes_emit(const float* grid, int res, double level, const doubl
 
 size_t mp_largest_component_workspace_bytes(int V, int F) {
   if (V < 0 || F < 0) return 0;
-  mp::Arena a(nullptr, 0);
+  mp::Arena a;
   mp::CcWs w;
-  mp::cc_carve(a, V > 0 ? V : 1, F > 0 ? F : 1, w);
-  return a.off + 4096;
+  mp::cc_carve(a, V, F, w);
+  return a.off;
 }
 
 int mp_largest_component(const float* verts, int V, const int64_t* faces, int F, float* verts_out, int64_t* faces_out,
@@ -830,8 +827,8 @@ int mp_largest_component(const float* verts, int V, const int64_t* faces, int F,
   cudaStream_t st = (cudaStream_t)stream;
   Arena a(workspace, workspace_bytes);
   CcWs w;
-  MP_REQUIRE(cc_carve(a, V, F, w), "mp_largest_component: workspace too small (%zu needed, %zu given)", a.off,
-             workspace_bytes);
+  cc_carve(a, V, F, w);
+  MP_TRY(a.fits("mp_largest_component"));
   MP_CHECK_CUDA(cudaMemsetAsync(w.bad, 0, sizeof(int), st));
   cc_check_kernel<<<div_up(3 * F, 256), 256, 0, st>>>(faces, 3ll * F, V, w.bad);
   MP_LAUNCH_CHECK();

@@ -101,6 +101,8 @@ int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, in
   MP_REQUIRE(imp->lin.n_layers == 9, "mp_field_pack: ImplicitNet must have 9 linear layers (got %d)",
              imp->lin.n_layers);
   MP_REQUIRE(imp->skip_layer == 4, "mp_field_pack: skip_in must be [4]");
+  Arena a(storage, storage_bytes);
+  MP_TRY(a.fits("mp_field_pack", "storage"));     // the base's alignment; the layout is checked after its carve below
   cudaStream_t st = (cudaStream_t)stream;
   mp_net* h = new mp_net();
   Field& f = h->f;
@@ -114,7 +116,6 @@ int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, in
   f.n_imp = imp->lin.n_layers;
   f.storage = (char*)storage;
   f.storage_bytes = storage_bytes;
-  Arena a(storage, storage_bytes);
   const int E = f.emb_dim;
   int rc = 0;
   // padded tails of biases / weight tiles must read as zero (0 * garbage could be NaN)

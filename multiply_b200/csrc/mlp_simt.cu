@@ -230,20 +230,16 @@ __global__ void view_embed_kernel(const float* __restrict__ dirs, int L, int N, 
 // ------------------------------------------------------------------------------------------
 // chains
 // ------------------------------------------------------------------------------------------
-size_t simt_workspace_bytes(int N) {
-  // H ping/pong (2 x 256), E (96), 8 x dact (256), colour input (<= 296), feat 256, ge0 96, misc;
-  // the chains process at most 65536 points per pass
-  size_t per = (size_t)(2 * 256 + 96 + 8 * 256 + 296 + 256 + 96 + 16) * sizeof(float);
-  int n = N < 65536 ? N : 65536;
-  if (n < 1) n = 1;
-  return per * (size_t)n + (1 << 16);
-}
+// points per pass of the chains: the backward keeps the 8 dact buffers, so it runs half as many
+constexpr int kSimtChunk = 65536, kSimtChunkBwd = 32768;
 
 struct SimtBufs {
+  int* nrem;
   float *H0, *H1, *E, *dact[8], *cin, *feat, *grad, *ntmp, *ge0;
 };
 
-static bool simt_take(Arena& a, int N, SimtBufs& b, bool need_grad) {
+static void simt_carve(Arena& a, int N, bool need_grad, SimtBufs& b) {
+  b.nrem = a.take<int>(1);
   b.H0 = a.take<float>((size_t)N * 256);
   b.H1 = a.take<float>((size_t)N * 256);
   b.E = a.take<float>((size_t)N * 96);
@@ -253,7 +249,16 @@ static bool simt_take(Arena& a, int N, SimtBufs& b, bool need_grad) {
   b.grad = a.take<float>((size_t)N * 4);
   b.ntmp = a.take<float>((size_t)N * 4);
   b.ge0 = a.take<float>((size_t)N * 96);
-  return a.ok;
+}
+
+// the larger of the two chunk layouts a list of N points can carve
+size_t simt_workspace_bytes(int N) {
+  N = max(N, 0);
+  Arena fwd, bwd;
+  SimtBufs b;
+  simt_carve(fwd, min(N, kSimtChunk), false, b);
+  simt_carve(bwd, min(N, kSimtChunkBwd), true, b);
+  return max(fwd.off, bwd.off);
 }
 
 // forward through layers 0..7 ; leaves h7 in *h7_out (one of H0/H1) ; h3 buffer holds [h3 | E]
@@ -311,14 +316,15 @@ static int simt_colour(const Field& f, const float* cin, int ldc, int n, const i
 int simt_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st) {
   const MlpProg prog = mlp_prog(c);
   const bool bwd = prog == MlpProg::kFull;
-  const int CH = bwd ? 32768 : 65536;
+  const int CH = bwd ? kSimtChunkBwd : kSimtChunk;
   const int E = f.emb_dim;
   for (int s = 0; s < c.cap; s += CH) {
     int n = min(CH, c.cap - s);
     Arena a(ws, ws_bytes);
     SimtBufs b;
-    int* nrem = a.take<int>(1);
-    MP_REQUIRE(simt_take(a, n, b, bwd), "simt_run: workspace too small (%zu needed)", a.off);
+    simt_carve(a, n, bwd, b);
+    MP_TRY(a.fits("simt_run"));
+    int* nrem = b.nrem;
     if (c.count) {
       // remaining count for this chunk = count - s (clamped by the kernels through min(N, *n_dev))
       sub_count_kernel<<<1, 1, 0, st>>>(c.count, s, nrem);
@@ -430,13 +436,12 @@ __global__ void colour_input_kernel(const float* __restrict__ pts, const float* 
 int simt_render(const Field& f, const float* pts, const float* nrm, const float* feat, int N, float* rgb, void* ws,
                 size_t ws_bytes, cudaStream_t st) {
   MP_REQUIRE(f.ren_mode == 0, "mp_render_forward: only the pose_no_view colour net takes (points, normals, feat)");
-  const int CH = 65536;
-  for (int s = 0; s < N; s += CH) {
-    int n = min(CH, N - s);
+  for (int s = 0; s < N; s += kSimtChunk) {
+    int n = min(kSimtChunk, N - s);
     Arena a(ws, ws_bytes);
     SimtBufs b;
-    a.take<int>(1);
-    MP_REQUIRE(simt_take(a, n, b, false), "simt_render: workspace too small (%zu needed)", a.off);
+    simt_carve(a, n, false, b);
+    MP_TRY(a.fits("simt_render"));
     const int ldc = 6 + 256;
     colour_input_kernel<<<div_up(n * ldc, 256), 256, 0, st>>>(pts + 3 * (size_t)s, nrm + 3 * (size_t)s,
                                                              feat + 256 * (size_t)s, n, b.cin, ldc);

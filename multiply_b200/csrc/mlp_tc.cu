@@ -1073,7 +1073,15 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-size_t tc_workspace_bytes(int N) { return (size_t)sm_count() * kScratchPerCta + 4096; }
+// One scratch slice per persistent CTA; a launch runs at most one CTA per SM and per 128-point tile.
+static int tc_max_grid(int cap) { return max(0, min(sm_count(), div_up(cap, 128))); }
+static char* tc_carve(Arena& a, int grid) { return a.take<char>((size_t)grid * kScratchPerCta); }
+
+size_t tc_workspace_bytes(int N) {
+  Arena a;
+  tc_carve(a, tc_max_grid(N));
+  return a.off;
+}
 
 // optional per-launch timing of the tensor-core kernel (bench.py roofline): CUDA events on the
 // launching stream + an async copy of the device-side point count into pinned memory
@@ -1156,7 +1164,7 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     for (int s = 0; s < P.nsteps; ++s)
       P.step[s].terms = (mode == 2 || (mode == 1 && P.step[s].kind == K_RELU)) ? 1 : 3;
   }
-  int grid = sm_count();
+  int grid = tc_max_grid(io.cap);
   {
     static int grid_override = -1;
     if (grid_override < 0) {
@@ -1165,12 +1173,10 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     }
     if (grid_override > 0 && grid_override < grid) grid = grid_override;
   }
-  int maxtiles = (io.cap + 127) / 128;
-  if (grid > maxtiles) grid = maxtiles;
   if (grid < 1) return 0;
-  MP_REQUIRE(ws && ws_bytes >= (size_t)grid * kScratchPerCta, "tensor-core engine: workspace too small (%zu < %zu)",
-             ws_bytes, (size_t)grid * kScratchPerCta);
-  io.scratch = (char*)ws;
+  Arena a(ws, ws_bytes);
+  io.scratch = tc_carve(a, grid);
+  MP_TRY(a.fits("tensor-core engine"));
   io.scratch_per_cta = kScratchPerCta;
   static const float rz_scale = [] {
     const char* er = getenv("MP_TC_RZ_SCALE");      // experiment knob: multiplies kRzPerMma (0 switches it off)

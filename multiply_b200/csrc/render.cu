@@ -119,7 +119,7 @@ struct RenderWs {
   size_t sub_bytes;
 };
 
-static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
+static void render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
   const mp_sampler_cfg_t& c = sc.sampler;
   int n = samples_per_ray(c);
   w.dirs = a.take<float>((size_t)R * 3);
@@ -154,7 +154,33 @@ static bool render_carve(Arena& a, const mp_scene_t& sc, int R, RenderWs& w) {
   }
   w.sub_bytes = sub;
   for (int i = 0; i <= sc.P; ++i) w.sub[i] = a.take<char>(sub);     // [P] = background branch
-  return a.ok;
+}
+
+// the outliers of mp_deform_inverse, then the MLP's workspace
+struct SdfDeformWs {
+  uint8_t* outl;
+  void* mlp;
+  size_t mlp_bytes;
+};
+static void sdf_deform_carve(Arena& a, int N, SdfDeformWs& w) {
+  w.outl = a.take<uint8_t>(N);
+  w.mlp_bytes = field_ws_bytes(N);
+  w.mlp = a.take<char>(w.mlp_bytes);
+}
+
+// the lattice is evaluated in slabs of at most 2^20 points
+struct SdfGridWs {
+  int chunk;
+  float* pts;
+  void* mlp;
+  size_t mlp_bytes;
+};
+static void sdf_grid_carve(Arena& a, int res, SdfGridWs& w) {
+  const long long n = (long long)(res + 1) * (res + 1) * (res + 1);
+  w.chunk = (int)(n < (1 << 20) ? n : (1 << 20));
+  w.pts = a.take<float>((size_t)w.chunk * 3);
+  w.mlp_bytes = field_ws_bytes(w.chunk);
+  w.mlp = a.take<char>(w.mlp_bytes);
 }
 
 }  // namespace mp
@@ -186,7 +212,7 @@ int mp_profile_read(double* ms_host, long long* launches_host, double* points_ho
   return mp::prof_read(ms_host, launches_host, points_host, reset);
 }
 
-size_t mp_mlp_workspace_bytes(int N) { return mp::field_ws_bytes(N) + (size_t)N * (9 + 1) * sizeof(float) + 4096; }
+size_t mp_mlp_workspace_bytes(int N) { return mp::field_ws_bytes(N); }
 
 int mp_implicit_forward(mp_net_t* f, const float* x, int N, float* sdf, float* feat, void* workspace,
                         size_t workspace_bytes, void* stream) {
@@ -237,9 +263,11 @@ int mp_bg_nets_forward(mp_net_t* bg_field, const float* pts, const float* view_d
 }
 
 size_t mp_sdf_grid_workspace_bytes(int res) {
-  long long n = (long long)(res + 1) * (res + 1) * (res + 1);
-  int chunk = (int)(n < (1 << 20) ? n : (1 << 20));
-  return mp::field_ws_bytes(chunk) + (size_t)chunk * 3 * sizeof(float) + 4096;
+  if (res < 1 || res > 1024) return 0;
+  mp::Arena a;
+  mp::SdfGridWs w;
+  mp::sdf_grid_carve(a, res, w);
+  return a.off;
 }
 
 int mp_sdf_grid(mp_net_t* field, const float* center_host, float extent, float pad, int res, float* values,
@@ -249,24 +277,30 @@ int mp_sdf_grid(mp_net_t* field, const float* center_host, float extent, float p
   MP_REQUIRE(!field->f.is_bg, "mp_sdf_grid: a foreground field is required");
   cudaStream_t st = (cudaStream_t)stream;
   const long long n = (long long)(res + 1) * (res + 1) * (res + 1);
-  const int chunk = (int)(n < (1 << 20) ? n : (1 << 20));
   mp::Arena a(workspace, workspace_bytes);
-  float* pts = a.take<float>((size_t)chunk * 3);
-  const size_t mb = mp::field_ws_bytes(chunk);
-  void* mws = a.take<char>(mb);
-  MP_REQUIRE(a.ok, "mp_sdf_grid: workspace too small (%zu needed)", a.off);
+  mp::SdfGridWs w;
+  mp::sdf_grid_carve(a, res, w);
+  MP_TRY(a.fits("mp_sdf_grid"));
+  const int chunk = w.chunk;
   for (long long s0 = 0; s0 < n; s0 += chunk) {
     const int cnt = (int)((n - s0) < chunk ? (n - s0) : chunk);
     mp::grid_points_kernel<<<mp::div_up(cnt, 256), 256, 0, st>>>(center_host[0], center_host[1], center_host[2], extent,
-                                                                  pad, res, s0, cnt, pts);
+                                                                  pad, res, s0, cnt, w.pts);
     MP_LAUNCH_CHECK();
     mp::MlpCall c{};
-    c.x = pts;
+    c.x = w.pts;
     c.cap = cnt;
     c.sdf = values + s0;
-    MP_TRY(mp::field_run(field->f, c, mws, mb, st));
+    MP_TRY(mp::field_run(field->f, c, w.mlp, w.mlp_bytes, st));
   }
   return 0;
+}
+
+size_t mp_sdf_with_deformer_workspace_bytes(int N) {
+  mp::Arena a;
+  mp::SdfDeformWs w;
+  mp::sdf_deform_carve(a, N > 0 ? N : 0, w);
+  return a.off;
 }
 
 int mp_sdf_with_deformer(mp_body_t* body, mp_net_t* field, const float* x, int N, float* sdf, float* x_c,
@@ -275,28 +309,27 @@ int mp_sdf_with_deformer(mp_body_t* body, mp_net_t* field, const float* x, int N
   if (N <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   mp::Arena a(workspace, workspace_bytes);
-  uint8_t* outl = a.take<uint8_t>(N);
-  size_t mb = mp::field_ws_bytes(N);
-  void* mws = a.take<char>(mb);
-  MP_REQUIRE(a.ok, "mp_sdf_with_deformer: workspace too small (%zu needed)", a.off);
-  MP_TRY(mp_deform_inverse(body, x, N, x_c, outl, 1, stream));
+  mp::SdfDeformWs w;
+  mp::sdf_deform_carve(a, N, w);
+  MP_TRY(a.fits("mp_sdf_with_deformer"));
+  MP_TRY(mp_deform_inverse(body, x, N, x_c, w.outl, 1, stream));
   mp::MlpCall c{};
   c.x = x_c;
   c.cap = N;
   c.sdf = sdf;
   c.feat = feat;
-  MP_TRY(mp::field_run(field->f, c, mws, mb, st));
-  mp::force_outlier_sdf_kernel<<<mp::div_up(N, 256), 256, 0, st>>>(outl, N, sdf);
+  MP_TRY(mp::field_run(field->f, c, w.mlp, w.mlp_bytes, st));
+  mp::force_outlier_sdf_kernel<<<mp::div_up(N, 256), 256, 0, st>>>(w.outl, N, sdf);
   MP_LAUNCH_CHECK();
   return 0;
 }
 
 size_t mp_render_workspace_bytes(const mp_scene_t* scene, int R) {
-  if (!scene) return 0;
-  mp::Arena a(nullptr, 0);
+  if (!scene || scene->P < 1 || scene->P > MP_MAX_PERSONS) return 0;
+  mp::Arena a;
   mp::RenderWs w;
   mp::render_carve(a, *scene, R, w);
-  return a.off + 8192;
+  return a.off;
 }
 
 namespace mp {
@@ -388,8 +421,8 @@ int mp_render_rays(const mp_scene_t* scene, const float* uv, const float* pose, 
   const int prune = prune_is_exact(beta) ? 1 : 0;
   Arena a(workspace, workspace_bytes);
   RenderWs w;
-  MP_REQUIRE(render_carve(a, *scene, R, w), "mp_render_rays: workspace too small (%zu needed, %zu given)", a.off,
-             workspace_bytes);
+  render_carve(a, *scene, R, w);
+  MP_TRY(a.fits("mp_render_rays"));
   MP_TRY(mp_camera_rays(uv, pose, intrinsics, R, w.dirs, w.cam, stream));     // multiply.py:223-227
   if (out->status) {
     MP_CHECK_CUDA(cudaMemsetAsync(out->status, 0, sizeof(int), caller));

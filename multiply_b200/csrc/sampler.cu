@@ -410,7 +410,7 @@ struct SamplerWs {
   size_t mlp_ws_bytes;
 };
 
-static bool sampler_carve(Arena& a, const mp_sampler_cfg_t& c, int R, SamplerWs& w) {
+static void sampler_carve(Arena& a, const mp_sampler_cfg_t& c, int R, SamplerWs& w) {
   int E = c.N_samples_eval, S = c.N_samples, X = c.N_samples_extra;
   size_t zcap = (size_t)c.max_total_iters * E;
   w.zA = a.take<float>((size_t)R * zcap);
@@ -429,7 +429,6 @@ static bool sampler_carve(Arena& a, const mp_sampler_cfg_t& c, int R, SamplerWs&
   w.tab.z_bg = a.take<float>(32);
   w.mlp_ws_bytes = field_ws_bytes(R * E);
   w.mlp_ws = a.take<char>(w.mlp_ws_bytes);
-  return a.ok;
 }
 
 // The whole Algorithm-1 loop for one person.  z_final [R, S+X+2].
@@ -450,7 +449,8 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
   if (R <= 0) return 0;
   Arena a(ws, ws_bytes);
   SamplerWs w;
-  MP_REQUIRE(sampler_carve(a, c, R, w), "sampler: workspace too small (%zu needed, %zu given)", a.off, ws_bytes);
+  sampler_carve(a, c, R, w);
+  MP_TRY(a.fits("sampler"));
   const int zcap = c.max_total_iters * E;
   const float beta0 = sampler_beta(c);
   const float bound_coef = 1.0f / (4.0f * logf((float)(c.eps + 1.0)));     // ray_sampler.py:75
@@ -518,10 +518,10 @@ int sample_rays(const mp_sampler_cfg_t& c, const Body& body, const Field& field,
 }
 
 size_t sampler_ws_bytes(const mp_sampler_cfg_t& c, int R) {
-  Arena a(nullptr, 0);
+  Arena a;
   SamplerWs w;
-  sampler_carve(a, c, R > 0 ? R : 1, w);
-  return a.off + 4096;
+  sampler_carve(a, c, R > 0 ? R : 0, w);
+  return a.off;
 }
 
 }  // namespace mp

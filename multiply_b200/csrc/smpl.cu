@@ -525,6 +525,30 @@ static int smpl_run(const Smpl& m, const float* scale, const float* transl, cons
   return 0;
 }
 
+// The model's per-handle buffers, in its caller's storage; `canon` holds the canonical pose's 86 parameters.
+static void smpl_carve(Arena& a, int V, Smpl& m, float*& canon) {
+  m.v_shaped = a.take<float>((size_t)V * 3);
+  m.verts_c = a.take<float>((size_t)V * 3);
+  m.pose_feature = a.take<float>(207);
+  m.A_abs = a.take<float>(24 * 16);
+  m.tfs_c_inv = a.take<float>(24 * 16);
+  m.tmp_tfs = a.take<float>(24 * 16);
+  m.J_t = a.take<float>(24 * 3);
+  m.J_s = a.take<float>(24 * 3 * 10);
+  canon = a.take<float>(86);
+}
+
+// The backward's per-call scratch: its own pose features, absolute and posed transforms, and per-CTA partials.
+struct SmplBackwardWs {
+  float *pose_feature, *A_abs, *tfs, *partials;
+};
+static void smpl_backward_carve(Arena& a, int V, SmplBackwardWs& w) {
+  w.pose_feature = a.take<float>(207);
+  w.A_abs = a.take<float>(24 * 16);
+  w.tfs = a.take<float>(24 * 16);
+  w.partials = a.take<float>((size_t)smpl_backward_blocks(V) * kSmplNP);
+}
+
 }  // namespace mp
 
 struct mp_smpl {
@@ -534,8 +558,11 @@ struct mp_smpl {
 extern "C" {
 
 size_t mp_smpl_bytes(int V) {
-  return mp::align_up((size_t)V * 3 * 4, 256) * 2 + 256 * 8 + mp::align_up(207 * 4, 256) + 3 * mp::align_up(24 * 16 * 4, 256) +
-         mp::align_up(86 * 4, 256) + mp::align_up(24 * 3 * 4, 256) + mp::align_up(24 * 3 * 10 * 4, 256) + 4096;
+  mp::Arena a;
+  mp::Smpl m{};
+  float* canon;
+  mp::smpl_carve(a, V > 0 ? V : 0, m, canon);
+  return a.off;
 }
 
 int mp_smpl_create(const float* v_template, const float* shapedirs, const float* posedirs, const float* J_regressor,
@@ -544,10 +571,12 @@ int mp_smpl_create(const float* v_template, const float* shapedirs, const float*
   using namespace mp;
   MP_REQUIRE(v_template && shapedirs && posedirs && J_regressor && parents_host && lbs_weights && storage && out,
              "mp_smpl_create: null argument");
-  MP_REQUIRE(storage_bytes >= mp_smpl_bytes(V), "mp_smpl_create: storage too small");
+  Arena a(storage, storage_bytes);
+  Smpl m{};
+  float* canon;
+  smpl_carve(a, V, m, canon);
+  MP_TRY(a.fits("mp_smpl_create", "storage"));
   cudaStream_t st = (cudaStream_t)stream;
-  mp_smpl* h = new mp_smpl();
-  Smpl& m = h->m;
   m.V = V;
   m.v_template = v_template;
   m.shapedirs = shapedirs;
@@ -555,21 +584,8 @@ int mp_smpl_create(const float* v_template, const float* shapedirs, const float*
   m.J_regressor = J_regressor;
   m.lbs_weights = lbs_weights;
   for (int i = 0; i < MP_NUM_JOINTS; ++i) m.parents[i] = parents_host[i];
-  Arena a(storage, storage_bytes);
-  m.v_shaped = a.take<float>((size_t)V * 3);
-  m.verts_c = a.take<float>((size_t)V * 3);
-  m.pose_feature = a.take<float>(207);
-  m.A_abs = a.take<float>(24 * 16);
-  m.tfs_c_inv = a.take<float>(24 * 16);
-  m.tmp_tfs = a.take<float>(24 * 16);
-  m.J_t = a.take<float>(24 * 3);
-  m.J_s = a.take<float>(24 * 3 * 10);
-  float* canon = a.take<float>(86);
-  if (!a.ok) {
-    delete h;
-    set_error("mp_smpl_create: arena overflow");
-    return -1;
-  }
+  mp_smpl* h = new mp_smpl();
+  h->m = m;
   // canonical pose (smpl.py:35-47): scale 1, no translation, hips +-pi/6 about z, the person's betas; absolute
   // transforms, inverted once
   float host[86];
@@ -619,9 +635,10 @@ int mp_smpl_forward(mp_smpl_t* h, const float* scale, const float* transl, const
 }
 
 size_t mp_smpl_backward_workspace_bytes(int V) {
-  using namespace mp;
-  return align_up(207 * 4, 256) + 2 * align_up(24 * 16 * 4, 256) +
-         align_up((size_t)smpl_backward_blocks(V > 0 ? V : 0) * kSmplNP * 4, 256) + 256;
+  mp::Arena a;
+  mp::SmplBackwardWs w;
+  mp::smpl_backward_carve(a, V > 0 ? V : 0, w);
+  return a.off;
 }
 
 int mp_smpl_backward(mp_smpl_t* h, const float* scale, const float* transl, const float* thetas, const float* betas,
@@ -630,18 +647,17 @@ int mp_smpl_backward(mp_smpl_t* h, const float* scale, const float* transl, cons
   using namespace mp;
   MP_REQUIRE(h && scale && transl && thetas && betas && d_scale && d_transl && d_thetas && d_betas,
              "mp_smpl_backward: null argument");
-  MP_REQUIRE(workspace && workspace_bytes >= mp_smpl_backward_workspace_bytes(h->m.V),
-             "mp_smpl_backward: workspace too small (%zu < %zu)", workspace_bytes,
-             mp_smpl_backward_workspace_bytes(h->m.V));
+  Arena a(workspace, workspace_bytes);
+  SmplBackwardWs w;
+  smpl_backward_carve(a, h->m.V, w);
+  MP_TRY(a.fits("mp_smpl_backward"));
   cudaStream_t st = (cudaStream_t)stream;
   Smpl m = h->m;   // a copy whose per-call scratch lives in the workspace
-  Arena a(workspace, workspace_bytes);
-  m.pose_feature = a.take<float>(207);
-  m.A_abs = a.take<float>(24 * 16);
-  float* tfs_scratch = a.take<float>(24 * 16);
+  m.pose_feature = w.pose_feature;
+  m.A_abs = w.A_abs;
+  float* tfs_scratch = w.tfs;
+  float* partials = w.partials;
   int nblk = d_verts ? smpl_backward_blocks(m.V) : 0;
-  float* partials = a.take<float>((size_t)smpl_backward_blocks(m.V) * kSmplNP);
-  MP_REQUIRE(a.ok, "mp_smpl_backward: workspace overflow");
   if (nblk) {
     smpl_pose_kernel<<<1, 1024, 0, st>>>(m, scale, transl, thetas, betas, absolute, tfs_scratch);
     MP_LAUNCH_CHECK();

@@ -54,3 +54,26 @@ def test_table_states_the_headers_status_and_stream_conventions():
         assert len(params) == (0 if plist.strip() == "void" else plist.count(",") + 1), name
     for name in ("mp_last_error", "mp_launch_count", "mp_field_pack_bytes", "mp_render_workspace_bytes") + tuple(INT_VALUES):
         assert L.SIGNATURES[name][0] not in (L.STATUS, None), name
+
+
+def test_size_queries_are_host_calls():
+    """Every workspace and storage query answers on the host: no launch, no device needed (on a machine without a GPU
+    the SM count is taken as 132), and a query of a larger problem never asks for less."""
+    n0 = L.call("mp_launch_count", 0)
+    c = L.SamplerCfg(3.0, 0.0, 64, 128, 32, 0.1, 10, 5, 1e-6, 0.1, 1e-4)
+    for name, small, large in (("mp_mlp_workspace_bytes", (1,), (32769,)),
+                               ("mp_sdf_with_deformer_workspace_bytes", (1,), (129,)),
+                               ("mp_sdf_grid_workspace_bytes", (8,), (101,)),
+                               ("mp_background_workspace_bytes", (1,), (301,)),
+                               ("mp_sampler_workspace_bytes", (c, 1), (c, 129)),
+                               ("mp_composite_workspace_bytes", (1, 1), (300, 3)),
+                               ("mp_composite_backward_workspace_bytes", (1, 1), (300, 3)),
+                               ("mp_deform_backward_workspace_bytes", (1,), (4097,)),
+                               ("mp_smpl_backward_workspace_bytes", (300,), (6890,)),
+                               ("mp_body_bytes", (3,), (6890,)),
+                               ("mp_smpl_bytes", (300,), (6890,)),
+                               ("mp_mise_workspace_bytes", (4, 1), (16, 2)),
+                               ("mp_marching_cubes_workspace_bytes", (8,), (64,)),
+                               ("mp_largest_component_workspace_bytes", (3, 1), (1000, 2000))):
+        assert 0 < L.call(name, *small) <= L.call(name, *large), name
+    assert L.call("mp_launch_count", 0) == n0

@@ -176,7 +176,7 @@ def gpu_callback(body, field, verts_p):
         xg = x.cuda()
         sdf = torch.empty(N, device="cuda")
         xc = torch.empty(N, 3, device="cuda")
-        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N) + N + 4096, "cuda")
+        ws = L.workspace(L.call("mp_sdf_with_deformer_workspace_bytes", N), "cuda")
         L.call("mp_sdf_with_deformer", body.handle, field.handle, xg, N, sdf, xc, None, ws, ws.numel())
         d2, _, _ = port.knn_points(x.double()[None], v64[None], return_nn=False)
         dist.append(d2[0, :, 0].sqrt().reshape(z.shape))
