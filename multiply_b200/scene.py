@@ -707,13 +707,52 @@ def smpl_scene_networks(P, S, seed):
     return nets, rest
 
 
+def model_opt(cfg):
+    """The mirror ``Multiply``'s options: MODEL_OPT with the ray sampler of the scene config ``cfg``."""
+    return dict(MODEL_OPT, ray_sampler=dict({k: v for k, v in cfg.items()
+                                             if k in ("near", "N_samples", "N_samples_eval", "N_samples_extra", "eps",
+                                                      "beta_iters", "max_total_iters", "add_tiny")},
+                                            N_samples_inverse_sphere=32))
+
+
+def mirror_state_dict(scene, frame_index=3):
+    """The mirror ``Multiply``'s state dict for a make_scene-style dict: every person's foreground nets, the background
+    nets, density.beta, and the frame latent, whose row ``frame_index`` holds the scene's frame code."""
+    sd = {}
+    for p, person in enumerate(scene["persons"]):
+        for k, v in person["implicit"].items():
+            sd[f"foreground_implicit_network_list.{p}.{k}"] = v
+        for k, v in person["render"].items():
+            sd[f"foreground_rendering_network_list.{p}.{k}"] = v
+    for k, v in scene["bg_implicit"].items():
+        sd["bg_implicit_network." + k] = v
+    for k, v in scene["bg_render"].items():
+        sd["bg_rendering_network." + k] = v
+    sd["density.beta"] = torch.tensor(scene["beta_param"])
+    fw = torch.zeros(75, 32)
+    fw[frame_index] = scene["frame_code"][0]
+    sd["frame_latent_encoder.weight"] = fw
+    return sd
+
+
+def mirror_model(scene, servers=None, culling="aabb", device="cuda", frame_index=3):
+    """The mirror ``Multiply`` (eval, on ``device``) holding the weights of a make_scene-style dict; its SMPL servers
+    are ``servers``, by default one SyntheticSMPLServer per person."""
+    from .model.multiply import Multiply
+    P = len(scene["persons"])
+    if servers is None:
+        servers = [SyntheticSMPLServer(p, P) for p in range(P)]
+    model = Multiply(model_opt(scene["cfg"]), smpl_server_list=servers, culling=culling)
+    model.load_state_dict(mirror_state_dict(scene, frame_index), strict=True)
+    return model.to(device).eval()
+
+
 def make_smpl_scene(P=2, S=64, seed=42, device="cuda", frame_index=3, pose_std=0.2, scale=0.5):
     """Returns (scene, model, smpl_inputs): `scene` is a make_scene-style dict (CPU tensors) whose persons are the
     outputs of the device SMPL servers for `smpl_inputs` (smpl_params / smpl_pose / smpl_shape / smpl_trans / idx, the
     reference's input-dict entries, SURVEY.md 8b); `model` is the mirror ``Multiply`` (eval, on `device`) holding the
     same weights and servers."""
     from .model.smpl import SMPLServer
-    from .model.multiply import Multiply
     servers = [SMPLServer(model=make_smpl_model(300 + p, body_seed=100 + p), device=device) for p in range(P)]
     for p, srv in enumerate(servers):          # canonical mesh of the capsules (SyntheticSMPLServer)
         srv.mesh_verts_c, srv.faces = make_body_mesh(100 + p)
@@ -730,24 +769,5 @@ def make_smpl_scene(P=2, S=64, seed=42, device="cuda", frame_index=3, pose_std=0
                             smpl_pose=smpl_pose[:, p].clone(), cond=smpl_pose[:, p, 3:] / math.pi, scale=scale,
                             implicit=nets[p]["implicit"], render=nets[p]["render"]))
     scene = dict(rest, persons=persons)
-    opt = dict(MODEL_OPT, ray_sampler=dict({k: v for k, v in scene["cfg"].items()
-                                            if k in ("near", "N_samples", "N_samples_eval", "N_samples_extra", "eps",
-                                                     "beta_iters", "max_total_iters", "add_tiny")},
-                                           N_samples_inverse_sphere=32))
-    model = Multiply(opt, smpl_server_list=servers)
-    sd = {}
-    for p, person in enumerate(persons):
-        for k, v in person["implicit"].items():
-            sd[f"foreground_implicit_network_list.{p}.{k}"] = v
-        for k, v in person["render"].items():
-            sd[f"foreground_rendering_network_list.{p}.{k}"] = v
-    for k, v in scene["bg_implicit"].items():
-        sd["bg_implicit_network." + k] = v
-    for k, v in scene["bg_render"].items():
-        sd["bg_rendering_network." + k] = v
-    sd["density.beta"] = torch.tensor(scene["beta_param"])
-    fw = torch.zeros(75, 32)
-    fw[frame_index] = scene["frame_code"][0]
-    sd["frame_latent_encoder.weight"] = fw
-    model.load_state_dict(sd, strict=True)
-    return scene, model.to(device).eval(), smpl_inputs
+    model = mirror_model(scene, servers, device=device, frame_index=frame_index)
+    return scene, model, smpl_inputs

@@ -19,7 +19,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from multiply_b200 import engine, scene as S          # noqa: E402
 from multiply_b200.utils import mesh as umesh         # noqa: E402
@@ -48,10 +47,9 @@ def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                        text=True)
     print("card: %s" % q.stdout.strip())
-    from test_gpu_mirror import _build
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42, weights="trained")
-    m = _build(sc)
+    m = S.mirror_model(sc)
     mod = None if a.no_reference else build_ref.load_mise()
     for pid, person in enumerate(sc["persons"]):
         cond = person["cond"].cuda()

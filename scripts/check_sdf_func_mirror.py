@@ -4,8 +4,6 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from multiply_b200 import scene as S
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
-from test_gpu_mirror import _build, OPT
 
 
 def check_sdf_func_with_smpl_deformer_mirror():
@@ -14,7 +12,7 @@ def check_sdf_func_with_smpl_deformer_mirror():
     from oracle import port
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42)
-    m = _build(sc)
+    m = S.mirror_model(sc)
     p1 = sc["persons"][1]
     g = torch.Generator().manual_seed(3)
     pts = torch.cat([p1["verts_p"][:300] + 0.02 * torch.randn(300, 3, generator=g),       # near the body

@@ -1,4 +1,5 @@
-"""Sentinel-padded device buffers for the GPU tests that call the C ABI through ``_lib.call``.
+"""Sentinel-padded device buffers for the GPU tests that call the C ABI through ``_lib.call``, and bitwise comparison of
+their outputs.
 
 An output buffer holds the elements a call may write plus a tail prefilled with a sentinel of its dtype; ``take``
 checks that the tail survived the call before it hands the elements back, so a write past the end fails the test
@@ -36,6 +37,26 @@ def take(buf, shape, what):
     bad = int((buf[n:] != sentinel(buf.dtype)).sum())
     assert bad == 0, "%s: %d values written past its %d elements" % (what, bad, n)
     return buf[:n].reshape(shape).cpu()
+
+
+def bits(t):
+    """The bytes of a tensor (NaNs compare by bit pattern), or a host value as is."""
+    if not torch.is_tensor(t):
+        return t
+    t = t.detach().contiguous().reshape(-1)
+    return t.to(torch.uint8) if t.dtype == torch.bool else t.view(torch.uint8)
+
+
+def same(a, b):
+    """Bit-identical tensors, or equal host values."""
+    a, b = bits(a), bits(b)
+    return torch.equal(a, b) if torch.is_tensor(a) else a == b
+
+
+def snap(out):
+    """A copy of every output of a call once the device is done with it."""
+    torch.cuda.synchronize()
+    return {k: v.detach().clone() if torch.is_tensor(v) else v for k, v in out.items()}
 
 
 def rows(t, N):

@@ -6,7 +6,6 @@ Gates are per element, err <= C * 2^-24 * M.  M is the float64 sum of |terms| be
 reduction over points (d_tfs: sum_i w_ij |dL/dA_i|; d_x: |A^-T| |g|); for the SMPL parameters, whose terms pass through the
 whole chain, M is the largest |gradient| among the four parameter outputs of the call.  C is 4x the worst measured on
 one H100 (printed as MEASURED)."""
-import ctypes as C
 import os
 import sys
 
@@ -26,6 +25,7 @@ from oracle import port                               # noqa: E402
 
 from _abi import padded, take                         # noqa: E402
 from _body_grad_port import port_smpl_grads, float64  # noqa: E402
+from _setups import Smpl, dirty_workspace, points, posed_body, small_model  # noqa: E402
 
 EPS = 2.0 ** -24
 MEASURED = {}
@@ -59,10 +59,6 @@ def _L():
     return L
 
 
-def _ws(nbytes):
-    return torch.full((max(int(nbytes), 1),), 0xFF, dtype=torch.uint8, device="cuda")
-
-
 def _bits(*arrs):
     return [np.asarray(a, np.float32).view(np.uint32).copy() for a in arrs]
 
@@ -70,48 +66,6 @@ def _bits(*arrs):
 # ---------------------------------------------------------------------------------------------
 # SMPL server
 # ---------------------------------------------------------------------------------------------
-
-class Smpl:
-    def __init__(self, model):
-        L = _L()
-        self.model, self.V = model, model["v_template"].shape[0]
-        self.d = {k: torch.as_tensor(np.ascontiguousarray(np.asarray(model[k]), np.float32)).cuda()
-                  for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "lbs_weights")}
-        pa = (C.c_int * 24)(*[max(int(p), 0) for p in model["parents"]])
-        self.storage = L.workspace(L.call("mp_smpl_bytes", self.V), "cuda")
-        self.h = L.Handle("mp_smpl_free")
-        d = self.d
-        L.call("mp_smpl_create", d["v_template"], d["shapedirs"], d["posedirs"], d["J_regressor"], pa, d["lbs_weights"],
-               self.V, None, self.storage, self.storage.numel(), C.byref(self.h))
-        ti = torch.empty(24, 4, 4, device="cuda")
-        L.call("mp_smpl_canonical", self.h, None, ti)
-        self.cinv = ti.cpu().numpy()
-
-    @staticmethod
-    def _args(scale, transl, theta, betas):
-        return [torch.from_numpy(np.asarray(a, np.float32).reshape(-1)).cuda() for a in ((scale,), transl, theta, betas)]
-
-    def forward(self, scale, transl, theta, betas, absolute):
-        v, t = torch.empty(self.V, 3, device="cuda"), torch.empty(24, 4, 4, device="cuda")
-        _L().call("mp_smpl_forward", self.h, *self._args(scale, transl, theta, betas), int(absolute), v, t)
-        return v, t
-
-    def backward(self, scale, transl, theta, betas, absolute, u_v, u_t):
-        L = _L()
-        dv = None if u_v is None else torch.from_numpy(np.asarray(u_v, np.float32)).cuda()
-        dt = None if u_t is None else torch.from_numpy(np.asarray(u_t, np.float32)).cuda()
-        outs = [padded(n) for n in (1, 3, 72, 10)]
-        ws = _ws(L.call("mp_smpl_backward_workspace_bytes", self.V))
-        L.call("mp_smpl_backward", self.h, *self._args(scale, transl, theta, betas), int(absolute), dv, dt, *outs, ws,
-               ws.numel())
-        torch.cuda.synchronize()
-        return [take(o, n, "d_" + k).numpy() for o, n, k in zip(outs, (1, 3, 72, 10), ("scale", "transl", "thetas", "betas"))]
-
-
-def _small_model(V):
-    from test_gpu_frame_geometry import small_model
-    return small_model(V)
-
 
 def _poses():
     rng = np.random.RandomState(21)
@@ -130,7 +84,7 @@ MODES = ["verts", "tfs", "both"]
 def test_smpl_backward_vs_port(name):
     """Every pose x (absolute, placement) x upstream mode against the port's float64 autograd; outputs padded, a 0xFF
     workspace, two runs bit-identical."""
-    model = G.model64() if name == "smpl6890" else _small_model(int(name[1:]))
+    model = G.model64() if name == "smpl6890" else small_model(int(name[1:]))
     model = {k: (v.numpy() if torch.is_tensor(v) else np.asarray(v)) for k, v in model.items()}
     model = {k: (v.astype(np.float32) if k != "parents" else v) for k, v in model.items()}
     hd = Smpl(model)
@@ -233,47 +187,12 @@ def _ref_inverse(x, idx, W, tfs, u, keep=None):
     return xc.detach(), xv.grad, d_tfs, M_x, M_tfs
 
 
-_BODY = {}
-
-
-def _posed_body():
-    if "b" not in _BODY:
-        from multiply_b200 import engine
-        from multiply_b200.model.smpl import SMPLServer
-        sm = S.make_smpl_model(300)
-        srv = SMPLServer(model=sm)
-        rng = np.random.RandomState(7)
-        o = srv(torch.ones(1), torch.zeros(1, 3), torch.from_numpy(rng.normal(0, 0.3, (1, 72)).astype(np.float32)),
-                torch.from_numpy(rng.normal(0, 1, (1, 10)).astype(np.float32)))
-        b = engine.Body(srv.verts_c[0], srv.weights[0], cano_cell=0.1001)
-        b.set_pose(o["smpl_verts"][0], o["smpl_tfs"][0])
-        _BODY["b"] = (b, srv)
-    return _BODY["b"]
-
-
-def _points(N, verts, seed, far_frac=0.1, far=0.3):
-    """Points within 0.09 of a vertex (inside the 0.1 outlier radius, where the grid search is exact either way), the first
-    far_frac of them moved by far * a random direction: ~N(0, far) per axis, or (far < 0) exactly |far| away, beyond the
-    grid's reach."""
-    rng = np.random.RandomState(seed)
-    v = verts.cpu().numpy()
-    off = rng.normal(0, 0.03, (N, 3))
-    n = np.linalg.norm(off, axis=1, keepdims=True)
-    off = np.where(n > 0.09, off * (0.09 / np.maximum(n, 1e-30)), off)
-    p = v[rng.randint(0, v.shape[0], N)] + off
-    nf = int(N * far_frac)
-    if nf:
-        d = rng.normal(0, 1, (nf, 3))
-        p[:nf] += d * far if far > 0 else -far * d / np.linalg.norm(d, axis=1, keepdims=True)
-    return torch.from_numpy(p.astype(np.float32))
-
-
 def _inv_backward(b, x, u, exact_far):
     L = _L()
     N = x.shape[0]
     xd, ud = x.cuda().contiguous(), u.cuda().float().contiguous()
     d_tfs, d_x, xc = padded((24, 4, 4)), padded((N, 3)), padded((N, 3))
-    ws = _ws(L.call("mp_deform_backward_workspace_bytes", N))
+    ws = dirty_workspace(L.call("mp_deform_backward_workspace_bytes", N))
     L.call("mp_deform_inverse_backward", b.handle, xd if N else None, N, int(exact_far), ud if N else None, d_tfs, d_x, xc,
            ws, ws.numel())
     torch.cuda.synchronize()
@@ -290,9 +209,9 @@ def test_deform_inverse_backward(N, exact_far):
     """d_x, the full 4x4 d_tfs (bottom row included) and the recomputed x_c (bit-equal to mp_deform_inverse's) against
     the port's float64 autograd; with exact_far = 0 the points are near the body or 5 away from it (no vertex:
     d_x = d_x_c, nothing to the bones).  Padded outputs, a 0xFF workspace, reruns bit-identical."""
-    b, _ = _posed_body()
+    b, _ = posed_body()
     far = 0.3 if exact_far else -5.0
-    x = _points(N, b.verts_p, 11 + N, far=far)
+    x = points(N, b.verts_p, 11 + N, far=far)
     u = torch.from_numpy(np.random.RandomState(N).randn(N, 3).astype(np.float32))
     d_tfs, d_x, xc = _inv_backward(b, x, u, exact_far)
     d_tfs2, d_x2, xc2 = _inv_backward(b, x, u, exact_far)
@@ -325,7 +244,7 @@ def test_deform_inverse_backward_ties():
     V = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
     W = np.random.RandomState(1).dirichlet(np.ones(24) * 0.3, V.shape[0]).astype(np.float32)
     b = engine.Body(torch.from_numpy(V), torch.from_numpy(W), cano_cell=0.1001)
-    _, srv = _posed_body()
+    _, srv = posed_body()
     o = srv(torch.ones(1), torch.zeros(1, 3), torch.from_numpy(np.random.RandomState(2).normal(0, 0.3, (1, 72)).astype(
         np.float32)), torch.zeros(1, 10))
     b.set_pose(torch.from_numpy(V), o["smpl_tfs"][0])
@@ -342,7 +261,7 @@ def test_deform_inverse_backward_ties():
 
 def test_deform_inverse_backward_refuses_root_finder():
     from multiply_b200 import _lib as L
-    b, _ = _posed_body()
+    b, _ = posed_body()
     b.set_root_finder(5)
     try:
         with pytest.raises(L.MpError, match="root finder"):
@@ -355,7 +274,7 @@ def _fwd_backward(b, xc, u_xd, u_J):
     L = _L()
     N = xc.shape[0]
     d_tfs, d_xc = padded((24, 4, 4)), padded((N, 3))
-    ws = _ws(L.call("mp_deform_backward_workspace_bytes", N))
+    ws = dirty_workspace(L.call("mp_deform_backward_workspace_bytes", N))
     dxd = None if u_xd is None else u_xd.cuda().float().contiguous()
     dJ = None if u_J is None else u_J.cuda().float().reshape(N, 9).contiguous()
     L.call("mp_deform_forward_jac_backward", b.handle, xc.cuda().contiguous(), N, dxd, dJ, d_tfs, d_xc, ws, ws.numel())
@@ -410,8 +329,8 @@ def _cano_mesh_sizes():
 def test_forward_jac_backward(mode):
     """On generate_mesh's canonical-mesh vertices (and N = 1, 257): d_x_c and d_tfs (bottom row 0) against the port's
     float64 autograd, d_x_d alone, d_Jinv alone and both; padded outputs, 0xFF workspace, reruns bit-identical."""
-    b, _ = _posed_body()
-    sets = [v for v in _cano_mesh_sizes()] + [_points(1, b.verts_c, 1), _points(257, b.verts_c, 2, far_frac=0.0)]
+    b, _ = posed_body()
+    sets = [v for v in _cano_mesh_sizes()] + [points(1, b.verts_c, 1), points(257, b.verts_c, 2, far_frac=0.0)]
     for k, xc in enumerate(sets):
         N = xc.shape[0]
         rng = np.random.RandomState(k)
@@ -541,7 +460,7 @@ def test_mirror_inverse_deformer_chain():
     sm, srv, dfm, params = _mirror_setup()
     with torch.no_grad():
         o0 = srv(params["scale"], params["transl"], params["thetas"], params["betas"])
-    x = _points(2000, o0["smpl_verts"][0], 8, far_frac=0.0)
+    x = points(2000, o0["smpl_verts"][0], 8, far_frac=0.0)
     u = torch.from_numpy(np.random.RandomState(5).randn(2000, 3).astype(np.float32))
     idx = _nearest(x, o0["smpl_verts"][0]).cpu()
     W = srv.weights[0].cpu().double()
@@ -569,7 +488,7 @@ def test_mirror_forward_skinning_chain():
     """SMPLServer -> forward_skinning + jacobian_inverse (the transforms the body is posed with) -> a seeded loss; a
     different transform tensor is refused."""
     sm, srv, dfm, params = _mirror_setup()
-    xc = _points(1500, srv.verts_c[0], 9, far_frac=0.0)
+    xc = points(1500, srv.verts_c[0], 9, far_frac=0.0)
     u_x = torch.from_numpy(np.random.RandomState(6).randn(1500, 3).astype(np.float32))
     u_J = torch.from_numpy(np.random.RandomState(7).randn(1500, 3, 3).astype(np.float32))
     idx = _nearest(xc, srv.verts_c[0]).cpu()
@@ -606,7 +525,7 @@ def test_mirror_no_grad_unchanged():
     for k in ("smpl_verts", "smpl_tfs"):
         assert a[k].grad_fn is None and b[k].grad_fn is None and c[k].grad_fn is not None
         assert torch.equal(a[k], b[k]) and torch.equal(a[k], c[k].detach())
-    x = _points(500, a["smpl_verts"][0], 3).cuda()
+    x = points(500, a["smpl_verts"][0], 3).cuda()
     xc0, o0 = dfm.forward(x, a["smpl_tfs"], return_weights=False, inverse=True, smpl_verts=a["smpl_verts"])
     xc1, o1 = dfm.forward(x, c["smpl_tfs"], return_weights=False, inverse=True, smpl_verts=c["smpl_verts"])
     assert xc0.grad_fn is None and xc1.grad_fn is not None

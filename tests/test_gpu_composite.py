@@ -21,9 +21,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from _abi import SENTINEL, padded, take     # noqa: E402
+from _abi import SENTINEL, padded, take                                     # noqa: E402
+from _setups import SMEM_CAP, make_inputs, person_samples, wpc_of           # noqa: E402
 
-SMEM_CAP = 200 * 1024                   # launch_composite: dynamic shared memory of one block
 N_MAX_P8 = SMEM_CAP // (12 * 8)         # 2133: the largest n with 12 * P * n <= 200 KB at P = 8
 # fp64 comparison gate of every output (fg_rgb, normal, acc, acc_person, bg_T); the measured worst values are quoted in
 # the docstring of test_composite_vs_fp64
@@ -89,63 +89,6 @@ def composite_ref(persons, R, n, beta, dtype=np.float64, reverse=False):
 # synthetic inputs
 # ---------------------------------------------------------------------------------------------
 
-def make_inputs(seed, P, R, n, substitute=False, ties=True):
-    """Per-person hit lists and sample rows.  Ray 0 is hit by every person, ray 1 by none, ray 2 by person 0 only, the
-    rest by random subsets; with `substitute` the last person's list is the single ray 0 (multiply.py:262-263).  Rows
-    are sorted z with a per-ray `far` shared by all persons as the last column; sdf spreads over [-1, 1] with exact
-    zeros.  With `ties`: persons 0 and 1 share one z row on ray 0 (and on every third ray both hit), some rows carry
-    zero-length intervals, and half of the rays end with a negative sdf on the last sample."""
-    rng = np.random.RandomState(seed)
-    H = rng.random_sample((P, R)) < 0.6
-    H[:, 0] = True
-    if R > 1:
-        H[:, 1] = False
-    if R > 2:
-        H[:, 2] = False
-        H[0, 2] = True
-    if substitute and P > 1:
-        H[P - 1] = False
-        H[P - 1, 0] = True
-    far = rng.uniform(3.0, 4.0, R).astype(np.float32)
-    neg_last = rng.random_sample(R) < 0.5
-    persons = []
-    for p in range(P):
-        idx = np.flatnonzero(H[p]).astype(np.int64)
-        Rp = idx.size
-        near = rng.uniform(0.5, 1.5, Rp)
-        u = np.sort(rng.random_sample((Rp, n - 1)), 1) if n > 1 else np.zeros((Rp, 0))
-        z = np.concatenate([near[:, None], near[:, None] + u * (far[idx] - near)[:, None], far[idx][:, None]], 1)
-        z = z.astype(np.float32)
-        z[:, -1] = far[idx]
-        zm = 0.5 * (z[:, :-1] + z[:, 1:])
-        surf = rng.uniform(0.8, 3.5, (Rp, 1))
-        k = rng.uniform(1.0, 20.0, (Rp, 1))
-        sdf = np.clip((surf - zm) * k + rng.normal(0, 0.05, zm.shape), -1, 1)
-        noisy = rng.random_sample(Rp) < 0.3
-        sdf[noisy] = rng.uniform(-1, 1, (int(noisy.sum()), n))
-        sdf[rng.random_sample(sdf.shape) < 0.05] = 0.0
-        sdf = sdf.astype(np.float32)
-        if ties:
-            if n > 2:        # zero-length intervals: z[i + 1] = z[i] on some rows
-                rows = rng.random_sample(Rp) < 0.3
-                cols = rng.randint(1, n - 1, int(rows.sum()))
-                z[np.flatnonzero(rows), cols + 1] = z[np.flatnonzero(rows), cols]
-            last_neg = neg_last[idx]
-            sdf[last_neg, -1] = -np.abs(sdf[last_neg, -1]) - np.float32(0.25)
-        persons.append(dict(idx=idx, z=np.ascontiguousarray(z), sdf=np.ascontiguousarray(sdf),
-                            rgb=rng.random_sample((Rp, n, 3)).astype(np.float32),
-                            nrm=rng.uniform(-1, 1, (Rp, n, 3)).astype(np.float32)))
-    if ties and P > 1:      # persons 0 and 1: identical z rows (and a negative-sdf stretch) on shared rays
-        a, b = persons[0], persons[1]
-        shared = np.intersect1d(a["idx"], b["idx"])
-        shared = shared[(shared % 3) == 0]
-        ra, rb = np.searchsorted(a["idx"], shared), np.searchsorted(b["idx"], shared)
-        b["z"][rb] = a["z"][ra]
-        b["sdf"][rb, : max(1, n // 2)] = -0.05
-        a["sdf"][ra, : max(1, n // 2)] = -0.02
-    return persons
-
-
 def subset(persons, rays):
     """The same samples composited for the rays `rays` only (sorted), renumbered 0 .. len(rays) - 1."""
     out = []
@@ -159,24 +102,6 @@ def subset(persons, rays):
 # ---------------------------------------------------------------------------------------------
 # the C ABI with sentinel-padded outputs
 # ---------------------------------------------------------------------------------------------
-
-def wpc_of(P, n):
-    """Rays per block of launch_composite."""
-    return max(1, min(8, SMEM_CAP // (12 * P * n)))
-
-
-def person_samples(persons):
-    """(mp_person_samples_t array, the device tensors it points to); a person without rays gets one-element
-    placeholders, so that every pointer is valid."""
-    from multiply_b200 import engine
-    keep = []
-    for d in persons:
-        if d["idx"].size:
-            keep.append([torch.from_numpy(np.ascontiguousarray(d[k])).cuda() for k in ("idx", "z", "sdf", "rgb", "nrm")])
-        else:
-            keep.append([torch.zeros(1, dtype=torch.int64, device="cuda")] + [torch.zeros(1, device="cuda")] * 4)
-    return engine.person_samples([t + [int(d["idx"].size)] for t, d in zip(keep, persons)]), keep
-
 
 def outputs(R, P):
     return dict(fg=padded((R, 3)), nrm=padded((R, 3)), acc=padded(R), accp=padded((R, P)), bgT=padded(R))

@@ -33,6 +33,7 @@ from multiply_b200 import scene as S          # noqa: E402  (CPU-only module)
 from oracle import render_grad as RG          # noqa: E402
 
 from _abi import SENTINEL_INT, padded, take     # noqa: E402
+from _setups import small_model                 # noqa: E402
 
 EPS = 2.0 ** -24
 MEASURED = {}
@@ -160,28 +161,6 @@ def canonical_ref(model, betas_c):
 
 def model_np(m):
     return {k: (v.numpy() if torch.is_tensor(v) else np.asarray(v)) for k, v in m.items()}
-
-
-def small_model(V, seed=301, dense=False):
-    """scene.make_smpl_model's construction at V vertices (the first V of the capsule body); dense: every vertex
-    regresses every joint (positive weights, rows summing to 1)."""
-    rng = np.random.RandomState(seed)
-    verts_t, W = S.make_body(100, V=V)
-    V = verts_t.shape[0]
-    Jr = np.zeros((24, V))
-    if dense:
-        Jr = rng.uniform(0.5, 1.5, (24, V))
-        Jr /= Jr.sum(1, keepdims=True)
-    else:
-        for j in range(24):
-            d = np.linalg.norm(verts_t - S._J[j], axis=1)
-            idx = np.argsort(d)[:min(64, V)]
-            w = np.exp(-(d[idx] / 0.08) ** 2) + 1e-6
-            Jr[j, idx] = w / w.sum()
-    f32 = lambda a: np.ascontiguousarray(a.astype(np.float32))
-    return dict(v_template=f32(verts_t), shapedirs=f32(0.01 * rng.randn(V, 3, 10)),
-                posedirs=f32(0.004 * rng.randn(207, V * 3)), J_regressor=f32(Jr),
-                parents=np.array(S.PARENTS, np.int64), lbs_weights=f32(W))
 
 
 def get_model(name):

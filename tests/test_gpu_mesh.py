@@ -8,8 +8,10 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from multiply_b200 import scene as S
-from oracle import mesh_port as port
+from multiply_b200 import scene as S                                              # noqa: E402
+from oracle import mesh_port as port                                              # noqa: E402
+
+from _setups import flags_from_taps, fused_setup, mirror_inputs, render_train, train  # noqa: E402
 
 
 @pytest.fixture(scope="module")
@@ -83,70 +85,6 @@ def test_mesh_surface_flags_vs_port(meshes):
 
 # ---- fused path and mirror -----------------------------------------------------------------------------------------
 
-OPT = dict(
-    with_bkgd=True, num_training_frames=75, dim_frame_encoding=32,
-    implicit_network=dict(feature_vector_size=256, d_in=3, d_out=1, dims=[256] * 8, init="geometry", bias=0.6,
-                          skip_in=[4], weight_norm=True, embedder_mode="fourier", multires=6, cond="smpl"),
-    rendering_network=dict(feature_vector_size=256, mode="pose_no_view", d_in=14, d_out=3, dims=[256] * 4,
-                           weight_norm=True, multires_view=-1),
-    bg_implicit_network=dict(feature_vector_size=256, d_in=4, d_out=1, dims=[256] * 8, init="none", bias=0.0,
-                             skip_in=[4], weight_norm=False, embedder_mode="fourier", multires=10, cond="frame"),
-    bg_rendering_network=dict(feature_vector_size=256, mode="nerf_frame_encoding", d_in=3, d_out=3, dims=[128],
-                              weight_norm=False, multires_view=4),
-    density=dict(params_init={"beta": 0.1}, beta_min=0.0001),
-    ray_sampler=dict(near=0.0, N_samples=16, N_samples_eval=32, N_samples_extra=8, eps=0.1, beta_iters=10,
-                     max_total_iters=5, N_samples_inverse_sphere=32, add_tiny=1.0e-6),
-)
-
-
-def _build(sc):
-    from multiply_b200.model.multiply import Multiply
-    P = len(sc["persons"])
-    m = Multiply(OPT, smpl_server_list=[S.SyntheticSMPLServer(p, P) for p in range(P)])
-    sd = {}
-    for p, person in enumerate(sc["persons"]):
-        for k, v in person["implicit"].items():
-            sd[f"foreground_implicit_network_list.{p}.{k}"] = v
-        for k, v in person["render"].items():
-            sd[f"foreground_rendering_network_list.{p}.{k}"] = v
-    for k, v in sc["bg_implicit"].items():
-        sd["bg_implicit_network." + k] = v
-    for k, v in sc["bg_render"].items():
-        sd["bg_rendering_network." + k] = v
-    sd["density.beta"] = torch.tensor(sc["beta_param"])
-    fw = torch.zeros(75, 32)
-    fw[3] = sc["frame_code"][0]
-    sd["frame_latent_encoder.weight"] = fw
-    m.load_state_dict(sd, strict=True)
-    return m.cuda().eval()
-
-
-def _inputs(sc, inp, hits, epoch):
-    P = 2
-    transl = torch.tensor([[0.8 * (p - (P - 1) / 2.0), 0.15, 0.3 * p] for p in range(P)])[None]
-    smpl_pose = torch.stack([sc["persons"][p]["smpl_pose"][0] for p in range(P)])[None]
-    smpl_params = torch.zeros(1, P, 86)
-    smpl_params[:, :, 0] = 0.5
-    d = dict(uv=inp["uv"].cuda(), pose=inp["pose"].cuda(), intrinsics=inp["intrinsics"].cuda(),
-             smpl_params=smpl_params.cuda(), smpl_pose=smpl_pose.cuda(), smpl_shape=torch.zeros(1, P, 10).cuda(),
-             smpl_trans=transl.cuda(), idx=torch.tensor([3]).cuda(), current_epoch=epoch)
-    d["smpl_pose_last"] = d["smpl_pose"] + 0.01
-    if hits is not None:
-        d["index_ray_box_list"] = hits
-    return d
-
-
-def _train(m, inputs, seed, id=-1):
-    m.train()
-    try:
-        torch.manual_seed(seed)
-        out = m(inputs, id=id)
-        torch.cuda.synchronize()
-    finally:
-        m.eval()
-    return out
-
-
 def test_forward_training_early_epoch_mirror(golden_dir):
     """Multiply.forward in .train() at current_epoch = 137 against the reference's training branch (flags of
     check_off_in_surface_points_cano_mesh merged as multiply.py:549-560, and every other output)."""
@@ -156,8 +94,8 @@ def test_forward_training_early_epoch_mirror(golden_dir):
     sc = S.make_scene(P=2, S=16, seed=42)
     inp = S.make_rays(sc, 40, seed=35, region="boxes")
     assert np.array_equal(inp["uv"].numpy(), g["uv"])
-    m = _build(sc)
-    out = _train(m, _inputs(sc, inp, [torch.from_numpy(g[f"hits_{p}"]).cuda() for p in range(2)], 137), 4322)
+    m = S.mirror_model(sc)
+    out = train(m, mirror_inputs(inp, 2, [torch.from_numpy(g[f"hits_{p}"]).cuda() for p in range(2)], epoch=137), 4322)
     edge = np.zeros(40, dtype=bool)
     for p in range(2):
         mn = g[f"min_signed_{p}"]
@@ -173,76 +111,22 @@ def test_forward_training_early_epoch_mirror(golden_dir):
         assert np.median(d) < 1e-5 and d.max() < tol, (k, float(d.max()))
 
 
-def _render_train(r, inp, hits, rngs, t_rand_bg, meshes, persons=None, thr=0.05):
-    tr = dict(rng=rngs, t_rand_bg=t_rand_bg)
-    if meshes is not None:
-        tr.update(meshes=meshes, threshold=thr)
-    out = r.render(inp, hits, debug=True, persons=persons, train=tr)
-    torch.cuda.synchronize()
-    return out
-
-
-def _fused_setup(R=256, empty_person1=False):
-    from multiply_b200 import engine
-    engine.set_engine("tc")
-    sc = S.make_scene(P=2, S=16, seed=42)
-    r = engine.Renderer(sc)
-    inp = S.make_rays(sc, R, seed=77, region="boxes")
-    hits = S.make_hit_lists(sc, inp)
-    if empty_person1:
-        hits[1] = torch.zeros(0, dtype=torch.int64)
-    meshes = [engine.CanonicalMesh(*S.make_body_mesh(100 + p)) for p in range(2)]
-    from multiply_b200.model.ray_sampler import ErrorBoundSampler
-    smp = ErrorBoundSampler(3.0, inverse_sphere_bg=True, **{k: sc["cfg"][k] for k in (
-        "near", "N_samples", "N_samples_eval", "N_samples_extra", "eps", "beta_iters", "max_total_iters", "add_tiny")})
-    torch.manual_seed(5)
-    rngs = [smp.draw_training_rng(max(h.numel(), 1)) for h in hits]
-    rngs = [{k: v for k, v in rg.items() if k != "states"} for rg in rngs]
-    return sc, r, inp, hits, meshes, rngs, torch.rand(R, 32)
-
-
-def _flags_from_taps(sc, r, inp, hits, meshes, out, plist, thr=0.05, xc_out=None):
-    """The flags recomputed with mp_mesh_surface_flags from the main pass's canonical points (z taps -> samples ->
-    mp_deform_inverse), merged on the host as multiply.py:549-560.  xc_out (a list) receives each person's (rows,
-    canonical points)."""
-    from multiply_b200.model import rend_util
-    dirs, cam = rend_util.get_camera_params(inp["uv"].cuda(), inp["pose"].cuda(), inp["intrinsics"].cuda())
-    dirs = dirs[0]
-    R = dirs.shape[0]
-    cam = cam.expand(R, 3)
-    n = r.n
-    off = torch.ones(R, len(plist), dtype=torch.bool, device="cuda")
-    inn = torch.zeros(R, len(plist), dtype=torch.bool, device="cuda")
-    for k, p in enumerate(plist):
-        h = hits[p] if hits[p].numel() else torch.zeros(1, dtype=torch.int64)
-        h = h.cuda()
-        z = out[f"z_vals_{k}"][:, :n]
-        pts = (cam[h][:, None] + z[..., None] * dirs[h][:, None]).reshape(-1, 3)
-        xc, _ = r.bodies[p].deform_inverse(pts, exact_far=True)
-        o, i = meshes[k].surface_flags(xc, n, thr)
-        if xc_out is not None:
-            xc_out.append((h, xc))
-        off[h, k] = o
-        inn[h, k] = i
-    return off.all(1), inn.any(1)
-
-
 @pytest.mark.parametrize("case", ["both", "single", "empty"])
 def test_fused_flags_match_standalone(case):
     """Flags of mp_render_rays == mp_mesh_surface_flags on the same canonical points, for both persons, a single
     rendered person (id = p: one column) and a person with an empty hit list (the ray-0 substitute); flags on or off
     leave every pixel output bit-identical."""
-    sc, r, inp, hits, meshes, rngs, tb = _fused_setup(empty_person1=(case == "empty"))
+    sc, r, inp, hits, meshes, rngs, tb = fused_setup(empty_person1=(case == "empty"))
     plist = [1] if case == "single" else [0, 1]
     hl = [hits[p] for p in plist]
     rg = [rngs[p] for p in plist]
     ms = [meshes[p] for p in plist]
-    on = _render_train(r, inp, hl, rg, tb, ms, persons=plist)
-    off_ = _render_train(r, inp, hl, rg, tb, None, persons=plist)
+    on = render_train(r, inp, hl, rg, tb, ms, persons=plist)
+    off_ = render_train(r, inp, hl, rg, tb, None, persons=plist)
     for k in ("rgb_values", "fg_rgb_values", "normal_values", "acc_map", "acc_person_list"):
         assert torch.equal(on[k], off_[k]), k
     assert "index_off_surface" not in off_
-    want_off, want_in = _flags_from_taps(sc, r, inp, hits, ms, on, plist)
+    want_off, want_in = flags_from_taps(sc, r, inp, hits, ms, on, plist)
     assert torch.equal(on["index_off_surface"], want_off)
     assert torch.equal(on["index_in_surface"], want_in)
     if case == "empty":
@@ -258,14 +142,14 @@ def test_set_canonical_mesh_and_missing_mesh(golden_dir):
     g = np.load(os.path.join(golden_dir, "forward_train_early.npz"))
     sc = S.make_scene(P=2, S=16, seed=42)
     inp = S.make_rays(sc, 40, seed=35, region="boxes")
-    m = _build(sc)
+    m = S.mirror_model(sc)
     hits = [torch.from_numpy(g[f"hits_{p}"]).cuda() for p in range(2)]
-    a = _train(m, _inputs(sc, inp, hits, 137), 4322)
+    a = train(m, mirror_inputs(inp, 2, hits, epoch=137), 4322)
     # a much larger mesh: every canonical sample lies inside it
     v, f = S.make_body_mesh(100)
     m.set_canonical_mesh(0, v * 20.0, f)
     m.set_canonical_mesh(1, v * 20.0, f)
-    b = _train(m, _inputs(sc, inp, hits, 137), 4322)
+    b = train(m, mirror_inputs(inp, 2, hits, epoch=137), 4322)
     hit_any = torch.zeros(40, dtype=torch.bool)
     for h in hits:
         hit_any[h.cpu()] = True
@@ -278,8 +162,8 @@ def test_set_canonical_mesh_and_missing_mesh(golden_dir):
     m.mesh_f_cano_list[1] = None
     m._cano_meshes.pop(1, None)
     with pytest.raises(ValueError, match="set_canonical_mesh"):
-        _train(m, _inputs(sc, inp, hits, 137), 4322)
-    late = _train(m, _inputs(sc, inp, hits, 251), 4322)
+        train(m, mirror_inputs(inp, 2, hits, epoch=137), 4322)
+    late = train(m, mirror_inputs(inp, 2, hits, epoch=251), 4322)
     assert late["index_off_surface"] is None and late["index_in_surface"] is None
 
 

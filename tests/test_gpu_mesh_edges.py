@@ -34,6 +34,7 @@ from multiply_b200 import scene as S
 from oracle import mesh_port as port
 
 from _abi import padded, take
+from _setups import flags_from_taps, fused_setup, render_train
 
 gpu = pytest.mark.gpu
 
@@ -681,11 +682,10 @@ def test_flags_nan_threshold_rejected():
 def test_fused_flags_threshold(thr):
     """mp_render_rays' fused flags at thr equal mp_mesh_surface_flags on the main pass's canonical points and the
     brute-force flags of those points; a NaN threshold is an error."""
-    import test_gpu_mesh as T
-    sc, r, inp, hits, meshes, rngs, tb = T._fused_setup()
-    on = T._render_train(r, inp, hits, rngs, tb, meshes, persons=[0, 1], thr=thr)
+    sc, r, inp, hits, meshes, rngs, tb = fused_setup()
+    on = render_train(r, inp, hits, rngs, tb, meshes, persons=[0, 1], thr=thr)
     xcs = []
-    want_off, want_in = T._flags_from_taps(sc, r, inp, hits, meshes, on, [0, 1], thr=thr, xc_out=xcs)
+    want_off, want_in = flags_from_taps(sc, r, inp, hits, meshes, on, [0, 1], thr=thr, xc_out=xcs)
     assert torch.equal(on["index_off_surface"], want_off)
     assert torch.equal(on["index_in_surface"], want_in)
     for p, (h, xc) in enumerate(xcs):
@@ -695,11 +695,11 @@ def test_fused_flags_threshold(thr):
         assert torch.equal(o, ro) and torch.equal(i, ri)
     if thr == -0.05:
         # the threshold matters: some ray keeps off only because of inside samples shallower than |thr|
-        o0, _ = T._flags_from_taps(sc, r, inp, hits, meshes, on, [0, 1], thr=0.0)
+        o0, _ = flags_from_taps(sc, r, inp, hits, meshes, on, [0, 1], thr=0.0)
         assert bool((want_off & ~o0).any())
     L = _L()
     with pytest.raises(L.MpError, match="NaN"):
-        T._render_train(r, inp, hits, rngs, tb, meshes, persons=[0, 1], thr=float("nan"))
+        render_train(r, inp, hits, rngs, tb, meshes, persons=[0, 1], thr=float("nan"))
 
 
 # ---------------------------------------------------------------------------------------------

@@ -16,10 +16,9 @@ from oracle import build_ref, mesh_extract as M
 
 @pytest.fixture(scope="module")
 def model():
-    from test_gpu_mirror import _build
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42, weights="trained")
-    return sc, _build(sc)
+    return sc, S.mirror_model(sc)
 
 
 def _values_at(m, pid, cond, R, center, extent):

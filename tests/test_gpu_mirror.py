@@ -8,59 +8,9 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from multiply_b200 import scene as S
+from multiply_b200 import scene as S     # noqa: E402
 
-OPT = dict(
-    with_bkgd=True, num_training_frames=75, dim_frame_encoding=32,
-    implicit_network=dict(feature_vector_size=256, d_in=3, d_out=1, dims=[256] * 8, init="geometry", bias=0.6,
-                          skip_in=[4], weight_norm=True, embedder_mode="fourier", multires=6, cond="smpl"),
-    rendering_network=dict(feature_vector_size=256, mode="pose_no_view", d_in=14, d_out=3, dims=[256] * 4,
-                           weight_norm=True, multires_view=-1),
-    bg_implicit_network=dict(feature_vector_size=256, d_in=4, d_out=1, dims=[256] * 8, init="none", bias=0.0,
-                             skip_in=[4], weight_norm=False, embedder_mode="fourier", multires=10, cond="frame"),
-    bg_rendering_network=dict(feature_vector_size=256, mode="nerf_frame_encoding", d_in=3, d_out=3, dims=[128],
-                              weight_norm=False, multires_view=4),
-    density=dict(params_init={"beta": 0.1}, beta_min=0.0001),
-    ray_sampler=dict(near=0.0, N_samples=16, N_samples_eval=32, N_samples_extra=8, eps=0.1, beta_iters=10,
-                     max_total_iters=5, N_samples_inverse_sphere=32, add_tiny=1.0e-6),
-)
-
-
-def _build(sc):
-    from multiply_b200.model.multiply import Multiply
-    P = len(sc["persons"])
-    servers = [S.SyntheticSMPLServer(p, P) for p in range(P)]
-    m = Multiply(OPT, smpl_server_list=servers)
-    sd = {}
-    for p, person in enumerate(sc["persons"]):
-        for k, v in person["implicit"].items():
-            sd[f"foreground_implicit_network_list.{p}.{k}"] = v
-        for k, v in person["render"].items():
-            sd[f"foreground_rendering_network_list.{p}.{k}"] = v
-    for k, v in sc["bg_implicit"].items():
-        sd["bg_implicit_network." + k] = v
-    for k, v in sc["bg_render"].items():
-        sd["bg_rendering_network." + k] = v
-    sd["density.beta"] = torch.tensor(sc["beta_param"])
-    fw = torch.zeros(75, 32)
-    fw[3] = sc["frame_code"][0]
-    sd["frame_latent_encoder.weight"] = fw
-    missing, unexpected = m.load_state_dict(sd, strict=True), None
-    return m.cuda().eval()
-
-
-def _drop_in_inputs(sc, inp, P, with_hits=None):
-    transl = torch.tensor([[0.8 * (p - (P - 1) / 2.0), 0.15, 0.3 * p] for p in range(P)])[None]
-    smpl_pose = torch.stack([sc["persons"][p]["smpl_pose"][0] for p in range(P)])[None]
-    smpl_params = torch.zeros(1, P, 86)
-    smpl_params[:, :, 0] = 0.5
-    inputs = dict(uv=inp["uv"].cuda(), pose=inp["pose"].cuda(), intrinsics=inp["intrinsics"].cuda(),
-                  smpl_params=smpl_params.cuda(), smpl_pose=smpl_pose.cuda(), smpl_shape=torch.zeros(1, P, 10).cuda(),
-                  smpl_trans=transl.cuda(), idx=torch.tensor([3]).cuda())
-    if with_hits is not None:
-        inputs["index_ray_box_list"] = with_hits
-    return inputs
-
+from _setups import mirror_inputs       # noqa: E402
 
 @pytest.mark.parametrize("pid", [-1, 0, 1])
 @pytest.mark.parametrize("device_culling", [False, True])
@@ -78,8 +28,8 @@ def test_multiply_forward_drop_in(pid, device_culling):
     plist = [0, 1] if pid == -1 else [pid]
     sub = dict(sc, persons=[sc["persons"][p] for p in plist])
     ref = port.multiply_forward(sub, inp, [hits[p] for p in plist])
-    m = _build(sc)
-    inputs = _drop_in_inputs(sc, inp, 2, None if device_culling else [h.cuda() for h in hits])
+    m = S.mirror_model(sc)
+    inputs = mirror_inputs(inp, 2, None if device_culling else [h.cuda() for h in hits])
     out = m(inputs, id=pid)
     torch.cuda.synchronize()
     assert set(out) == {"acc_map", "acc_person_list", "rgb_values", "fg_rgb_values", "normal_values"}
@@ -99,7 +49,7 @@ def test_multiply_forward_canonical_pose():
     from oracle import port
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42)
-    m = _build(sc)
+    m = S.mirror_model(sc)
     P = 2
     cpose = torch.zeros(1, 72)
     cpose[0, 5], cpose[0, 8] = math.pi / 6, -math.pi / 6
@@ -112,7 +62,7 @@ def test_multiply_forward_canonical_pose():
     hits = S.make_hit_lists(csc, inp)
     assert sum(h.numel() for h in hits) > 40
     ref = port.multiply_forward(csc, inp, hits)
-    out = m(_drop_in_inputs(sc, inp, P, [h.cuda() for h in hits]), canonical_pose=True)
+    out = m(mirror_inputs(inp, P, [h.cuda() for h in hits]), canonical_pose=True)
     torch.cuda.synchronize()
     for k in ("rgb_values", "fg_rgb_values", "acc_map", "acc_person_list"):
         assert float((out[k].cpu() - ref[k]).abs().max()) < 1e-4, k
@@ -148,7 +98,7 @@ def test_query_oc_and_dense_grid(golden_dir):
     engine.set_engine("tc")
     g = np.load(os.path.join(golden_dir, "sdf_grid.npz"))
     sc = S.make_scene(P=2, S=64, seed=42)
-    m = _build(sc)
+    m = S.mirror_model(sc)
     p1 = sc["persons"][1]
     cond = {"smpl": p1["cond"].cuda()}
     pts = torch.from_numpy(g["points"]).cuda()
@@ -178,7 +128,7 @@ def test_sampler_training_mode(golden_dir):
     d, o = dirs[idx].cuda(), cam[idx].cuda()
     R = idx.numel()
     p0 = sc["persons"][0]
-    m = _build(sc)
+    m = S.mirror_model(sc)
     cfg = sc["cfg"]
     smp = ErrorBoundSampler(3.0, cfg["near"], cfg["N_samples"], cfg["N_samples_eval"], cfg["N_samples_extra"], cfg["eps"],
                             cfg["beta_iters"], cfg["max_total_iters"], inverse_sphere_bg=True, add_tiny=cfg["add_tiny"])
@@ -237,10 +187,8 @@ def test_forward_training_values(golden_dir):
     sc = S.make_scene(P=2, S=16, seed=42)
     inp = S.make_rays(sc, 40, seed=33, region="boxes")
     assert np.array_equal(inp["uv"].numpy(), g["uv"])
-    m = _build(sc)
-    inputs = _drop_in_inputs(sc, inp, 2, [torch.from_numpy(g[f"hits_{p}"]).cuda() for p in range(2)])
-    inputs["current_epoch"] = 251
-    inputs["smpl_pose_last"] = inputs["smpl_pose"] + 0.01
+    m = S.mirror_model(sc)
+    inputs = mirror_inputs(inp, 2, [torch.from_numpy(g[f"hits_{p}"]).cuda() for p in range(2)], epoch=251)
     m.train()
     try:
         torch.manual_seed(4321)
@@ -260,7 +208,7 @@ def test_load_reference_checkpoint_keys():
     """A Lightning checkpoint of the reference (keys 'model.*', plus smpl_server_list / deformer_list buffers and
     MultiplyModel's body_model_list, train.py:16-22) loads through load_reference_checkpoint with strict=True."""
     sc = S.make_scene(P=2, S=16, seed=42)
-    m = _build(sc)
+    m = S.mirror_model(sc)
     sd = {"model." + k: v for k, v in m.state_dict().items()}
     sd["model.smpl_server_list.0.smpl.v_template"] = torch.zeros(6890, 3)
     sd["model.deformer_list.1.smpl.smpl.lbs_weights"] = torch.zeros(6890, 24)
@@ -278,7 +226,7 @@ def test_operator_mirrors():
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42)
     p0 = sc["persons"][0]
-    net = networks.ImplicitNet(OPT["implicit_network"])
+    net = networks.ImplicitNet(S.MODEL_OPT["implicit_network"])
     net.load_state_dict(p0["implicit"], strict=True)
     net = net.cuda().eval()
     x = (torch.rand(300, 3, generator=torch.Generator().manual_seed(1)) - 0.5)
@@ -287,7 +235,7 @@ def test_operator_mirrors():
         ref = port.implicit_forward(p0["implicit"], x, p0["cond"], 6)
     assert y.shape == (1, 300, 257)
     assert float((y[0].cpu() - ref).abs().max()) < 5e-5
-    rn = networks.RenderingNet(OPT["rendering_network"])
+    rn = networks.RenderingNet(S.MODEL_OPT["rendering_network"])
     rn.load_state_dict(p0["render"], strict=True)
     rn = rn.cuda().eval()
     nrm = torch.nn.functional.normalize(torch.randn(300, 3, generator=torch.Generator().manual_seed(2)), dim=1)
@@ -313,7 +261,7 @@ def test_sdf_func_with_smpl_deformer_mirror():
     from oracle import port
     engine.set_engine("tc")
     sc = S.make_scene(P=2, S=16, seed=42)
-    m = _build(sc)
+    m = S.mirror_model(sc)
     p1 = sc["persons"][1]
     g = torch.Generator().manual_seed(3)
     pts = torch.cat([p1["verts_p"][:300] + 0.02 * torch.randn(300, 3, generator=g),       # near the body
@@ -376,13 +324,13 @@ def test_sequence_directory_drives_forward(tmp_path):
     engine.set_engine("tc")
     P, res = 2, 24
     sc = S.make_scene(P=P, S=16, seed=42)
-    model = _build(sc)
+    model = S.mirror_model(sc)
     K, pose = S.make_camera(f=900.0 * res / 512, res=res)         # same field of view as the 512 x 512 test camera
-    base = _drop_in_inputs(sc, dict(S.grid_rays(res=res), intrinsics=K, pose=pose), P)
+    base = mirror_inputs(dict(S.grid_rays(res=res), intrinsics=K, pose=pose), P)
 
     Rm = pose[0, :3, :3].double().numpy().T                       # world -> camera
     c = pose[0, :3, 3].double().numpy()
-    scale_mat = np.diag([2.0, 2.0, 2.0, 1.0])                      # scale = 0.5, as _drop_in_inputs
+    scale_mat = np.diag([2.0, 2.0, 2.0, 1.0])                      # scale = 0.5, as smpl_scene_inputs
     world = np.eye(4)
     world[:3, :4] = K[0, :3, :3].double().numpy() @ np.concatenate([Rm, (-Rm @ (2.0 * c))[:, None]], 1)
     np.save(tmp_path / "mean_shape.npy", np.zeros((P, 10), np.float32))
@@ -420,8 +368,8 @@ def test_multiply_root_finder_switch():
     sc = S.make_scene(P=2, S=16, seed=42)
     inp = S.make_rays(sc, 96, seed=11, region="boxes")
     hits = S.make_hit_lists(sc, inp)
-    m = _build(sc)
-    inputs = _drop_in_inputs(sc, inp, 2, with_hits=[h.cuda() for h in hits])
+    m = S.mirror_model(sc)
+    inputs = mirror_inputs(inp, 2, [h.cuda() for h in hits])
     plain = {k: v.clone() for k, v in m(inputs).items()}
     m.set_root_finder(10, 1e-5)
     on = {k: v.clone() for k, v in m(inputs).items()}
@@ -449,11 +397,8 @@ def test_oriented_box_culling():
     inp = S.make_rays(sc, 160, seed=21, region="image")
     P = 2
     servers = [S.SyntheticSMPLServer(p, P) for p in range(P)]
-    from multiply_b200.model.multiply import Multiply
-    m = Multiply(OPT, smpl_server_list=servers, culling="obb")
-    m.load_state_dict(_build(sc).state_dict())
-    m = m.cuda().eval()
-    inputs = _drop_in_inputs(sc, inp, P)
+    m = S.mirror_model(sc, servers, culling="obb")
+    inputs = mirror_inputs(inp, P)
     out = m(inputs)
     torch.cuda.synchronize()
     # the same lists on the host

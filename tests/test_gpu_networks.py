@@ -31,6 +31,7 @@ from multiply_b200 import scene as S          # noqa: E402
 from oracle import port                       # noqa: E402
 
 from _abi import padded, rows, take           # noqa: E402
+from _setups import mirror_inputs             # noqa: E402
 
 ENGINES = ["simt", "tc"]
 WEIGHTS = ["geometric", "trained"]
@@ -517,38 +518,15 @@ def test_mirror_checkpoint_trained():
     engine.set_engine("tc")
     sc = _scene("trained")
     P = 2
-    opt = dict(S.MODEL_OPT, ray_sampler=dict({k: v for k, v in sc["cfg"].items() if k in (
-        "near", "N_samples", "N_samples_eval", "N_samples_extra", "eps", "beta_iters", "max_total_iters", "add_tiny")},
-        N_samples_inverse_sphere=32))
-    m = Multiply(opt, smpl_server_list=[S.SyntheticSMPLServer(p, P) for p in range(P)])
-    sd = {}
-    for p, person in enumerate(sc["persons"]):
-        for k, v in person["implicit"].items():
-            sd[f"model.foreground_implicit_network_list.{p}.{k}"] = v
-        for k, v in person["render"].items():
-            sd[f"model.foreground_rendering_network_list.{p}.{k}"] = v
-    for k, v in sc["bg_implicit"].items():
-        sd["model.bg_implicit_network." + k] = v
-    for k, v in sc["bg_render"].items():
-        sd["model.bg_rendering_network." + k] = v
-    sd["model.density.beta"] = torch.tensor(sc["beta_param"])
-    fw = torch.zeros(75, 32)
-    fw[3] = sc["frame_code"][0]
-    sd["model.frame_latent_encoder.weight"] = fw
+    m = Multiply(S.model_opt(sc["cfg"]), smpl_server_list=[S.SyntheticSMPLServer(p, P) for p in range(P)])
+    sd = {"model." + k: v for k, v in S.mirror_state_dict(sc).items()}
     res = m.load_reference_checkpoint(sd, strict=True)
     assert not res.missing_keys and not res.unexpected_keys
     m = m.cuda().eval()
     inp = S.make_rays(sc, 96, seed=11, region="boxes")
     hits = S.make_hit_lists(sc, inp)
     ref = port.multiply_forward(sc, inp, hits)
-    smpl_pose = torch.stack([sc["persons"][p]["smpl_pose"][0] for p in range(P)])[None]
-    smpl_params = torch.zeros(1, P, 86)
-    smpl_params[:, :, 0] = 0.5
-    transl = torch.tensor([[0.8 * (p - (P - 1) / 2.0), 0.15, 0.3 * p] for p in range(P)])[None]
-    inputs = dict(uv=inp["uv"].cuda(), pose=inp["pose"].cuda(), intrinsics=inp["intrinsics"].cuda(),
-                  smpl_params=smpl_params.cuda(), smpl_pose=smpl_pose.cuda(), smpl_shape=torch.zeros(1, P, 10).cuda(),
-                  smpl_trans=transl.cuda(), idx=torch.tensor([3]).cuda(), index_ray_box_list=[h.cuda() for h in hits])
-    out = m(inputs)
+    out = m(mirror_inputs(inp, P, [h.cuda() for h in hits]))
     torch.cuda.synchronize()
     for k in ("rgb_values", "fg_rgb_values", "acc_map", "acc_person_list", "normal_values"):
         assert _err(out[k].cpu(), ref[k]) < TOL_GATE, k

@@ -29,7 +29,7 @@ for p in (ROOT, HERE):
 
 from oracle import render_grad as RG                            # noqa: E402
 from _abi import SENTINEL, padded, take                         # noqa: E402
-from test_gpu_composite import make_inputs, person_samples, wpc_of     # noqa: E402
+from _setups import make_inputs, mirror_inputs, person_samples, wpc_of  # noqa: E402
 
 EPS = 2.0 ** -24
 TINY = 2.0 ** -102
@@ -358,16 +358,11 @@ def _loss(rgb, acc, accp, gt, mask):
 
 
 def _mirror_case(P, seed=33):
-    from test_gpu_mirror import _build, _drop_in_inputs
     from multiply_b200 import scene as S
     sc = S.make_scene(P=P, S=16, seed=42, weights="trained")
     inp = S.make_rays(sc, 40, seed=seed, region="boxes")
     hits = [h.cuda() for h in S.make_hit_lists(sc, inp)]
-    m = _build(sc)
-    inputs = _drop_in_inputs(sc, inp, P, hits)
-    inputs["current_epoch"] = 251
-    inputs["smpl_pose_last"] = inputs["smpl_pose"] + 0.01
-    return m, inputs
+    return S.mirror_model(sc), mirror_inputs(inp, P, hits, epoch=251)
 
 
 def _run_mirror(m, inputs, pid, grad_on, streams=1):

@@ -31,6 +31,7 @@ from oracle import port                       # noqa: E402
 
 from _abi import SENTINEL, SENTINEL_INT, padded, take                                            # noqa: E402
 from _sampler_ref import EPS, MASK_MAX_M4096, MASK_MAX_TRIPS, cfg_of, compare, far_of, report      # noqa: E402
+from _setups import rays, train_rng                                                              # noqa: E402
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -74,39 +75,6 @@ def const_field(p, c):
     f = engine.Field(imp, p["render"])
     f.set_cond(p["cond"])
     return f
-
-
-def rays(scene, R, seed=5):
-    """R rays of person 0's box (repeated if the box has fewer hits), as float32 (dirs, cam) on the host."""
-    inp = S.make_rays(scene, max(4 * R, 64), seed=seed, region="boxes")
-    dirs, cam = port.get_camera_params(inp["uv"], inp["pose"], inp["intrinsics"])
-    dirs = dirs.reshape(-1, 3)
-    cam = cam.unsqueeze(1).repeat(1, dirs.shape[0] // cam.shape[0], 1).reshape(-1, 3)
-    idx = S.make_hit_lists(scene, inp)[0]
-    idx = idx.repeat((R + idx.numel() - 1) // idx.numel())[:R]
-    return dirs[idx].contiguous(), cam[idx].contiguous()
-
-
-def train_rng(cfg, R, seed=0, edges=False):
-    """Draws of mp_sample_rays_train with distinct per-trip rows.  edges: t_rand / u_final hold exact 0 and 1 - 2^-24
-    (stratified samples tie with near and with each other) and eik_idx hits S+X+1."""
-    E, S_, X, T = cfg["N_samples_eval"], cfg["N_samples"], cfg["N_samples_extra"], cfg["max_total_iters"]
-    g = torch.Generator().manual_seed(seed)
-    t_rand, u_final = torch.rand(R, E, generator=g), torch.rand(R, S_, generator=g)
-    if edges:
-        top = 1.0 - 2.0 ** -24
-        t_rand[:, 0::3] = 0.0
-        t_rand[:, 1::5] = top
-        u_final[:, 0::4] = 0.0
-        u_final[:, 1::4] = top
-    perm = torch.zeros(T, T * E, dtype=torch.int32)
-    for t in range(T):
-        perm[t, :(t + 1) * E] = torch.randperm((t + 1) * E, generator=g).to(torch.int32)
-    eik = torch.randint(S_ + X + 2, (T, R), generator=g, dtype=torch.int32)
-    if edges:
-        eik[:, 0::2] = S_ + X + 1
-    bg = torch.rand(T, R, 32, generator=g)
-    return dict(t_rand=t_rand, u_final=u_final, extra_perm=perm, eik_idx=eik, t_rand_bg=bg)
 
 
 def run(cfg, body, field, d, o, rng=None, ws=None, fill=None):

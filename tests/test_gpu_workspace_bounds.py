@@ -10,7 +10,6 @@ The MLP operator query (mp_mlp_workspace_bytes, and the MLP share of every layou
 of both engines and all their programs, because the engine can change between the query and the call.  Every call runs
 under both engines.  A call whose own layout is that largest one (the gradient chains, and every layout that nests the
 MLP query) is refused one byte less under at least one engine; any other call must write nothing past that byte."""
-import ctypes as C
 from contextlib import contextmanager
 
 import numpy as np
@@ -21,7 +20,10 @@ pytestmark = pytest.mark.gpu
 
 from multiply_b200 import engine, scene as S, _lib as L     # noqa: E402
 from multiply_b200.utils import mesh as umesh               # noqa: E402
-from test_gpu_workspace_reuse import geo, trained, _composite_inputs, _pts, P_C, R_C, N_C, BETA_C  # noqa: F401
+
+import _calls as calls                                                              # noqa: E402
+from _abi import same, sentinel, snap                                               # noqa: E402
+from _setups import Smpl, geo, points, posed_body, pts, train_rng, trained        # noqa: E402,F401
 
 TAIL = 4096 + 256
 SENT = 0xA5
@@ -83,36 +85,20 @@ def _release():
     placed.keep.clear()
 
 
-def _bits(v):
-    if not torch.is_tensor(v):
-        return v
-    v = v.detach().contiguous().reshape(-1)
-    return v.to(torch.uint8) if v.dtype == torch.bool else v.view(torch.uint8).clone()
-
-
-def _snap(out):
-    torch.cuda.synchronize()
-    return {k: _bits(v) for k, v in out.items()}
-
-
-def _equal(a, b):
-    return torch.equal(a, b) if torch.is_tensor(a) else a == b
-
-
 def check_bounds(monkeypatch, name, run, outs=dict, pos=-2, refuse=True):
     """name: the entry point, or a tuple of entry points that share one buffer.  run(o) makes the calls (``o = outs()``,
     output buffers filled with sentinels) and returns a dict of outputs.  refuse=False: the call may accept one byte
     less (see the module docstring).  Returns whether it refused."""
     names = name if isinstance(name, tuple) else (name,)
     with placed(monkeypatch, names, "generous", pos):
-        want = _snap(run(outs()))
+        want = snap(run(outs()))
     with placed(monkeypatch, names, "exact", pos) as seen:
-        got = _snap(run(outs()))
+        got = snap(run(outs()))
     assert seen, "%s was not called" % name
     for k in want:
-        assert _equal(want[k], got[k]), "%s: output %s differs with exactly the query's bytes" % (name, k)
+        assert same(want[k], got[k]), "%s: output %s differs with exactly the query's bytes" % (name, k)
     o = outs()
-    before = _snap(o)
+    before = snap(o)
     refused = True
     try:
         with placed(monkeypatch, names, "short", pos):
@@ -121,9 +107,9 @@ def check_bounds(monkeypatch, name, run, outs=dict, pos=-2, refuse=True):
     except L.MpError as e:
         assert "too small" in str(e), str(e)
     if refused:
-        after = _snap(o)
+        after = snap(o)
         for k in before:
-            assert _equal(before[k], after[k]), "%s: output %s written by a refused call" % (name, k)
+            assert same(before[k], after[k]), "%s: output %s written by a refused call" % (name, k)
     assert refused or not refuse, "%s accepted one byte less than its query" % name
     with pytest.raises(L.MpError, match="256-byte aligned"):
         with placed(monkeypatch, names, "misaligned", pos):
@@ -146,12 +132,15 @@ def check_engines(monkeypatch, name, run, outs=dict, need_refusal=True):
 
 def _full(shape, dtype=torch.float32):
     shape = shape if isinstance(shape, tuple) else (shape,)
-    v = -1234.5 if dtype.is_floating_point else (0xA5 if dtype == torch.uint8 else -7)
-    return torch.full(shape, v, dtype=dtype, device="cuda")
+    return torch.full(shape, sentinel(dtype), dtype=dtype, device="cuda")
 
 
-def _mlp_ws(N):
-    return L.workspace(L.call("mp_mlp_workspace_bytes", N), "cuda")
+def _case(case, x):
+    """check_bounds' (name, run, outs) for a call case on inputs x: sentinel-filled outputs, a workspace of the query's
+    bytes, and every output buffer compared whole."""
+    def run(o):
+        return {**case.call(x, o, L.workspace(case.query(), "cuda")), **o}
+    return case.name, run, lambda: {k: _full(shape, dtype) for k, (shape, dtype) in case.outs.items()}
 
 
 # ---------------------------------------------------------------------------------------------
@@ -164,31 +153,17 @@ EDGES = [1, 127, 129, 32767, 32769]
 @pytest.mark.parametrize("N", EDGES)
 @pytest.mark.parametrize("grad", [False, True])
 def test_implicit_forward_bounds(monkeypatch, trained, N, grad):
-    f = trained[1][0]
-    x = _pts(N, 3, 10 + N)
-    name = "mp_implicit_forward_grad" if grad else "mp_implicit_forward"
-
-    def outs():
-        return dict(sdf=_full(N), feat=_full((N, 256)), grad=_full((N, 3)))
-
-    def run(o):
-        ws = _mlp_ws(N)
-        if grad:
-            L.call(name, f.handle, x, N, o["sdf"], o["feat"], o["grad"], ws, ws.numel())
-        else:
-            L.call(name, f.handle, x, N, o["sdf"], o["feat"], ws, ws.numel())
-        return o
-
-    check_engines(monkeypatch, name, run, outs, need_refusal=grad)
+    c = calls.implicit_forward(trained[1][0], N, grad)
+    check_engines(monkeypatch, *_case(c, c.inputs(10 + N)), need_refusal=grad)
 
 
 @pytest.mark.parametrize("N", [1, 129, 65537])
 def test_render_forward_bounds(monkeypatch, trained, N):
     f = trained[1][0]
-    x, nrm, feat = _pts(N, 3, 1), _pts(N, 3, 2), _pts(N, 256, 3)
+    x, nrm, feat = pts(N, 3, 1), pts(N, 3, 2), pts(N, 256, 3)
 
     def run(o):
-        ws = _mlp_ws(N)
+        ws = L.workspace(L.call("mp_mlp_workspace_bytes", N), "cuda")
         L.call("mp_render_forward", f.handle, x, nrm, feat, N, o["rgb"], ws, ws.numel())
         return o
 
@@ -197,38 +172,22 @@ def test_render_forward_bounds(monkeypatch, trained, N):
 
 @pytest.mark.parametrize("N", [1, 127, 129])
 def test_bg_nets_forward_bounds(monkeypatch, trained, N):
-    bg = trained[2]
-    pts, view = _pts(N, 4, 5), _pts(N, 3, 6)
-    view = (view / view.norm(dim=1, keepdim=True)).contiguous()
-
-    def run(o):
-        ws = _mlp_ws(N)
-        L.call("mp_bg_nets_forward", bg.handle, pts, view, N, o["sdf"], o["rgb"], ws, ws.numel())
-        return o
-
-    check_engines(monkeypatch, "mp_bg_nets_forward", run, lambda: dict(sdf=_full(N), rgb=_full((N, 3))),
-                  need_refusal=False)
+    c = calls.bg_nets_forward(trained[2], N)
+    check_engines(monkeypatch, *_case(c, c.inputs(5)), need_refusal=False)
 
 
 @pytest.mark.parametrize("res", [8, 101])
 def test_sdf_grid_bounds(monkeypatch, trained, res):
     """res 101: (res + 1)^3 > 2^20, two slabs."""
     sc, fields, _ = trained
-    center, extent, pad = umesh.bounds(sc["persons"][0]["verts_c"])
-
-    def run(o):
-        ws = L.workspace(L.call("mp_sdf_grid_workspace_bytes", res), "cuda")
-        L.call("mp_sdf_grid", fields[0].handle, L.vec3(C.c_float, center), float(extent), float(pad), res, o["v"], ws,
-               ws.numel())
-        return o
-
-    check_engines(monkeypatch, "mp_sdf_grid", run, lambda: dict(v=_full((res + 1) ** 3)))
+    c = calls.sdf_grid(sc, fields, res)
+    check_engines(monkeypatch, *_case(c, c.inputs(0)))
 
 
 @pytest.mark.parametrize("N", [1, 129, 32769])
 def test_sdf_with_deformer_bounds(monkeypatch, geo, N):
     sc, f, body = geo
-    x = _pts(N, 3, 7, -0.8, 0.8)
+    x = pts(N, 3, 7, -0.8, 0.8)
 
     def run(o):
         ws = L.workspace(L.call("mp_sdf_with_deformer_workspace_bytes", N), "cuda")
@@ -241,17 +200,8 @@ def test_sdf_with_deformer_bounds(monkeypatch, geo, N):
 
 @pytest.mark.parametrize("R", [1, 301])
 def test_background_bounds(monkeypatch, trained, R):
-    bg = trained[2]
-    d = _pts(R, 3, 8)
-    d = (d / d.norm(dim=1, keepdim=True)).contiguous()
-    c = _pts(R, 3, 9, -1.5, 1.5)
-
-    def run(o):
-        ws = L.workspace(L.call("mp_background_workspace_bytes", R), "cuda")
-        L.call("mp_background", bg.handle, d, c, R, 3.0, o["rgb"], ws, ws.numel())
-        return o
-
-    check_engines(monkeypatch, "mp_background", run, lambda: dict(rgb=_full((R, 3))))
+    c = calls.background(trained[2], R)
+    check_engines(monkeypatch, *_case(c, c.inputs(8)))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -261,109 +211,31 @@ def test_background_bounds(monkeypatch, trained, R):
 @pytest.mark.parametrize("R", [1, 129])
 @pytest.mark.parametrize("train", [False, True])
 def test_sample_rays_bounds(monkeypatch, geo, R, train):
-    from test_gpu_sampler import rays, train_rng
     sc, f, body = geo
-    cfg = dict(sc["cfg"], beta_param=sc["beta_param"])
-    c = engine.sampler_cfg(cfg, cfg["beta_param"])
-    n = cfg["N_samples"] + cfg["N_samples_extra"] + 2
-    d, o_ = (t.cuda() for t in rays(sc, R, seed=4))
-    rng, keep = engine.sampler_rng_struct(train_rng(cfg, R, seed=4), torch.device("cuda"))
-    name = "mp_sample_rays_train" if train else "mp_sample_rays"
-
-    def outs():
-        return dict(z=_full((R, n)), z_bg=_full((R, 32)), z_eik=_full(R), trips=_full(1, torch.int32))
-
-    def run(o):
-        ws = L.workspace(L.call("mp_sampler_workspace_bytes", c, R), "cuda")
-        if train:
-            L.call(name, c, body.handle, f.handle, d, o_, R, rng, o["z"], o["z_bg"], o["z_eik"], o["trips"], ws,
-                   ws.numel())
-        else:
-            L.call(name, c, body.handle, f.handle, d, o_, R, o["z"], o["z_bg"], o["trips"], ws, ws.numel())
-        return o
-
-    check_engines(monkeypatch, name, run, outs)
+    c = calls.sample_rays(sc, f, body, R, train)
+    check_engines(monkeypatch, *_case(c, c.inputs(4)))
 
 
 def test_composite_bounds(monkeypatch):
-    x = _composite_inputs(11)
-
-    def outs():
-        return dict(fg=_full((R_C, 3)), nrm=_full((R_C, 3)), acc=_full(R_C), accp=_full((R_C, P_C)), bgT=_full(R_C))
-
-    def run(o):
-        ws = L.workspace(L.call("mp_composite_workspace_bytes", R_C, P_C), "cuda")
-        L.call("mp_composite", x["arr"], P_C, R_C, N_C, BETA_C, o["fg"], o["nrm"], o["acc"], o["accp"], o["bgT"], ws,
-               ws.numel())
-        return o
-
-    check_bounds(monkeypatch, "mp_composite", run, outs)
+    c = calls.composite()
+    check_bounds(monkeypatch, *_case(c, c.inputs(11)))
 
 
 def test_composite_backward_bounds(monkeypatch):
-    x = _composite_inputs(12)
-    u = x["ups"]
-
-    def outs():
-        o = dict(d_beta=_full(1))
-        for p in range(P_C):
-            for k in ("sdf", "rgb", "nrm"):
-                o["%s%d" % (k, p)] = _full((R_C, N_C, 3 if k != "sdf" else 1))
-        return o
-
-    def run(o):
-        gr = (L.PersonSampleGrads * P_C)()
-        for p in range(P_C):
-            gr[p].d_sdf, gr[p].d_rgb, gr[p].d_normal = (L.ptr(o["%s%d" % (k, p)]) for k in ("sdf", "rgb", "nrm"))
-        ws = L.workspace(L.call("mp_composite_backward_workspace_bytes", R_C, P_C), "cuda")
-        L.call("mp_composite_backward", x["arr"], P_C, R_C, N_C, BETA_C, u["d_fg"], u["d_nrm"], u["d_acc"], u["d_accp"],
-               u["d_bgT"], gr, o["d_beta"], ws, ws.numel())
-        return o
-
-    check_bounds(monkeypatch, "mp_composite_backward", run, outs)
+    c = calls.composite_backward()
+    check_bounds(monkeypatch, *_case(c, c.inputs(12)))
 
 
 def test_smpl_backward_bounds(monkeypatch):
-    from test_gpu_body_grad import Smpl
-    sm = Smpl(S.make_smpl_model(300))
-    rng = np.random.RandomState(1)
-    args = Smpl._args(1.05, rng.normal(0, 0.3, 3), rng.normal(0, 0.4, 72), rng.normal(0, 1, 10))
-    dv = torch.from_numpy(rng.standard_normal((sm.V, 3)).astype(np.float32)).cuda()
-    dt = torch.from_numpy(rng.standard_normal((24, 4, 4)).astype(np.float32)).cuda()
-
-    def run(o):
-        ws = L.workspace(L.call("mp_smpl_backward_workspace_bytes", sm.V), "cuda")
-        L.call("mp_smpl_backward", sm.h, *args, 0, dv, dt, o["scale"], o["transl"], o["thetas"], o["betas"], ws,
-               ws.numel())
-        return o
-
-    check_bounds(monkeypatch, "mp_smpl_backward", run,
-                 lambda: dict(scale=_full(1), transl=_full(3), thetas=_full(72), betas=_full(10)))
+    c = calls.smpl_backward(Smpl(S.make_smpl_model(300)))
+    check_bounds(monkeypatch, *_case(c, c.inputs(1)))
 
 
 @pytest.mark.parametrize("N", [1, 4097])
 def test_deform_backward_bounds(monkeypatch, N):
-    from test_gpu_body_grad import _points, _posed_body
-    body, _ = _posed_body()
-    p = _points(N, body.verts_p, 71).cuda()
-    u = torch.from_numpy(np.random.RandomState(1).randn(N, 3).astype(np.float32)).cuda()
-    uj = torch.from_numpy(np.random.RandomState(2).randn(N, 9).astype(np.float32)).cuda()
-
-    def outs():
-        return dict(d_tfs=_full((24, 4, 4)), d_x=_full((N, 3)), xc=_full((N, 3)))
-
-    def run_inv(o):
-        ws = L.workspace(L.call("mp_deform_backward_workspace_bytes", N), "cuda")
-        L.call("mp_deform_inverse_backward", body.handle, p, N, 1, u, o["d_tfs"], o["d_x"], o["xc"], ws, ws.numel())
-        return o
-
-    def run_fwd(o):
-        ws = L.workspace(L.call("mp_deform_backward_workspace_bytes", N), "cuda")
-        L.call("mp_deform_forward_jac_backward", body.handle, p, N, u, uj, o["d_tfs"], o["d_x"], ws, ws.numel())
-        return o
-
-    check_bounds(monkeypatch, "mp_deform_inverse_backward", run_inv, outs)
-    check_bounds(monkeypatch, "mp_deform_forward_jac_backward", run_fwd, outs)
+    body, _ = posed_body()
+    for c in (calls.deform_inverse_backward(body, N), calls.deform_forward_jac_backward(body, N)):
+        check_bounds(monkeypatch, *_case(c, c.inputs(71)))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -373,17 +245,8 @@ def test_deform_backward_bounds(monkeypatch, N):
 @pytest.mark.parametrize("res_init,depth", [(4, 1), (16, 2)])
 def test_mise_bounds(monkeypatch, trained, res_init, depth):
     sc, fields, _ = trained
-    center, extent, pad = umesh.bounds(sc["persons"][0]["verts_c"])
-    n1 = (res_init << depth) + 1
-
-    def run(o):
-        n = C.c_longlong(0)
-        ws = L.workspace(L.call("mp_mise_workspace_bytes", res_init, depth), "cuda")
-        L.call("mp_mise", fields[0].handle, L.vec3(C.c_float, center), float(extent), float(pad), res_init, depth, 0.0,
-               o["grid"], o["ev"], C.byref(n), ws, ws.numel())
-        return dict(o, n=n.value)
-
-    check_engines(monkeypatch, "mp_mise", run, lambda: dict(grid=_full(n1 ** 3), ev=_full(n1 ** 3, torch.uint8)))
+    c = calls.mise(sc, fields, res_init, depth)
+    check_engines(monkeypatch, *_case(c, c.inputs(0)))
 
 
 @pytest.fixture(scope="module")
@@ -397,33 +260,15 @@ def grid64(trained):
 
 def test_marching_cubes_bounds(monkeypatch, grid64):
     """Count and emit share one workspace (emit reads the count's offsets)."""
-    R = grid64.shape[0] - 1
     v0, f0 = engine.marching_cubes(grid64, 0.0)
-    V, F = v0.shape[0], f0.shape[0]
-
-    def run(o):
-        ws = L.workspace(L.call("mp_marching_cubes_workspace_bytes", R), "cuda")
-        nv, nf = C.c_longlong(0), C.c_longlong(0)
-        L.call("mp_marching_cubes_count", grid64, R, 0.0, C.byref(nv), C.byref(nf), ws, ws.numel())
-        L.call("mp_marching_cubes_emit", grid64, R, 0.0, L.vec3(C.c_double, (R / 2.0,) * 3), float(R), 1.0, o["v"],
-               o["f"], ws, ws.numel())
-        return dict(o, V=nv.value, F=nf.value)
-
-    check_bounds(monkeypatch, ("mp_marching_cubes_count", "mp_marching_cubes_emit"), run,
-                 lambda: dict(v=_full(3 * V), f=_full(3 * F, torch.int64)))
+    c = calls.marching_cubes(grid64.shape[0] - 1, v0.shape[0], f0.shape[0])
+    check_bounds(monkeypatch, *_case(c, grid64))
 
 
 def test_largest_component_bounds(monkeypatch, grid64):
     v, f = engine.marching_cubes(grid64, 0.0)
-    V, F = v.shape[0], f.shape[0]
-
-    def run(o):
-        ws = L.workspace(L.call("mp_largest_component_workspace_bytes", V, F), "cuda")
-        nv, nf = C.c_int(0), C.c_int(0)
-        L.call("mp_largest_component", v, V, f, F, o["v"], o["f"], C.byref(nv), C.byref(nf), ws, ws.numel())
-        return dict(o, V=nv.value, F=nf.value)
-
-    check_bounds(monkeypatch, "mp_largest_component", run, lambda: dict(v=_full(3 * V), f=_full(3 * F, torch.int64)))
+    c = calls.largest_component(v.shape[0], f.shape[0])
+    check_bounds(monkeypatch, *_case(c, (v, f)))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -432,8 +277,7 @@ def test_largest_component_bounds(monkeypatch, grid64):
 
 def test_body_storage_bounds(monkeypatch, trained):
     p = trained[0]["persons"][1]
-    from test_gpu_body_grad import _points
-    x = _points(4097, p["verts_p"], 90).cuda()
+    x = points(4097, p["verts_p"], 90).cuda()
 
     def run(o):
         b = engine.Body(p["verts_c"], p["weights"], cano_cell=0.1001 / p["scale"])
@@ -445,7 +289,6 @@ def test_body_storage_bounds(monkeypatch, trained):
 
 
 def test_smpl_storage_bounds(monkeypatch):
-    from test_gpu_body_grad import Smpl
     model = S.make_smpl_model(301)
     rng = np.random.RandomState(4)
     args = (1.1, rng.normal(0, 0.3, 3), rng.normal(0, 0.4, 72), rng.normal(0, 1, 10))
@@ -495,13 +338,12 @@ def test_zero_size_calls_take_the_query_with_a_null_buffer(trained, geo):
     """At N = 0 the deformer backward's layout is empty: its query answers 0 and the call takes (NULL, 0), still
     writing d_tfs = 0.  The calls that return before their carve at a zero size take (NULL, their query) as well, and
     write nothing."""
-    from test_gpu_body_grad import _posed_body
-    body, _ = _posed_body()
+    body, _ = posed_body()
     assert L.call("mp_deform_backward_workspace_bytes", 0) == 0
     for P in (1, 3):
         assert L.call("mp_composite_workspace_bytes", 0, P) == 0
         assert L.call("mp_composite_backward_workspace_bytes", 0, P) == 0
-    one, u = _pts(1, 3, 1), _pts(1, 9, 2)
+    one, u = pts(1, 3, 1), pts(1, 9, 2)
     for name, args in (("mp_deform_inverse_backward", (body.handle, None, 0, 1, None)),
                        ("mp_deform_forward_jac_backward", (body.handle, None, 0, None, None))):
         d_tfs = _full((24, 4, 4))
@@ -549,7 +391,6 @@ def render_setup():
 
 @pytest.mark.parametrize("mode", ["eval", "device_counts", "train", "train_meshes"])
 def test_render_rays_bounds(monkeypatch, render_setup, mode):
-    from test_gpu_sampler import train_rng
     sc, r, inp, hits, meshes = render_setup
     R = inp["uv"].shape[1]
     hl = [h.cuda() for h in hits]
