@@ -214,6 +214,9 @@ __device__ __forceinline__ void nearest_vertex(const GridHeader& g, const int* _
     best = INFINITY;
     bi = 0x7fffffff;
     for (int j = 0; j < V; ++j) nn_consider(__ldg(&sorted[j]), px, py, pz, best, bi);
+    // no finite distance (a non-finite coordinate, or every squared distance overflows): no nearest vertex, rather
+    // than the lowest index of a tie at infinity
+    if (!(best < INFINITY)) bi = 0x7fffffff;
   }
 }
 
@@ -282,23 +285,33 @@ __global__ void vertex_tf_kernel(const float* __restrict__ weights, const float*
 // closed-form inverse with J^-1 = the inverse blended 3x3 at the start point (the weights are detached, so that IS the
 // Jacobian inside a Voronoi cell), rank-one "good Broyden" updates of J^-1 (Sherman-Morrison), lowest-residual
 // iterate kept.  The reference has no such step (SURVEY.md fact 0-1); parity is against oracle/port.py:deform_broyden.
-__device__ __forceinline__ void skin_forward_point(const Body& b, const GridHeader& gc, const float x[3], float f[3],
+// Returns false, leaving f untouched, when x has no nearest vertex (a non-finite coordinate, or every fp32 squared
+// distance overflows): such a point has no skinning weights.
+__device__ __forceinline__ bool skin_forward_point(const Body& b, const GridHeader& gc, const float x[3], float f[3],
                                                    int& vi) {
   float d2;
   nearest_vertex(gc, b.cano_cell_start, b.cano_sorted, b.V, x[0], x[1], x[2], true, d2, vi);
+  if (vi == 0x7fffffff) return false;
   float T[12], s;
   blend_tf(b.weights + (size_t)vi * MP_NUM_JOINTS, b.tfs, T, s);
   f[0] = fmaf(T[0], x[0], fmaf(T[1], x[1], fmaf(T[2], x[2], T[3])));
   f[1] = fmaf(T[4], x[0], fmaf(T[5], x[1], fmaf(T[6], x[2], T[7])));
   f[2] = fmaf(T[8], x[0], fmaf(T[9], x[1], fmaf(T[10], x[2], T[11])));
+  return true;
 }
 
+// An iterate without a nearest vertex ends the iteration: the best iterate so far and its residual are returned and
+// `steps` counts the steps taken.  A start without one is returned as it is, with a NaN residual and no step.
 __device__ __noinline__ void broyden_refine(const Body& b, float px, float py, float pz, int max_steps, float thr,
                                             float xc[3], float& resid, int& steps) {
   const GridHeader gc = *b.cano_hdr;
   float x[3] = {xc[0], xc[1], xc[2]}, f[3], g[3];
   int vi;
-  skin_forward_point(b, gc, x, f, vi);
+  steps = 0;
+  if (!skin_forward_point(b, gc, x, f, vi)) {
+    resid = __int_as_float(0x7fffffff);
+    return;
+  }
   g[0] = f[0] - px;
   g[1] = f[1] - py;
   g[2] = f[2] - pz;
@@ -310,14 +323,16 @@ __device__ __noinline__ void broyden_refine(const Body& b, float px, float py, f
     Ji[8] = r2.z;
   }
   float best = sqrtf(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
-  steps = 0;
   for (int k = 0; k < max_steps && best >= thr; ++k) {
     float dx[3], gn[3], dg[3], u[3], vt[3];
 #pragma unroll
     for (int r = 0; r < 3; ++r) dx[r] = -(Ji[3 * r] * g[0] + Ji[3 * r + 1] * g[1] + Ji[3 * r + 2] * g[2]);
 #pragma unroll
     for (int r = 0; r < 3; ++r) x[r] += dx[r];
-    skin_forward_point(b, gc, x, f, vi);
+    if (!skin_forward_point(b, gc, x, f, vi)) {
+      steps = k + 1;
+      break;
+    }
     gn[0] = f[0] - px;
     gn[1] = f[1] - py;
     gn[2] = f[2] - pz;
@@ -486,16 +501,24 @@ __global__ void deform_forward_jac_kernel(Body b, const float* __restrict__ x_c,
   float d2;
   int vi;
   nearest_vertex(g, b.cano_cell_start, b.cano_sorted, b.V, px, py, pz, true, d2, vi);
+  const bool none = vi == 0x7fffffff;   // no nearest vertex (non-finite or overflowing x_c): x_d and J^-1 are NaN
+  const float nan = __int_as_float(0x7fffffff);
   if (x_d) {
-    float T[12], s;
-    blend_tf(b.weights + (size_t)vi * MP_NUM_JOINTS, b.tfs, T, s);
-    x_d[3 * i] = T[0] * px + T[1] * py + T[2] * pz + T[3];
-    x_d[3 * i + 1] = T[4] * px + T[5] * py + T[6] * pz + T[7];
-    x_d[3 * i + 2] = T[8] * px + T[9] * py + T[10] * pz + T[11];
+    if (none) {
+      x_d[3 * i] = x_d[3 * i + 1] = x_d[3 * i + 2] = nan;
+    } else {
+      float T[12], s;
+      blend_tf(b.weights + (size_t)vi * MP_NUM_JOINTS, b.tfs, T, s);
+      x_d[3 * i] = T[0] * px + T[1] * py + T[2] * pz + T[3];
+      x_d[3 * i + 1] = T[4] * px + T[5] * py + T[6] * pz + T[7];
+      x_d[3 * i + 2] = T[8] * px + T[9] * py + T[10] * pz + T[11];
+    }
   }
   if (Jinv) {
-    const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
-                 r2 = __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
+    const float4 nan4 = make_float4(nan, nan, nan, nan);
+    const float4 r0 = none ? nan4 : __ldg(&b.vert_tf[3 * (size_t)vi]),
+                 r1 = none ? nan4 : __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
+                 r2 = none ? nan4 : __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
     if (jstride == 12) {   // padded rows: three 128-bit stores
       float4* o = reinterpret_cast<float4*>(Jinv + 12 * (size_t)i);
       o[0] = make_float4(r0.x, r0.y, r0.z, r1.x);
@@ -637,39 +660,43 @@ __global__ void __launch_bounds__(kBgThreads) deform_forward_jac_backward_kernel
       float d2;
       int vi;
       nearest_vertex(g, b.cano_cell_start, b.cano_sorted, b.V, px, py, pz, true, d2, vi);
-      w = b.weights + (size_t)vi * MP_NUM_JOINTS;
-      float dxc[3] = {0.f, 0.f, 0.f};
-      if (d_xd) {
-        const float gx = d_xd[3 * i], gy = d_xd[3 * i + 1], gz = d_xd[3 * i + 2];
-        const float gg[3] = {gx, gy, gz}, xh[4] = {px, py, pz, 1.f};
-        float T[12], s;
-        blend_tf(w, b.tfs, T, s);
+      if (vi == 0x7fffffff) {   // no nearest vertex: d_x_c is NaN and nothing goes to the bones (w stays null)
+        if (d_xc) d_xc[3 * i] = d_xc[3 * i + 1] = d_xc[3 * i + 2] = __int_as_float(0x7fffffff);
+      } else {
+        w = b.weights + (size_t)vi * MP_NUM_JOINTS;
+        float dxc[3] = {0.f, 0.f, 0.f};
+        if (d_xd) {
+          const float gx = d_xd[3 * i], gy = d_xd[3 * i + 1], gz = d_xd[3 * i + 2];
+          const float gg[3] = {gx, gy, gz}, xh[4] = {px, py, pz, 1.f};
+          float T[12], s;
+          blend_tf(w, b.tfs, T, s);
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
+          for (int r = 0; r < 3; ++r)
 #pragma unroll
-          for (int c = 0; c < 4; ++c) dA[4 * r + c] = gg[r] * xh[c];
+            for (int c = 0; c < 4; ++c) dA[4 * r + c] = gg[r] * xh[c];
 #pragma unroll
-        for (int c = 0; c < 3; ++c) dxc[c] = T[c] * gx + T[4 + c] * gy + T[8 + c] * gz;
-      }
-      if (d_Jinv) {
-        const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
-                     r2 = __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
-        const float I[9] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z};
-        const float* dJ = d_Jinv + 9 * (size_t)i;
-        float H[9];   // d_Jinv Jinv^T
+          for (int c = 0; c < 3; ++c) dxc[c] = T[c] * gx + T[4 + c] * gy + T[8 + c] * gz;
+        }
+        if (d_Jinv) {
+          const float4 r0 = __ldg(&b.vert_tf[3 * (size_t)vi]), r1 = __ldg(&b.vert_tf[3 * (size_t)vi + 1]),
+                       r2 = __ldg(&b.vert_tf[3 * (size_t)vi + 2]);
+          const float I[9] = {r0.x, r0.y, r0.z, r1.x, r1.y, r1.z, r2.x, r2.y, r2.z};
+          const float* dJ = d_Jinv + 9 * (size_t)i;
+          float H[9];   // d_Jinv Jinv^T
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
+          for (int r = 0; r < 3; ++r)
 #pragma unroll
-          for (int c = 0; c < 3; ++c) H[3 * r + c] = dJ[3 * r] * I[3 * c] + dJ[3 * r + 1] * I[3 * c + 1] + dJ[3 * r + 2] * I[3 * c + 2];
+            for (int c = 0; c < 3; ++c) H[3 * r + c] = dJ[3 * r] * I[3 * c] + dJ[3 * r + 1] * I[3 * c + 1] + dJ[3 * r + 2] * I[3 * c + 2];
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
+          for (int r = 0; r < 3; ++r)
 #pragma unroll
-          for (int c = 0; c < 3; ++c) dA[4 * r + c] -= I[r] * H[c] + I[3 + r] * H[3 + c] + I[6 + r] * H[6 + c];
-      }
-      if (d_xc) {
-        d_xc[3 * i] = dxc[0];
-        d_xc[3 * i + 1] = dxc[1];
-        d_xc[3 * i + 2] = dxc[2];
+            for (int c = 0; c < 3; ++c) dA[4 * r + c] -= I[r] * H[c] + I[3 + r] * H[3 + c] + I[6 + r] * H[6 + c];
+        }
+        if (d_xc) {
+          d_xc[3 * i] = dxc[0];
+          d_xc[3 * i + 1] = dxc[1];
+          d_xc[3 * i + 2] = dxc[2];
+        }
       }
     }
     bone_grad_warp<3>(w, dA, acc[warp], lane);
@@ -807,10 +834,9 @@ int mp_body_set_root_finder(mp_body_t* h, int max_steps, float cvg_threshold) {
 int mp_deform_broyden(mp_body_t* h, const float* x, int N, int max_steps, float cvg_threshold, float* x_c,
                       float* residual, uint8_t* converged, uint8_t* outlier, int* steps, void* stream) {
   MP_REQUIRE(h && h->b.tfs, "mp_deform_broyden: body has no pose (call mp_body_set_pose)");
-  MP_REQUIRE(x_c, "mp_deform_broyden: null output");
   MP_REQUIRE(max_steps >= 0 && max_steps <= 64 && cvg_threshold > 0.f, "mp_deform_broyden: bad iteration limits");
-  if (N <= 0) return 0;
-  MP_REQUIRE(x, "mp_deform_broyden: null input");
+  if (N <= 0) return 0;   // nothing is read or written: every buffer may be null
+  MP_REQUIRE(x && x_c, "mp_deform_broyden: null input or output");
   mp::deform_broyden_kernel<<<mp::div_up(N, 128), 128, 0, (cudaStream_t)stream>>>(
       h->b, x, N, max_steps, cvg_threshold, x_c, residual, converged, outlier, steps);
   MP_LAUNCH_CHECK();
