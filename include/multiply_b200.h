@@ -424,6 +424,47 @@ int mp_mesh_surface_flags(const mp_mesh_t* mesh, const float* x_c, int rows, int
                           uint8_t* in, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * posed-mesh depth maps and the nearest partner vertex: the pytorch3d operators of opt_depth's geometric losses,
+ * Renderer.render_multiple_depth_map (lib/model/render.py:135-157, layer 0 of zbuf, multiply_model.py:396-401) and
+ * pytorch3d.ops.knn_points(K=1, return_nn=True) (multiply_model.py:539).  Definitions: oracle/raster.py and
+ * oracle/port.py:knn_points (DESIGN §3.8).  Backward sums are stable sorts by vertex, each vertex summing its terms in
+ * a fixed order in fp64 (no float atomics): reruns are bit-identical.  Every output element is written.
+ * ---------------------------------------------------------------------------------------- */
+/* The camera of Renderer.set_camera in OpenCV's convention (the flips of render.py:73-78 cancel): (X, Y, Z) = R v + T,
+ * u = fx X / Z + cx, v = fy Y / Z + cy; fx, fy, cx, cy = K[0,0], K[1,1], K[0,2], K[1,2] of cv2's decomposition. */
+typedef struct {
+  float R[9];              /* world -> camera rotation, row-major */
+  float T[3];
+  float fx, fy, cx, cy;
+} mp_camera_t;
+/* verts [V,3] fp32, faces [F,3] int64 -> zbuf [H,W] (view-space depth of the nearest covering face, -1 where none) and
+ * pix_to_face [H,W] int64 (its index, -1 where none).  Pixel (r, c) samples the image point (c + 0.5, r + 0.5); a face
+ * covers it when the point lies in the closed projected triangle; depth z = 1 / sum_i(b_i / Z_i) (perspective-correct,
+ * fp64 on the fp32 inputs, rounded to fp32 once); the nearest fp32 depth wins, then the lowest face index.  Faces with a
+ * vertex at Z <= 0, of zero projected area, or with an index outside [0, V) are skipped.  Needs H, W >= 1, V, F >= 0. */
+size_t mp_depth_raster_workspace_bytes(int H, int W, int F);
+int mp_depth_raster(const mp_camera_t* cam_host, const float* verts, int V, const int64_t* faces, int F, int H, int W,
+                    float* zbuf, int64_t* pix_to_face, void* workspace, size_t workspace_bytes, void* stream);
+/* d_verts [V,3] = sum over pixels of d_zbuf [H,W] times the exact derivative of the pixel's z with respect to its face's
+ * world-space vertices, the face (pix_to_face, as mp_depth_raster wrote it) held fixed; vertices no such face touches
+ * get 0. */
+size_t mp_depth_raster_backward_workspace_bytes(int H, int W, int V);
+int mp_depth_raster_backward(const mp_camera_t* cam_host, const float* verts, int V, const int64_t* faces, int F, int H,
+                             int W, const int64_t* pix_to_face, const float* d_zbuf, float* d_verts, void* workspace,
+                             size_t workspace_bytes, void* stream);
+/* p1 [N1,3], p2 [N2,3] fp32 (N2 >= 1) -> dists [N1] = min_j (dx*dx + dy*dy) + dz*dz (fp32, each step rounded), idx [N1]
+ * int64 the arg-min (lowest index on ties), nn [N1,3] = p2[idx]; any output may be NULL (not written).  Finite inputs. */
+size_t mp_knn1_workspace_bytes(int N1);
+int mp_knn1(const float* p1, int N1, const float* p2, int N2, float* dists, int64_t* idx, float* nn, void* workspace,
+            size_t workspace_bytes, void* stream);
+/* Backward of mp_knn1 at its idx: d_dists [N1] and d_nn [N1,3] may be NULL (zero).  d_p1 [N1,3] = 2 (p1 - nn) d_dists;
+ * d_p2 [N2,3] = sum over the queries i with idx[i] = j of d_nn[i] - 2 (p1 - nn) d_dists[i]. */
+size_t mp_knn1_backward_workspace_bytes(int N1, int N2);
+int mp_knn1_backward(const float* p1, int N1, const float* p2, int N2, const int64_t* idx, const float* d_dists,
+                     const float* d_nn, float* d_p1, float* d_p2, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * mesh extraction: lib/utils/mesh.py:generate_mesh (:78-132) — MISE, marching cubes, largest component (DESIGN §3.7).
  * Grids are [(R+1)^3] fp32, x-major: value (ix, iy, iz) at (ix*(R+1) + iy)*(R+1) + iz, as mp_sdf_grid writes them.
  * ---------------------------------------------------------------------------------------- */

@@ -76,6 +76,11 @@ class MeshPlan(C.Structure):
                 ("n_refs", C.c_longlong), ("storage_bytes", C.c_size_t)]
 
 
+class Camera(C.Structure):
+    _fields_ = [("R", C.c_float * 9), ("T", C.c_float * 3), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float),
+                ("cy", C.c_float)]
+
+
 class Scene(C.Structure):
     _fields_ = [("sampler", SamplerCfg), ("P", C.c_int),
                 ("body", C.c_void_p * MP_MAX_PERSONS), ("field", C.c_void_p * MP_MAX_PERSONS),
@@ -175,6 +180,14 @@ SIGNATURES = {
     "mp_mesh_distance": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, STREAM]),
     "mp_mesh_check_sign": (STATUS, [_VP, _VP, _I, _VP, STREAM]),
     "mp_mesh_surface_flags": (STATUS, [_VP, _VP, _I, _I, _F, _VP, _VP, STREAM]),
+    "mp_depth_raster_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mp_depth_raster": (STATUS, [C.POINTER(Camera), _VP, _I, _VP, _I, _I, _I, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_depth_raster_backward_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "mp_depth_raster_backward": (STATUS, [C.POINTER(Camera), _VP, _I, _VP, _I, _I, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_knn1_workspace_bytes": (_SZ, [_I]),
+    "mp_knn1": (STATUS, [_VP, _I, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_knn1_backward_workspace_bytes": (_SZ, [_I, _I]),
+    "mp_knn1_backward": (STATUS, [_VP, _I, _VP, _I, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_mise_workspace_bytes": (_SZ, [_I, _I]),
     "mp_mise": (STATUS, [_VP, c_float_p, _F, _F, _I, _I, C.c_double, _VP, _VP, C.POINTER(C.c_longlong), _VP, _SZ,
                          STREAM]),

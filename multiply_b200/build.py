@@ -19,10 +19,12 @@ COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 # reference-semantics kernels: keep a*a + b*b as two roundings (see sampler.cu header).  mesh.cu too: its fp64
 # closest-point and crossing arithmetic must round step by step as the CPU definitions' (oracle/mesh_port.py) do, so that
 # distance types, tie-breaks and crossing parities agree exactly; mesh_extract.cu for the same reason (vertex
-# positions, the asymptotic decider and component areas against oracle/mesh_extract.py)
-NO_FMAD = {"sampler.cu", "composite.cu", "rays.cu", "background.cu", "deform.cu", "mesh.cu", "mesh_extract.cu"}
+# positions, the asymptotic decider and component areas against oracle/mesh_extract.py); raster.cu for the same reason
+# (projections, inside tests and depths against oracle/raster.py, distances against oracle/port.py:knn_points)
+NO_FMAD = {"sampler.cu", "composite.cu", "rays.cu", "background.cu", "deform.cu", "mesh.cu", "mesh_extract.cu",
+           "raster.cu"}
 SOURCES = ["host_util.cu", "rays.cu", "deform.cu", "mlp_pack.cu", "mlp_simt.cu", "mlp_tc.cu", "sampler.cu",
-           "composite.cu", "background.cu", "render.cu", "smpl.cu", "mesh.cu", "mesh_extract.cu"]
+           "composite.cu", "background.cu", "render.cu", "smpl.cu", "mesh.cu", "mesh_extract.cu", "raster.cu"]
 
 
 def _nvcc():

@@ -307,6 +307,88 @@ class CanonicalMesh:
             return off.bool(), ins.bool()
 
 
+def camera(R, T, fx, fy, cx, cy):
+    """mp_camera_t of a world-to-camera R [3,3], T [3] (OpenCV convention) and the intrinsics, all rounded to fp32."""
+    c = L.Camera()
+    c.R[:] = [float(x) for x in np.asarray(R, dtype=np.float32).reshape(9)]
+    c.T[:] = [float(x) for x in np.asarray(T, dtype=np.float32).reshape(3)]
+    c.fx, c.fy, c.cx, c.cy = (float(np.float32(x)) for x in (fx, fy, cx, cy))
+    return c
+
+
+class DepthRaster(torch.autograd.Function):
+    """Layer 0 of pytorch3d's hard rasteriser (render.py:135-157) as one autograd node (mp_depth_raster): input verts
+    [V,3] (any device; faces [F,3] and the camera are constants), outputs zbuf [H,W] fp32 (-1 where no face covers the
+    pixel) and pix_to_face [H,W] int64 (not differentiable), on the device of ``device``.  The backward
+    (mp_depth_raster_backward) holds each pixel's face fixed and returns d verts."""
+
+    @staticmethod
+    def forward(ctx, cam, H, W, device, verts, faces):
+        dev = torch.device(device)
+        with torch.cuda.device(dev):
+            v = L.dev(verts.reshape(-1, 3), dev)
+            f = L.dev(faces.reshape(-1, 3), dev, torch.int64)
+            V, F = v.shape[0], f.shape[0]
+            ws = L.workspace(L.call("mp_depth_raster_workspace_bytes", H, W, F), dev)
+            zbuf = torch.empty(H, W, device=dev)
+            p2f = torch.empty(H, W, dtype=torch.int64, device=dev)
+            L.call("mp_depth_raster", cam, v if V else None, V, f if F else None, F, H, W, zbuf, p2f, ws, ws.numel())
+        ctx.cam, ctx.H, ctx.W, ctx.dev, ctx.verts_in = cam, H, W, dev, verts
+        ctx.save_for_backward(v, f, p2f)
+        ctx.mark_non_differentiable(p2f)
+        return zbuf, p2f
+
+    @staticmethod
+    def backward(ctx, d_zbuf, _d_p2f):
+        if d_zbuf is None:
+            return None, None, None, None, None, None
+        v, f, p2f = ctx.saved_tensors
+        V, F, dev = v.shape[0], f.shape[0], ctx.dev
+        with torch.cuda.device(dev):
+            g = L.dev(d_zbuf, dev)
+            ws = L.workspace(L.call("mp_depth_raster_backward_workspace_bytes", ctx.H, ctx.W, V), dev)
+            d_v = torch.empty(V, 3, device=dev)
+            L.call("mp_depth_raster_backward", ctx.cam, v if V else None, V, f if F else None, F, ctx.H, ctx.W, p2f, g,
+                   d_v if V else None, ws, ws.numel())
+        return None, None, None, None, _grad_like(d_v, ctx.verts_in), None
+
+
+class Knn1(torch.autograd.Function):
+    """pytorch3d.ops.knn_points(p1, p2, K=1, return_nn=True) (multiply_model.py:539) as one autograd node (mp_knn1):
+    inputs p1 [N1,3], p2 [N2,3] (N2 >= 1), outputs dists [N1] (squared), idx [N1] int64 (not differentiable) and nn
+    [N1,3] = p2[idx], on p1's device.  The backward (mp_knn1_backward) returns d p1 and d p2."""
+
+    @staticmethod
+    def forward(ctx, p1, p2):
+        dev = p1.device
+        with torch.cuda.device(dev):
+            a = L.dev(p1.reshape(-1, 3), dev)
+            b = L.dev(p2.reshape(-1, 3), dev)
+            N1, N2 = a.shape[0], b.shape[0]
+            ws = L.workspace(L.call("mp_knn1_workspace_bytes", N1), dev)
+            dists = torch.empty(N1, device=dev)
+            idx = torch.empty(N1, dtype=torch.int64, device=dev)
+            nn = torch.empty(N1, 3, device=dev)
+            L.call("mp_knn1", a, N1, b, N2, dists, idx, nn, ws, ws.numel())
+        ctx.inputs = (p1, p2)
+        ctx.save_for_backward(a, b, idx)
+        ctx.mark_non_differentiable(idx)
+        return dists, idx, nn
+
+    @staticmethod
+    def backward(ctx, d_dists, _d_idx, d_nn):
+        a, b, idx = ctx.saved_tensors
+        N1, N2, dev = a.shape[0], b.shape[0], a.device
+        with torch.cuda.device(dev):
+            ws = L.workspace(L.call("mp_knn1_backward_workspace_bytes", N1, N2), dev)
+            d_a = torch.empty(N1, 3, device=dev)
+            d_b = torch.empty(N2, 3, device=dev)
+            L.call("mp_knn1_backward", a, N1, b, N2, idx, L.dev(d_dists, dev), L.dev(d_nn, dev), d_a, d_b, ws,
+                   ws.numel())
+        p1, p2 = ctx.inputs
+        return _grad_like(d_a, p1), _grad_like(d_b, p2)
+
+
 def marching_cubes(grid, level=0.0, center=(0.0, 0.0, 0.0), extent=None, pad=1.1):
     """Marching cubes (DESIGN §3.7) on a device grid [R+1]*3 (x-major): returns (verts [V,3] fp32 in world space
     ((p / R - 0.5) * pad) * extent + centre, faces [F,3] int64).  extent=None: lattice coordinates (pad 1, extent R,
