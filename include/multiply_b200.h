@@ -110,9 +110,22 @@ int mp_set_streams(int on);
 
 /* Per-launch timing of the tensor-core MLP kernel (CUDA events on the launching stream), by program kind:
  * [0] sdf-only, [1] forward (sdf + features), [2] full shade, [3] background.  mp_profile_read synchronises
- * on the recorded events and returns summed milliseconds, launch counts and processed points (host arrays of 4). */
+ * on the recorded events and returns summed milliseconds, launch counts and processed points (host arrays of 4).
+ * on = 2 also runs the kernel's stall-accounting build: every consumer warp (lane 0) and the weight loader sum clock64
+ * intervals by step kind and phase into a per-CTA block of the MLP workspace, added after each launch into a
+ * process-wide device total on the current device.  The block is part of mp_mlp_workspace_bytes (and of every query that
+ * nests it) only while on = 2, so switch it on before sizing the workspaces it will run with.
+ * mp_profile_read_stalls synchronises the device and copies that total out: clocks_host
+ * [4 program kinds][MP_STALL_WARPS][MP_STALL_WORDS], warp 0 the loader lane, warps 1.. the consumer warps; word
+ * MP_STALL_PHASES * k + ph is step kind k (0 softplus, 1 softplus saving sigma', 2 seed of the reverse sweep, 3 features,
+ * 4 reverse, 5 final gradient, 6 ReLU) and phase ph (0 whole step, 1 blocked on a weight slot, 2 in wgmma waits,
+ * 3 in named barriers, 4 epilogue, 5 loader blocked on a free ring position), then MP_STALL_PROLOGUE (tile
+ * prologues) and MP_STALL_ELAPSED (the warp's whole run).  reset != 0 zeroes the total. */
+enum { MP_STALL_KINDS = 7, MP_STALL_PHASES = 6, MP_STALL_PROLOGUE = 42, MP_STALL_ELAPSED = 43, MP_STALL_WORDS = 44,
+       MP_STALL_WARPS = 9 };
 int mp_profile_enable(int on);
 int mp_profile_read(double* ms_host, long long* launches_host, double* points_host, int reset);
+int mp_profile_read_stalls(unsigned long long* clocks_host, int reset);
 
 /* ImplicitNet.forward (networks.py:126-208): x [N,d_in] -> out [N,257] (sdf | feature).
  * sdf / feat may be NULL.  Replaces `self.foreground_implicit_network_list[p](x_c, cond)`. */

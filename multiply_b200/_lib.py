@@ -16,6 +16,8 @@ LIB_PATH = os.environ.get("MP_LIB") or os.path.join(HERE, "libmultiply_b200.so")
 
 MP_MAX_LAYERS = 12
 MP_MAX_PERSONS = 8
+# layout of mp_profile_read_stalls' array: [4 program kinds][MP_STALL_WARPS][MP_STALL_WORDS]
+MP_STALL_PHASES, MP_STALL_PROLOGUE, MP_STALL_ELAPSED, MP_STALL_WORDS, MP_STALL_WARPS = 6, 42, 43, 44, 9
 
 c_float_p = C.POINTER(C.c_float)
 c_int_p = C.POINTER(C.c_int)
@@ -126,6 +128,7 @@ SIGNATURES = {
     "mp_profile_enable": (STATUS, [_I]),
     "mp_set_streams": (STATUS, [_I]),
     "mp_profile_read": (STATUS, [C.POINTER(C.c_double), C.POINTER(C.c_longlong), C.POINTER(C.c_double), _I]),
+    "mp_profile_read_stalls": (STATUS, [C.POINTER(C.c_ulonglong), _I]),
     "mp_implicit_forward": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_implicit_forward_grad": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _SZ, STREAM]),
     "mp_render_forward": (STATUS, [_VP, _VP, _VP, _VP, _I, _VP, _VP, _SZ, STREAM]),

@@ -200,6 +200,7 @@ size_t tc_pack_bytes();
 void tc_free(Field& f);
 int prof_enable(int on);
 int prof_read(double* ms, long long* launches, double* points, int reset);
+int prof_read_stalls(unsigned long long* clocks, int reset);
 extern std::atomic<int> g_precision;
 
 // engine dispatch (render.cu): g_engine 1 = tensor cores, 0 = SIMT; field_ws_bytes covers either engine

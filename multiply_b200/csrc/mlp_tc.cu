@@ -94,10 +94,28 @@ struct TcIO : MlpCall {
   float rz;              // relative truncation loss of ONE tensor-core accumulation (see kRzPerMma)
   char* scratch;         // per-CTA scratch
   size_t scratch_per_cta;
+  unsigned long long* stalls;   // stall-accounting build only: per CTA [kStallWarps][MP_STALL_WORDS] clock64 totals
 };
 
 constexpr int kConsumers = 2;                                 // consumer warpgroups (64 rows each)
 constexpr int kThreads = 128 * (1 + kConsumers);
+
+// Stall accounting (mp_profile_enable(2), the PROF instantiation of the kernel): phases of a step, as laid out in
+// include/multiply_b200.h
+enum { PH_STEP = 0, PH_FULL = 1, PH_WGMMA = 2, PH_BAR = 3, PH_EPI = 4, PH_EMPTY = 5 };
+constexpr int kStallWarps = 1 + 4 * kConsumers;               // the loader lane, then the consumer warps
+static_assert(MP_STALL_WARPS == kStallWarps && MP_STALL_KINDS == K_RELU + 1 && MP_STALL_PHASES == PH_EMPTY + 1 &&
+                  MP_STALL_PROLOGUE == MP_STALL_KINDS * MP_STALL_PHASES && MP_STALL_ELAPSED == MP_STALL_PROLOGUE + 1 &&
+                  MP_STALL_WORDS == MP_STALL_ELAPSED + 1,
+              "stall record layout of include/multiply_b200.h");
+template <bool PROF>
+__device__ __forceinline__ long long stall_clock() {
+  if constexpr (PROF) return clock64();
+  else return 0;
+}
+__device__ __forceinline__ void stall_add(unsigned long long* rec, int word, long long clocks) {
+  atomicAdd(rec + word, (unsigned long long)clocks);
+}
 
 // per-CTA scratch layout (bytes); sigma' and the stashed features are indexed by (warpgroup, register group, thread)
 constexpr size_t kSigBytes = (size_t)8 * kConsumers * 32 * 128 * 16;   // sigma' [8][2][32][128] float4
@@ -105,6 +123,12 @@ constexpr size_t kFeatBytes = (size_t)kConsumers * 32 * 128 * 16;      // featur
 constexpr size_t kGeBytes = (size_t)96 * 128 * 4;            // skip gradient [E<=96][128 rows]
 constexpr size_t kEmbBytes = (size_t)96 * 128 * 4;           // input embedding of the tile [E<=96][128 rows]
 constexpr size_t kScratchPerCta = kSigBytes + kFeatBytes + kGeBytes + kEmbBytes;
+
+// The epilogue's scratch reads (sigma' in the reverse sweep, the stashed features) go through volatile asm, which the
+// compiler keeps in program order with the discard of the previous group (which waits for that group's data) and the
+// stmatrix stores: issued in place, every load would start only after the previous one returned.  So they are issued
+// kAhead of the epilogue's 16 column groups (16 columns each) ahead of their use.
+constexpr int kAhead = 4;
 
 // shared memory carve-up
 constexpr int kABytes = 2 * 4 * 128 * 128;                   // hi + lo, 4 K-blocks of [128 x 128B]
@@ -407,6 +431,8 @@ __device__ __forceinline__ void final_grad(const TcProgram& P, const TcIO& io, c
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
+// PROF: the stall-accounting build (mp_profile_enable(2)); the default build reads no clock.
+template <bool PROF>
 __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
                                                                const __grid_constant__ TcIO io) {
   extern __shared__ uint8_t smem_raw[];
@@ -436,26 +462,42 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
     // ===================== weight loader =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     if (warp == 0 && lane == 0) {
+      const long long t_run = stall_clock<PROF>();
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         for (int s = 0; s < P.nsteps; ++s) {
+          const long long t_step = stall_clock<PROF>();
+          long long c_empty = 0;
           const char* src = (const char*)P.blob + (size_t)P.step[s].slot_off * kSlotBytes;
           const int nslot = 2 * P.step[s].nk;
           const int jstep = P.step[s].terms == 1 ? 2 : 1;
           for (int j = 0; j < nslot; j += jstep, ++it) {
             int r = it % kRing;
             uint32_t ph = (it / kRing) & 1;
+            const long long t0 = stall_clock<PROF>();
             mbar_wait(&empty[r], ph ^ 1);
+            c_empty += stall_clock<PROF>() - t0;
             mbar_expect_tx(&full[r], kSlotBytes);
             bulk_g2s(ring + (size_t)r * kSlotBytes, src + (size_t)j * kSlotBytes, kSlotBytes, &full[r]);
           }
+          if constexpr (PROF) {
+            unsigned long long* rec = io.stalls + (size_t)blockIdx.x * kStallWarps * MP_STALL_WORDS +
+                                      P.step[s].kind * MP_STALL_PHASES;
+            stall_add(rec, PH_STEP, clock64() - t_step);
+            stall_add(rec, PH_EMPTY, c_empty);
+          }
         }
       }
+      if constexpr (PROF)
+        stall_add(io.stalls + (size_t)blockIdx.x * kStallWarps * MP_STALL_WORDS, MP_STALL_ELAPSED, clock64() - t_run);
     }
     return;
   }
   // ===================== consumer warpgroups: MMAs + epilogue =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const long long t_run = stall_clock<PROF>();
+  // this warp's stall record (PROF): lane 0 adds to it
+  auto srec = [&]() { return io.stalls + ((size_t)blockIdx.x * kStallWarps + warp - 3) * MP_STALL_WORDS; };
   const int g = (warp >> 2) - 1;                 // consumer warpgroup: tile rows 64 g .. 64 g + 63
   const int t = threadIdx.x & 127;               // thread in the warpgroup
   const int wq = warp & 3, q = lane & 3;
@@ -482,6 +524,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   uint32_t it = 0;                               // ring position
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long t_tile = stall_clock<PROF>();
     int pt[2], slot[2];
     bool valid[2];
     float x[2][4];
@@ -552,8 +595,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
     // colour-net extra inputs: foreground [x_c, n] (networks.py:281) live in registers (n arrives at the end of the
     // reverse sweep); the background view-dir embedding (:275) was parked in `ge` by the prologue
     float nrm[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    if constexpr (PROF)
+      if (lane == 0) stall_add(srec(), MP_STALL_PROLOGUE, clock64() - t_tile);
     for (int s = 0; s < P.nsteps; ++s) {
       const TcStep st = P.step[s];
+      const long long t_step = stall_clock<PROF>();
+      long long c_full = 0, c_wgmma = 0, c_bar = 0;     // PROF: clocks of this step blocked in each phase
       // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
       const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
       const bool one_term = st.terms == 1;
@@ -571,7 +618,11 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       // ---------------- MMAs: acc = A . W^T over st.nk K-blocks ----------------
       // this warpgroup's rows of A are complete: publish them to the tensor cores
       fence_async_smem();
-      wg_sync(bar_id);
+      {
+        const long long t0 = stall_clock<PROF>();
+        wg_sync(bar_id);
+        c_bar += stall_clock<PROF>() - t0;
+      }
       wgmma_fence();
       // Every weight slot's MMAs form one commit group.  A slot is released as soon as the group after it has been
       // committed and all but that newest group have completed, so a warpgroup holds at most one slot in flight while
@@ -584,7 +635,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       auto slot_issued = [&](uint32_t slot_it) {
         wgmma_commit();
         if (held) {
+          const long long t0 = stall_clock<PROF>();
           wgmma_wait<1>();
+          c_wgmma += stall_clock<PROF>() - t0;
           release(held_slot);
         }
         held = true;
@@ -594,8 +647,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         if (kc == 4) {
           // extra-input K-block (colour layer 0): once the MMAs over K-block 0 have drained it, this row's extra inputs
           // (16 columns per lane of the quad, zero padded to 64) take its place and accumulate into the same tile
-          wgmma_wait<0>();
-          acc_fence(acc);
+          {
+            const long long t0 = stall_clock<PROF>();
+            wgmma_wait<0>();
+            acc_fence(acc);
+            c_wgmma += stall_clock<PROF>() - t0;
+          }
           if (held) release(held_slot);
           held = false;
 #pragma unroll
@@ -618,13 +675,19 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
             }
           }
           fence_async_smem();
-          wg_sync(bar_id);
+          {
+            const long long t0 = stall_clock<PROF>();
+            wg_sync(bar_id);
+            c_bar += stall_clock<PROF>() - t0;
+          }
           wgmma_fence();
         }
         const uint32_t ka = (uint32_t)(kc & 3) * 16384u;
         // hi slot: A_hi.W_hi + A_lo.W_hi
         int r = it % kRing;
+        long long t0 = stall_clock<PROF>();
         mbar_wait(&full[r], (it / kRing) & 1);
+        c_full += stall_clock<PROF>() - t0;
         uint32_t wb = smem_u32(ring + (size_t)r * kSlotBytes);
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
@@ -636,23 +699,55 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         if (!one_term) {
           // lo slot: A_hi.W_lo
           r = it % kRing;
+          t0 = stall_clock<PROF>();
           mbar_wait(&full[r], (it / kRing) & 1);
+          c_full += stall_clock<PROF>() - t0;
           wb = smem_u32(ring + (size_t)r * kSlotBytes);
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), make_desc(wb + ks * 32), 1);
           slot_issued(it++);
         }
       }
-      wgmma_wait<0>();
-      acc_fence(acc);
+      {
+        const long long t0 = stall_clock<PROF>();
+        wgmma_wait<0>();
+        acc_fence(acc);
+        c_wgmma += stall_clock<PROF>() - t0;
+      }
       if (held) release(held_slot);
 
       // ---------------- epilogue ----------------
+      const long long t_epi = stall_clock<PROF>();
+      auto step_done = [&]() {
+        if constexpr (PROF) {
+          if (lane == 0) {
+            const long long now = clock64();
+            unsigned long long* rec = srec() + st.kind * MP_STALL_PHASES;
+            stall_add(rec, PH_STEP, now - t_step);
+            stall_add(rec, PH_FULL, c_full);
+            stall_add(rec, PH_WGMMA, c_wgmma);
+            stall_add(rec, PH_BAR, c_bar);
+            stall_add(rec, PH_EPI, now - t_epi);
+          }
+        }
+      };
       auto reload_features = [&]() {
+        // loaded kAhead groups ahead of their use: a load issued after the previous group's discard and stmatrix
+        // would wait for that group's load to return (see kAhead)
+        uint4 pre[kAhead][2];
+#pragma unroll
+        for (int k = 0; k < kAhead; ++k) {
+          pre[k][0] = ld_stream(&fsc[(size_t)k * 128 + t]);
+          pre[k][1] = ld_stream(&fsc[(size_t)(16 + k) * 128 + t]);
+        }
 #pragma unroll
         for (int jp = 0; jp < 16; ++jp) {
-          const uint4 fh = ld_stream(&fsc[(size_t)jp * 128 + t]);
-          const uint4 fl = ld_stream(&fsc[(size_t)(16 + jp) * 128 + t]);
+          const uint4 fh = pre[jp % kAhead][0];
+          const uint4 fl = pre[jp % kAhead][1];
+          if (jp + kAhead < 16) {
+            pre[jp % kAhead][0] = ld_stream(&fsc[(size_t)(jp + kAhead) * 128 + t]);
+            pre[jp % kAhead][1] = ld_stream(&fsc[(size_t)(16 + jp + kAhead) * 128 + t]);
+          }
           store_pairs(lane_base, lane_x, jp, fh, fl);
           if ((lane & 7) == 0) {
             discard_line(&fsc[(size_t)jp * 128 + t], fh.x);
@@ -664,12 +759,21 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         final_grad(P, io, acc, isc, q, ge, emb, rowt, valid, pt, slot, nrm);
         // the MMAs of the reverse sweep are done with A: the features return as the colour net's input
         if (s + 1 < P.nsteps) reload_features();
+        step_done();
         continue;
       }
 
       auto run_epi = [&](auto kind) {
         constexpr int KIND = decltype(kind)::value;
         float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};     // sdf / rgb partial dots of the two rows
+        // K_BWD: this step's sigma' groups j = 0 .. 31 (8 columns each), loaded 2 kAhead groups ahead of their use
+        const float4* sig_g = &sig[((size_t)(st.sig < 0 ? 0 : st.sig) * kConsumers + g) * 32 * 128 + t];
+        float4 sig_pre[2 * kAhead];
+        if constexpr (KIND == K_BWD) {
+#pragma unroll
+          for (int k = 0; k < 2 * kAhead; ++k)
+            sig_pre[k] = st.sig >= 0 ? ld_stream(sig_g + (size_t)k * 128) : make_float4(1.f, 1.f, 1.f, 1.f);
+        }
 #pragma unroll
         for (int jp = 0; jp < 16; ++jp) {
           float* v = acc + 8 * jp;
@@ -727,9 +831,10 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
                   if (valid[h]) *(float2*)(io.feat + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
               }
             } else if constexpr (KIND == K_BWD) {
-              float4 s4 = make_float4(1.f, 1.f, 1.f, 1.f);
-              const float4* sp = &sig[(((size_t)(st.sig < 0 ? 0 : st.sig) * kConsumers + g) * 32 + j) * 128 + t];
-              if (st.sig >= 0) s4 = ld_stream(sp);
+              const float4 s4 = sig_pre[j % (2 * kAhead)];
+              if (j + 2 * kAhead < 32 && st.sig >= 0)
+                sig_pre[j % (2 * kAhead)] = ld_stream(sig_g + (size_t)(j + 2 * kAhead) * 128);
+              const float4* sp = sig_g + (size_t)j * 128;
               const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
               if ((st.flags & F_SKIP_GRAD) && c + 1 >= P.inj_col) {
                 // columns >= inj_col are d/d embed through the skip connection: park them, zero them in A
@@ -805,8 +910,11 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       }
       // the skip gradient parked in `ge` is read by other lanes of the quad at the final-gradient step
       if (st.flags & F_SKIP_GRAD) __threadfence_block();
+      step_done();
     }
   }
+  if constexpr (PROF)
+    if (lane == 0) stall_add(srec(), MP_STALL_ELAPSED, clock64() - t_run);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1075,12 +1183,28 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 // One scratch slice per persistent CTA; a launch runs at most one CTA per SM and per 128-point tile.
 static int tc_max_grid(int cap) { return max(0, min(sm_count(), div_up(cap, 128))); }
-static char* tc_carve(Arena& a, int grid) { return a.take<char>((size_t)grid * kScratchPerCta); }
+// the stall-accounting build's counters (mp_profile_enable(2)) follow the scratch, one record per warp of each CTA
+constexpr size_t kStallWordsPerCta = (size_t)kStallWarps * MP_STALL_WORDS;
+static std::atomic<bool> g_prof_stalls{false};
+static void tc_carve(Arena& a, int grid, bool stalls, TcIO& io) {
+  io.scratch = a.take<char>((size_t)grid * kScratchPerCta);
+  io.stalls = stalls ? a.take<unsigned long long>((size_t)grid * kStallWordsPerCta) : nullptr;
+}
 
 size_t tc_workspace_bytes(int N) {
   Arena a;
-  tc_carve(a, tc_max_grid(N));
+  TcIO io{};
+  tc_carve(a, tc_max_grid(N), g_prof_stalls.load(), io);
   return a.off;
+}
+
+// total[w] += sum over the grid's CTAs of rec[cta][w]
+__global__ void stall_sum_kernel(const unsigned long long* __restrict__ rec, int grid, unsigned long long* total) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= (int)kStallWordsPerCta) return;
+  unsigned long long v = 0;
+  for (int c = 0; c < grid; ++c) v += rec[(size_t)c * kStallWordsPerCta + w];
+  atomicAdd(total + w, v);
 }
 
 // optional per-launch timing of the tensor-core kernel (bench.py roofline): CUDA events on the
@@ -1099,14 +1223,33 @@ static std::vector<ProfEntry>* g_prof = nullptr;
 static int* g_prof_pinned = nullptr;
 static int g_prof_used = 0;
 constexpr int kProfMax = 1 << 16;
+static unsigned long long* g_stall_total = nullptr;     // device [4 program kinds][kStallWordsPerCta]
+constexpr size_t kStallTotalBytes = 4 * kStallWordsPerCta * sizeof(unsigned long long);
 
 int prof_enable(int on) {
+  MP_REQUIRE(on >= 0 && on <= 2, "mp_profile_enable: 0 (off), 1 (launch times) or 2 (launch times and stall clocks)");
   std::lock_guard<std::mutex> g(g_prof_mu);
   if (on && !g_prof) {
     g_prof = new std::vector<ProfEntry>();
     MP_CHECK_CUDA(cudaMallocHost(&g_prof_pinned, kProfMax * sizeof(int)));
   }
+  if (on == 2 && !g_stall_total) {
+    MP_CHECK_CUDA(cudaMalloc(&g_stall_total, kStallTotalBytes));
+    MP_CHECK_CUDA(cudaMemset(g_stall_total, 0, kStallTotalBytes));
+  }
+  g_prof_stalls = on == 2;
   g_prof_on = on != 0;
+  return 0;
+}
+int prof_read_stalls(unsigned long long* clocks, int reset) {
+  std::lock_guard<std::mutex> g(g_prof_mu);
+  if (!g_stall_total) {
+    memset(clocks, 0, kStallTotalBytes);
+    return 0;
+  }
+  MP_CHECK_CUDA(cudaDeviceSynchronize());
+  MP_CHECK_CUDA(cudaMemcpy(clocks, g_stall_total, kStallTotalBytes, cudaMemcpyDeviceToHost));
+  if (reset) MP_CHECK_CUDA(cudaMemset(g_stall_total, 0, kStallTotalBytes));
   return 0;
 }
 int prof_read(double* ms, long long* launches, double* points, int reset) {
@@ -1175,9 +1318,13 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
   }
   if (grid < 1) return 0;
   Arena a(ws, ws_bytes);
-  io.scratch = tc_carve(a, grid);
+  tc_carve(a, grid, g_prof_stalls.load(), io);
   MP_TRY(a.fits("tensor-core engine"));
   io.scratch_per_cta = kScratchPerCta;
+  if (io.stalls) {
+    MP_REQUIRE(g_stall_total, "tensor-core engine: stall accounting is not enabled");
+    MP_CHECK_CUDA(cudaMemsetAsync(io.stalls, 0, (size_t)grid * kStallWordsPerCta * sizeof(unsigned long long), st));
+  }
   static const float rz_scale = [] {
     const char* er = getenv("MP_TC_RZ_SCALE");      // experiment knob: multiplies kRzPerMma (0 switches it off)
     return er ? (float)atof(er) : 1.f;
@@ -1191,7 +1338,8 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     MP_CHECK_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> g(attr_mu);
     if (dev < 0 || dev >= 64 || !((attr_done >> dev) & 1ull)) {
-      MP_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+      MP_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+      MP_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
       if (dev >= 0 && dev < 64) attr_done |= 1ull << dev;
     }
   }
@@ -1211,11 +1359,20 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
     }
     MP_CHECK_CUDA(cudaEventRecord(pe.e0, st));
   }
-  tc_chain_kernel<<<grid, kThreads, kSmemBytes, st>>>(P, io);
+  if (io.stalls) {
+    tc_chain_kernel<true><<<grid, kThreads, kSmemBytes, st>>>(P, io);
+  } else {
+    tc_chain_kernel<false><<<grid, kThreads, kSmemBytes, st>>>(P, io);
+  }
   MP_LAUNCH_CHECK();
   if (prof) {
     MP_CHECK_CUDA(cudaEventRecord(pe.e1, st));
     g_prof->push_back(pe);
+  }
+  if (io.stalls) {
+    stall_sum_kernel<<<div_up((int)kStallWordsPerCta, 128), 128, 0, st>>>(io.stalls, grid,
+                                                                          g_stall_total + (int)kind * kStallWordsPerCta);
+    MP_LAUNCH_CHECK();
   }
   return 0;
 }

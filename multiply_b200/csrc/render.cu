@@ -212,6 +212,11 @@ int mp_profile_read(double* ms_host, long long* launches_host, double* points_ho
   return mp::prof_read(ms_host, launches_host, points_host, reset);
 }
 
+int mp_profile_read_stalls(unsigned long long* clocks_host, int reset) {
+  MP_REQUIRE(clocks_host, "mp_profile_read_stalls: null argument");
+  return mp::prof_read_stalls(clocks_host, reset);
+}
+
 size_t mp_mlp_workspace_bytes(int N) { return mp::field_ws_bytes(N); }
 
 int mp_implicit_forward(mp_net_t* f, const float* x, int N, float* sdf, float* feat, void* workspace,
