@@ -17,8 +17,7 @@
  *     multiply.py:208, deformer.py:22-24).
  *   - scratch memory comes from caller-provided workspaces sized by the *_workspace_bytes calls, and persistent
  *     handles live in caller storage sized by the *_bytes calls (mp_mesh_plan's storage_bytes).  Exactly the query's
- *     bytes suffice and a call writes none beyond them (mp_field_pack_bytes, which takes no shapes, is an upper
- *     bound); where a query answers 0 the call also takes a NULL buffer.  Every workspace, storage and scratch base
+ *     bytes suffice and a call writes none beyond them; where a query answers 0 the call also takes a NULL buffer.  Every workspace, storage and scratch base
  *     (mp_mesh_plan's MP_MESH_PLAN_SCRATCH_BYTES included) must be 256-byte aligned, as every cudaMalloc and torch
  *     allocation is.  A call refuses a smaller or misaligned buffer before it enqueues anything.
  */
@@ -86,8 +85,11 @@ typedef struct {
 /* A foreground field = ImplicitNet + RenderingNet of one person; background field = bg pair.
  * Packing folds weight-norm (networks.py:82-83), the 1/sqrt(2) of the skip layer (:166-167) and
  * lays the weights out for the kernels (fp32 transposed for the SIMT engine, fp16 hi/lo
- * swizzled K-major tiles for the tensor-core engine).  The handle is immutable afterwards. */
-size_t mp_field_pack_bytes(void);
+ * swizzled K-major tiles for the tensor-core engine).  The handle is immutable afterwards.
+ * mp_field_pack_bytes is the storage of exactly these two networks; it reads only the descriptors' dimensions and
+ * whether lin_pose is given (no weight is dereferenced), and answers 0 for a pair mp_field_pack would refuse.  The
+ * pack refuses a pair, or a short or misaligned storage, before it enqueues anything. */
+size_t mp_field_pack_bytes(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background);
 int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background,
                   void* storage, size_t storage_bytes, mp_net_t** out, void* stream);
 void mp_field_free(mp_net_t* f);

@@ -117,7 +117,7 @@ SIGNATURES = {
     "mp_device_sm_count": (_I, []),
     "mp_linspace_host": (STATUS, [_F, _F, _I, c_float_p]),
     "mp_launch_count": (C.c_longlong, [_I]),
-    "mp_field_pack_bytes": (_SZ, []),
+    "mp_field_pack_bytes": (_SZ, [C.POINTER(ImplicitDesc), C.POINTER(RenderDesc), _I]),
     "mp_field_pack": (STATUS, [C.POINTER(ImplicitDesc), C.POINTER(RenderDesc), _I, _VP, _SZ, C.POINTER(_VP), STREAM]),
     "mp_field_free": (None, [_VP]),
     "mp_field_set_cond": (STATUS, [_VP, _VP, STREAM]),

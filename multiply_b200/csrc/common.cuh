@@ -122,6 +122,7 @@ struct Body {
 
 // packed network (mlp_pack.cu)
 constexpr int kHidden = 256;
+struct TcBlob;
 struct Field {
   int is_bg;
   int d_in, multires, emb_dim, cond_dim, skip_layer, n_imp;   // implicit
@@ -144,10 +145,9 @@ struct Field {
   int ren_cond_dim;
   float* ren_cb;                   // [out0] Wc0[:, feat] . b8[1:]  (colour layer 0 folded onto the feature layer)
   float* ren_b0_fold;              // [out0] ren_b0_eff + ren_cb : bias of the folded layer (tensor-core chains)
-  // tensor-core engine blobs (mlp_tc.cu); null until packed
-  void* tc;
-  char* storage;
-  size_t storage_bytes;
+  bool tc_full;                    // the tensor-core engine has a full program: the fused shade chain (foreground) or the
+                                   // background chain
+  TcBlob* tc;                      // tensor-core programs (mlp_tc.cu); null until packed
 };
 
 // launch helpers
@@ -195,9 +195,10 @@ int simt_render(const Field& f, const float* pts, const float* nrm, const float*
 // tensor-core engine (mlp_tc.cu)
 size_t tc_workspace_bytes(int N);
 int tc_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st);
-int tc_pack(Field& f, Arena& a, cudaStream_t st);
-size_t tc_pack_bytes();
-void tc_free(Field& f);
+TcBlob* tc_new();
+void tc_free(TcBlob* tb);
+void tc_pack_carve(Arena& a, Field& f);
+int tc_pack(const Field& f, cudaStream_t st);
 int prof_enable(int on);
 int prof_read(double* ms, long long* launches, double* points, int reset);
 int prof_read_stalls(unsigned long long* clocks, int reset);

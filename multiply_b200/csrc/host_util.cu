@@ -35,7 +35,7 @@ int sm_count() {
 
 extern "C" {
 
-int mp_version(void) { return 102; }
+int mp_version(void) { return 103; }
 
 const char* mp_last_error(void) { return mp::g_err; }
 

@@ -5,6 +5,7 @@
 //     skip             layer 4 input = [h3, embed(x)] / sqrt(2)    (:166-167)  -> 1/sqrt(2) folded into W4
 //     lin_pose         colour input [x, n, lin_pose(pose), feat]   (:277-281)  -> folded into the bias per call
 #include "common.cuh"
+#include <memory>
 
 namespace mp {
 
@@ -66,11 +67,6 @@ __global__ void add_vec_kernel(const float* __restrict__ a, const float* __restr
   if (i < n) d[i] = a[i] + b[i];
 }
 
-__global__ void copy_kernel(const float* __restrict__ s, float* __restrict__ d, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) d[i] = s[i];
-}
-
 static int fold(const float* v, const float* g, int out, int in, float scale, float* W, cudaStream_t st) {
   fold_kernel<<<div_up(out, 8), 256, 0, st>>>(v, g, out, in, scale, W);
   MP_LAUNCH_CHECK();
@@ -81,32 +77,20 @@ static int tcols(const float* W, int out, int in, int off, int n, float* Wt, int
   MP_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace mp
-
-extern "C" {
-
-size_t mp_field_pack_bytes(void) {
-  // fp32: 2 copies (natural + transposed) of <= 14 layers of <= 257x325 + small vectors; tc blobs
-  size_t fp32 = (size_t)14 * 2 * 260 * 328 * sizeof(float) + (1u << 20);
-  return fp32 + mp::tc_pack_bytes() + (1u << 16);
+static int copy(float* dst, const float* src, int n, cudaStream_t st) {
+  MP_CHECK_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
 }
 
-int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background, void* storage,
-                  size_t storage_bytes, mp_net_t** out, void* stream) {
-  using namespace mp;
-  MP_REQUIRE(imp && ren && storage && out, "mp_field_pack: null argument (both networks are required)");
-  MP_REQUIRE(storage_bytes >= mp_field_pack_bytes(), "mp_field_pack: storage too small (%zu < %zu)", storage_bytes,
-             mp_field_pack_bytes());
+// Every condition the pack sets on the two networks, checked on the host from the descriptors' dimensions and whether
+// lin_pose is there: fills the field's dimensions and decides whether the tensor-core engine gets a full program for it
+// (the fused foreground shade chain or the background chain).
+static int field_check(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background, Field& f) {
   MP_REQUIRE(imp->lin.n_layers == 9, "mp_field_pack: ImplicitNet must have 9 linear layers (got %d)",
              imp->lin.n_layers);
   MP_REQUIRE(imp->skip_layer == 4, "mp_field_pack: skip_in must be [4]");
-  Arena a(storage, storage_bytes);
-  MP_TRY(a.fits("mp_field_pack", "storage"));     // the base's alignment; the layout is checked after its carve below
-  cudaStream_t st = (cudaStream_t)stream;
-  mp_net* h = new mp_net();
-  Field& f = h->f;
-  memset(&f, 0, sizeof(f));
+  MP_REQUIRE(ren->lin.n_layers >= 1 && ren->lin.n_layers <= MP_MAX_LAYERS,
+             "mp_field_pack: RenderingNet must have 1 to %d linear layers (got %d)", MP_MAX_LAYERS, ren->lin.n_layers);
   f.is_bg = is_background;
   f.d_in = imp->d_in;
   f.multires = imp->multires;
@@ -114,131 +98,138 @@ int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, in
   f.cond_dim = imp->cond_dim;
   f.skip_layer = imp->skip_layer;
   f.n_imp = imp->lin.n_layers;
-  f.storage = (char*)storage;
-  f.storage_bytes = storage_bytes;
   const int E = f.emb_dim;
-  int rc = 0;
-  // padded tails of biases / weight tiles must read as zero (0 * garbage could be NaN)
-  MP_CHECK_CUDA(cudaMemsetAsync(storage, 0, mp_field_pack_bytes(), st));
-  // ---- implicit net -------------------------------------------------------------------
-  float* nat[MP_MAX_LAYERS];
-  for (int l = 0; l < f.n_imp && rc == 0; ++l) {
-    int in = imp->lin.in_dim[l], o = imp->lin.out_dim[l];
-    f.imp_in[l] = in;
-    f.imp_out[l] = o;
-    bool ok = true;
+  for (int l = 0; l < f.n_imp; ++l) {
+    const int in = imp->lin.in_dim[l], o = imp->lin.out_dim[l];
+    bool ok;
     if (l == 0) ok = (in == E + f.cond_dim) && o == kHidden;
     else if (l == f.skip_layer - 1) ok = (in == kHidden) && (o == kHidden - E);
     else if (l == f.n_imp - 1) ok = (in == kHidden) && (o == kHidden + 1);
     else ok = (in == kHidden) && (o == kHidden);
-    if (!ok) {
-      set_error("mp_field_pack: implicit layer %d has unsupported shape %dx%d", l, o, in);
-      rc = -1;
-      break;
-    }
-    nat[l] = a.take<float>((size_t)o * in);
-    f.imp_W[l] = nat[l];
-    f.imp_Wt[l] = a.take<float>((size_t)in * o);
-    f.imp_b[l] = a.take<float>(o < 264 ? 264 : o);   // padded: the tensor-core epilogue reads 256 columns
-    if (!a.ok) break;
-    float scale = (l == f.skip_layer) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
-    rc = fold(imp->lin.weight_v[l], imp->lin.weight_g[l], o, in, scale, nat[l], st);
-    if (rc) break;
-    rc = tcols(nat[l], o, in, 0, in, f.imp_Wt[l], o, st);
-    if (rc) break;
-    copy_kernel<<<div_up(o, 256), 256, 0, st>>>(imp->lin.bias[l], f.imp_b[l], o);
-    g_launches++;
+    MP_REQUIRE(ok, "mp_field_pack: implicit layer %d has unsupported shape %dx%d", l, o, in);
+    f.imp_in[l] = in;
+    f.imp_out[l] = o;
   }
-  if (rc == 0 && a.ok) {
-    f.imp_W0cond = f.imp_Wt[0] + (size_t)E * kHidden;   // rows E.. of the transposed layer-0 weights
-    f.imp_b0_eff = a.take<float>(kHidden);
-  }
-  // ---- rendering net ------------------------------------------------------------------
   f.n_ren = ren->lin.n_layers;
   f.ren_mode = ren->mode;
   f.multires_view = ren->multires_view;
-  float* rnat[MP_MAX_LAYERS];
-  if (rc == 0 && a.ok) {
-    int in0 = ren->lin.in_dim[0], out0 = ren->lin.out_dim[0];
-    if (ren->mode == 0) {
-      f.ren_extra = 6;
-      f.ren_cond_dim = 69;
-      if (in0 != 6 + 8 + kHidden || !ren->lin_pose_weight || !ren->lin_pose_bias) {
-        set_error("mp_field_pack: pose_no_view colour net must take 270 inputs and carry lin_pose");
-        rc = -1;
-      }
+  for (int l = 0; l < f.n_ren; ++l) {
+    f.ren_in[l] = ren->lin.in_dim[l];
+    f.ren_out[l] = ren->lin.out_dim[l];
+  }
+  if (ren->mode == 0) {
+    f.ren_extra = 6;
+    f.ren_cond_dim = 69;
+    MP_REQUIRE(f.ren_in[0] == 6 + 8 + kHidden && ren->lin_pose_weight && ren->lin_pose_bias,
+               "mp_field_pack: pose_no_view colour net must take 270 inputs and carry lin_pose");
+  } else {
+    f.ren_extra = 3 * (1 + 2 * ren->multires_view);
+    f.ren_cond_dim = 32;
+    MP_REQUIRE(f.ren_in[0] == f.ren_extra + 32 + kHidden,
+               "mp_field_pack: nerf_frame_encoding colour net has unsupported input width %d", f.ren_in[0]);
+  }
+  const bool fg_chain = (f.ren_mode == 0) && (f.n_ren == 5) && f.ren_out[0] == kHidden;
+  const bool bg_chain = (f.ren_mode == 1) && (f.n_ren == 2) && f.ren_out[0] <= kHidden && f.ren_extra <= 27;
+  MP_REQUIRE(!fg_chain || (f.d_in <= 4 && 1 + 2 * f.multires <= 14),
+             "tc_pack: the final-gradient step keeps 1 + 2 * multires <= 14 embedding columns per axis");
+  f.tc_full = fg_chain || bg_chain;
+  return 0;
+}
+
+// The whole storage of a packed field, one take per buffer: the fp32 layers (natural and transposed weights, biases
+// padded to 264 because the tensor-core epilogue reads 256 columns), the per-call folded biases and conditioning
+// columns, then the tensor-core share (tc_pack_carve).  On a sizing Arena it only measures.
+static void field_carve(Arena& a, Field& f) {
+  for (int l = 0; l < f.n_imp; ++l) {
+    const int in = f.imp_in[l], o = f.imp_out[l];
+    f.imp_W[l] = a.take<float>((size_t)o * in);
+    f.imp_Wt[l] = a.take<float>((size_t)in * o);
+    f.imp_b[l] = a.take<float>(o < 264 ? 264 : o);
+  }
+  f.imp_b0_eff = a.take<float>(kHidden);
+  for (int l = 0; l < f.n_ren; ++l) {
+    const int in = f.ren_in[l], o = f.ren_out[l];
+    f.ren_W[l] = a.take<float>((size_t)o * in);
+    f.ren_Wt[l] = a.take<float>((size_t)in * o);
+    f.ren_b[l] = a.take<float>(o < 264 ? 264 : o);
+  }
+  const int out0 = f.ren_out[0];
+  f.ren_b0_eff = a.take<float>(out0 < 264 ? 264 : out0);
+  f.ren_b0_base = a.take<float>(out0);
+  f.ren_W0cond = a.take<float>((size_t)f.ren_cond_dim * out0);
+  tc_pack_carve(a, f);
+}
+
+// The fp32 layers into the zeroed storage: weight norm and the skip's 1/sqrt(2) folded in, natural and transposed, and
+// colour layer 0's conditioning columns split off for mp_field_set_cond.
+static int field_fold(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, Field& f, cudaStream_t st) {
+  for (int l = 0; l < f.n_imp; ++l) {
+    const int in = f.imp_in[l], o = f.imp_out[l];
+    const float scale = (l == f.skip_layer) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
+    MP_TRY(fold(imp->lin.weight_v[l], imp->lin.weight_g[l], o, in, scale, f.imp_W[l], st));
+    MP_TRY(tcols(f.imp_W[l], o, in, 0, in, f.imp_Wt[l], o, st));
+    MP_TRY(copy(f.imp_b[l], imp->lin.bias[l], o, st));
+  }
+  f.imp_W0cond = f.imp_Wt[0] + (size_t)f.emb_dim * kHidden;   // rows E.. of the transposed layer-0 weights
+  for (int l = 0; l < f.n_ren; ++l) {
+    const int in = f.ren_in[l], o = f.ren_out[l];
+    MP_TRY(fold(ren->lin.weight_v[l], ren->lin.weight_g[l], o, in, 1.0f, f.ren_W[l], st));
+    if (l == 0) {
+      // Wt0 rows: [extra inputs | feature block]; the conditioning columns go to ren_W0cond
+      const int cpos = f.ren_extra, cw = (f.ren_mode == 0) ? 8 : 32;
+      MP_TRY(tcols(f.ren_W[0], o, in, 0, f.ren_extra, f.ren_Wt[0], o, st));
+      MP_TRY(tcols(f.ren_W[0], o, in, cpos + cw, kHidden, f.ren_Wt[0] + (size_t)f.ren_extra * o, o, st));
     } else {
-      f.ren_extra = 3 * (1 + 2 * ren->multires_view);
-      f.ren_cond_dim = 32;
-      if (in0 != f.ren_extra + 32 + kHidden) {
-        set_error("mp_field_pack: nerf_frame_encoding colour net has unsupported input width %d", in0);
-        rc = -1;
-      }
+      MP_TRY(tcols(f.ren_W[l], o, in, 0, in, f.ren_Wt[l], o, st));
     }
-    for (int l = 0; l < f.n_ren && rc == 0; ++l) {
-      int in = ren->lin.in_dim[l], o = ren->lin.out_dim[l];
-      f.ren_in[l] = in;
-      f.ren_out[l] = o;
-      rnat[l] = a.take<float>((size_t)o * in);
-      f.ren_W[l] = rnat[l];
-      f.ren_Wt[l] = a.take<float>((size_t)in * o);
-      f.ren_b[l] = a.take<float>(o < 264 ? 264 : o);
-      if (!a.ok) break;
-      rc = fold(ren->lin.weight_v[l], ren->lin.weight_g[l], o, in, 1.0f, rnat[l], st);
-      if (rc) break;
-      if (l == 0) {
-        // Wt0 rows: [extra inputs | feature block]; the conditioning columns go to ren_W0cond
-        int cpos = f.ren_extra, cw = (ren->mode == 0) ? 8 : 32;
-        rc = tcols(rnat[0], o, in, 0, f.ren_extra, f.ren_Wt[0], o, st);
-        if (rc) break;
-        rc = tcols(rnat[0], o, in, cpos + cw, kHidden, f.ren_Wt[0] + (size_t)f.ren_extra * o, o, st);
-        if (rc) break;
-        f.ren_in[0] = f.ren_extra + kHidden;
-      } else {
-        rc = tcols(rnat[l], o, in, 0, in, f.ren_Wt[l], o, st);
-        if (rc) break;
-      }
-      copy_kernel<<<div_up(o, 256), 256, 0, st>>>(ren->lin.bias[l], f.ren_b[l], o);
-      g_launches++;
-    }
-    if (rc == 0 && a.ok) {
-      f.ren_b0_eff = a.take<float>(out0 < 264 ? 264 : out0);
-      f.ren_b0_base = a.take<float>(out0);
-      f.ren_W0cond = a.take<float>((size_t)f.ren_cond_dim * out0);
-      if (a.ok) {
-        if (ren->mode == 0) {
-          pose_fold_kernel<<<div_up(out0, 128), 128, 0, st>>>(rnat[0], in0, out0, f.ren_b[0], ren->lin_pose_weight,
-                                                              ren->lin_pose_bias, 8, 69, 6, f.ren_W0cond,
-                                                              f.ren_b0_base);
-          g_launches++;
-        } else {
-          rc = tcols(rnat[0], out0, in0, f.ren_extra, 32, f.ren_W0cond, out0, st);
-          copy_kernel<<<div_up(out0, 256), 256, 0, st>>>(f.ren_b[0], f.ren_b0_base, out0);
-          g_launches++;
-        }
-      }
-    }
+    MP_TRY(copy(f.ren_b[l], ren->lin.bias[l], o, st));
   }
-  if (rc == 0 && !a.ok) {
-    set_error("mp_field_pack: arena overflow (need %zu bytes)", a.off);
-    rc = -1;
+  const int in0 = f.ren_in[0], out0 = f.ren_out[0];
+  if (f.ren_mode == 0) {
+    pose_fold_kernel<<<div_up(out0, 128), 128, 0, st>>>(f.ren_W[0], in0, out0, f.ren_b[0], ren->lin_pose_weight,
+                                                        ren->lin_pose_bias, 8, 69, 6, f.ren_W0cond, f.ren_b0_base);
+    MP_LAUNCH_CHECK();
+  } else {
+    MP_TRY(tcols(f.ren_W[0], out0, in0, f.ren_extra, 32, f.ren_W0cond, out0, st));
+    MP_TRY(copy(f.ren_b0_base, f.ren_b[0], out0, st));
   }
-  if (rc == 0) rc = tc_pack(f, a, st);
-  if (rc == 0 && cudaGetLastError() != cudaSuccess) {
-    set_error("mp_field_pack: kernel launch failed");
-    rc = -3;
-  }
-  if (rc) {
-    tc_free(f);
-    delete h;
-    return rc;
-  }
-  *out = h;
+  return 0;
+}
+
+}  // namespace mp
+
+extern "C" {
+
+size_t mp_field_pack_bytes(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background) {
+  mp::Field f{};
+  if (!imp || !ren || mp::field_check(imp, ren, is_background, f) != 0) return 0;
+  mp::Arena a;
+  mp::field_carve(a, f);
+  return a.off;
+}
+
+int mp_field_pack(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren, int is_background, void* storage,
+                  size_t storage_bytes, mp_net_t** out, void* stream) {
+  using namespace mp;
+  MP_REQUIRE(imp && ren && storage && out, "mp_field_pack: null argument (both networks are required)");
+  std::unique_ptr<mp_net, void (*)(mp_net*)> h(new mp_net(), mp_field_free);
+  Field& f = h->f;
+  MP_TRY(field_check(imp, ren, is_background, f));
+  f.tc = tc_new();
+  Arena a(storage, storage_bytes);
+  field_carve(a, f);
+  MP_TRY(a.fits("mp_field_pack", "storage"));
+  cudaStream_t st = (cudaStream_t)stream;
+  // padded tails of biases / weight tiles must read as zero (0 * garbage could be NaN)
+  MP_CHECK_CUDA(cudaMemsetAsync(storage, 0, a.off, st));
+  MP_TRY(field_fold(imp, ren, f, st));
+  MP_TRY(tc_pack(f, st));
+  *out = h.release();
   return 0;
 }
 
 void mp_field_free(mp_net_t* f) {
-  if (f) mp::tc_free(f->f);
+  if (f) mp::tc_free(f->f.tc);
   delete f;
 }
 

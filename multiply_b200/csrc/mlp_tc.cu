@@ -60,10 +60,6 @@ enum {
 constexpr int kMaxSteps = 24;
 constexpr int kSlotBytes = 32768;          // 256 rows x 64 fp16
 constexpr int kRing = 3;
-// Weight slots of a field's blob.  The programs share their slots (the full program contains the forward one, which
-// contains the sdf-only one); the longest, the foreground's full program, has at most 2 * 2 (L0, E <= 96) +
-// 7 * 8 (L1..L7) + 8 (L8) + 8 * 8 (B7..B0) + 10 (folded colour layer 0) + 3 * 8 (colour layers 1..3) = 166.
-constexpr int kBlobSlots = 170;
 
 struct TcStep {
   int nk;               // 64-wide K chunks of A consumed by this layer (5 with F_EXTRA_IN: the last one re-uses K-block 0)
@@ -920,11 +916,29 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
 // ---------------------------------------------------------------------------------------------
 // packing
 // ---------------------------------------------------------------------------------------------
+// Where one packed layer's weights come from: its nk K-chunks of hi/lo weight slots, from slot slot_off on, hold
+// B[n][k] = W[n_off + n][k] (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere, scaled by the
+// 2^s of max |W[0, total)|.
+struct TcSrc {
+  const float* W;
+  int ld, transposed, n_off, n_valid, k_valid, nk, total, perm16, slot_off;
+};
+
+constexpr int kLdM = 320;     // row stride of the chains' folded colour layer 0 (see tc_pack)
+
 struct TcBlob {
   TcProgram sdf_prog;     // L0..L7 + sdf dot
-  TcProgram full_prog;    // forward + reverse + colour
+  TcProgram full_prog;    // forward + reverse + colour (Field::tc_full)
   TcProgram fwd_prog;     // L0..L8 (sdf + features), operator API
-  bool has_full;
+  // what tc_pack writes into the field's storage: the chains' folded colour layer 0, the programs' constants, and for
+  // packed layer i (src[i]) its 2^-s at inv_scale[i] and its weight slots in blob
+  float* Mfold;           // [256][kLdM]
+  float* w8row;           // W8[0,:]
+  float* Wrgb;            // [3][256] rgb head, zero padded
+  float* b8feat;          // b8[1:], 16-byte aligned copy (the epilogue loads float4)
+  float* inv_scale;
+  uint8_t* blob;
+  std::vector<TcSrc> src;
 };
 
 // inv_scale[0] = 2^-s of the weights W[0, n)
@@ -982,19 +996,6 @@ __global__ void pack_slot_kernel(const float* __restrict__ W, int ld, int transp
   *(__half*)(dst_lo + off) = l;
 }
 
-__global__ void copy_strided_kernel(const float* __restrict__ src, int stride, int n, float* __restrict__ dst) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[(size_t)i * stride];
-}
-
-// dst[r][c] (ld 256, zero padded) = src[r * lds + c] for c < ncols
-__global__ void pad_rows_kernel(const float* __restrict__ src, int lds, int nrows, int ncols, float* __restrict__ dst) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nrows * 256) return;
-  int r = i >> 8, c = i & 255;
-  dst[i] = (c < ncols) ? src[(size_t)r * lds + c] : 0.f;
-}
-
 // M[n][k] = sum_j Wc[n][coff + j] * W8f[j][k]   (n < n_rows, k < 256; W8f = W8[1:], row stride ld8; M row stride ldm)
 // cb[n]   = sum_j Wc[n][coff + j] * b8f[j]
 __global__ void fold_mm_kernel(const float* __restrict__ Wc, int ldc, int coff, const float* __restrict__ W8f, int ld8,
@@ -1022,132 +1023,54 @@ __global__ void fill_extra_cols_kernel(const float* __restrict__ Wt, int n_out, 
   M[(size_t)n * ldm + 256 + e] = (n < n_out && e < n_extra) ? Wt[(size_t)e * n_out + n] : 0.f;
 }
 
-size_t tc_pack_bytes() { return (size_t)kBlobSlots * kSlotBytes + (1 << 20); }
+TcBlob* tc_new() { return new TcBlob(); }
+void tc_free(TcBlob* tb) { delete tb; }
 
-struct PackCtx {
-  cudaStream_t st;
-  uint8_t* blob;
-  int nslots;
-  int nlayers;        // packed layers so far (index into inv_scale)
-  float* inv_scale;   // [kMaxSteps]
-};
-
-// One layer step: its descriptor, the 2^s scale of W and nk K-chunks of hi/lo weight slots holding B[n][k] = W[n_off + n][k]
-// (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere.
-static int pack_layer(PackCtx& c, TcStep& stp, int kind, int flags, int sig, const float* bias, const float* W, int ld,
-                      int transposed, int n_off, int n_valid, int k_valid, int nk, int total_elems, int perm16 = 0) {
-  MP_REQUIRE(c.nslots + 2 * nk <= kBlobSlots, "tc_pack: slot budget exceeded (%d)", c.nslots + 2 * nk);
-  const int layer = c.nlayers++;
-  stp.nk = nk;
-  stp.kind = kind;
-  stp.flags = flags;
-  stp.sig = sig;
-  stp.bias = bias;
-  stp.slot_off = c.nslots;
-  stp.sc = layer;
-  stp.terms = 3;
-  absmax_kernel<<<1, 256, 0, c.st>>>(W, total_elems, c.inv_scale + layer);
-  MP_LAUNCH_CHECK();
-  for (int kc = 0; kc < nk; ++kc) {
-    uint8_t* hi = c.blob + (size_t)c.nslots * kSlotBytes;
-    uint8_t* lo = hi + kSlotBytes;
-    pack_slot_kernel<<<64, 256, 0, c.st>>>(W, ld, transposed, n_off, 0, n_valid, k_valid, kc, c.inv_scale + layer, hi,
-                                           lo, perm16);
-    MP_LAUNCH_CHECK();
-    c.nslots += 2;
-  }
-  return 0;
-}
-
-void tc_free(Field& f) {
-  delete (TcBlob*)f.tc;
-  f.tc = nullptr;
-}
-
-// The three programs, one pack_layer per step (kind, flags, sigma' layer, bias, then the weight source).  L0..L7 are
+// The three programs, one layer() per packed step (kind, flags, sigma' layer, bias, then the weight source).  L0..L7 are
 // packed once and shared: the sdf-only, forward and background programs run them as plain softplus steps, the fused
-// foreground program saves sigma' and seeds the reverse sweep.
-int tc_pack(Field& f, Arena& a, cudaStream_t st) {
-  TcBlob* tb = new TcBlob();
-  memset(tb, 0, sizeof(*tb));
-  f.tc = tb;
+// foreground program saves sigma' and seeds the reverse sweep.  Slots are assigned in packing order and the number
+// assigned is returned; on a sizing layout (null pointers) that is all this is for.
+static int tc_programs(const Field& f, TcBlob& tb) {
+  int nslots = 0;
+  auto layer = [&](TcStep& stp, int kind, int flags, int sig, const float* bias, const float* W, int ld, int transposed,
+                   int n_off, int n_valid, int k_valid, int nk, int total, int perm16 = 0) {
+    stp = TcStep{nk, kind, flags, sig, bias, nslots, (int)tb.src.size(), 3};
+    tb.src.push_back(TcSrc{W, ld, transposed, n_off, n_valid, k_valid, nk, total, perm16, nslots});
+    nslots += 2 * nk;
+  };
   const int E = f.emb_dim;
-  PackCtx c;
-  c.st = st;
-  c.nslots = 0;
-  c.nlayers = 0;
-  c.blob = (uint8_t*)a.take<uint4>((size_t)kBlobSlots * kSlotBytes / 16);
-  c.inv_scale = a.take<float>(32);
-  float* w8row = a.take<float>(256);
-  float* Wrgb = a.take<float>(3 * 256);
-  float* b8feat = a.take<float>(256);      // b8[1:], 16-byte aligned copy (the epilogue loads float4)
-  MP_REQUIRE(a.ok, "tc_pack: storage too small");
-  MP_CHECK_CUDA(cudaMemsetAsync(c.blob, 0, (size_t)kBlobSlots * kSlotBytes, st));
-  TcProgram P;
-  memset(&P, 0, sizeof(P));
-  P.blob = (const uint4*)c.blob;
-  P.inv_scale = c.inv_scale;
+  TcProgram P{};
   P.d_in = f.d_in;
   P.multires = f.multires;
   P.E = E;
   P.inj_col = kHidden - E;
-  P.w8row = w8row;
+  P.w8row = tb.w8row;
   P.b8 = f.imp_b[8];
-  P.Wrgb = Wrgb;
+  P.Wrgb = tb.Wrgb;
   P.n_extra = f.ren_extra;
-  copy_strided_kernel<<<1, 256, 0, st>>>(f.imp_W[8], 1, 256, w8row);     // W8[0,:]
-  MP_LAUNCH_CHECK();
-  copy_strided_kernel<<<1, 256, 0, st>>>(f.imp_b[8] + 1, 1, 256, b8feat);
-  MP_LAUNCH_CHECK();
   int s = 0;
   // ---- forward L0..L7: the sdf-only program ----
   for (int l = 0; l < 8; ++l) {
     const int in = f.imp_in[l], out = f.imp_out[l];
     const int flags = ((l == f.skip_layer - 1) ? F_INJECT_EMB : 0) | ((l == 7) ? F_SDF_DOT : 0);
-    MP_TRY(pack_layer(c, P.step[s++], K_SP_PLAIN, flags, l, (l == 0) ? f.imp_b0_eff : f.imp_b[l], f.imp_W[l], in, 0,
-                      0, out, (l == 0) ? E : in, (l == 0) ? (E + 63) / 64 : 4, out * in));
+    layer(P.step[s++], K_SP_PLAIN, flags, l, (l == 0) ? f.imp_b0_eff : f.imp_b[l], f.imp_W[l], in, 0, 0, out,
+          (l == 0) ? E : in, (l == 0) ? (E + 63) / 64 : 4, out * in);
   }
   P.nsteps = s;
-  tb->sdf_prog = P;
+  tb.sdf_prog = P;
   // ---- L8 features (operator API: sdf + features) ----
-  tb->fwd_prog = P;
-  MP_TRY(pack_layer(c, tb->fwd_prog.step[s], K_FEAT, 0, -1, b8feat, f.imp_W[8], 256, 0, 1, 256, 256, 4, 257 * 256));
-  tb->fwd_prog.nsteps = s + 1;
-  const bool fg_chain = (f.ren_mode == 0) && (f.n_ren == 5) && f.ren_out[0] == 256;
-  const bool bg_chain = (f.ren_mode == 1) && (f.n_ren == 2) && f.ren_out[0] <= 256 && f.ren_extra <= 27;
-  tb->has_full = fg_chain || bg_chain;
-  // The feature layer L8 and the colour layer 0 have no non-linearity in between (networks.py:199-207 -> :281,:305):
-  //   C0_pre = Wc0[:, feat] (W8[1:] h7 + b8[1:]) + Wc0[:, extra] extra + b0  =  M h7 + (Wc0f b8f + b0) + ...
-  // so the fused chains run ONE layer with M = Wc0[:, feat] . W8[1:, :] instead of two.
-  // the colour layer 0 the chains run: [ M | extra-input columns | 0 ]  (256 x 320, K-blocks 0..3 | 4)
-  constexpr int kLdM = 320;
-  float* Mfold = a.take<float>(256 * kLdM);
-  f.ren_cb = a.take<float>(264);
-  f.ren_b0_fold = a.take<float>(264);
-  MP_REQUIRE(a.ok, "tc_pack: storage too small");
-  if (tb->has_full) {
-    const int in0 = f.ren_in[0] == 0 ? 0 : (f.ren_mode == 0 ? 6 + 8 + 256 : f.ren_extra + 32 + 256);
-    const int coff = f.ren_mode == 0 ? 14 : f.ren_extra + 32;
-    const int o0 = f.ren_out[0];
-    fold_mm_kernel<<<dim3(256 / 16, div_up(o0, 16)), dim3(16, 16), 0, st>>>(f.ren_W[0], in0, coff, f.imp_W[8] + 256, 256,
-                                                                          f.imp_b[8] + 1, o0, Mfold, kLdM, f.ren_cb);
-    MP_LAUNCH_CHECK();
-    MP_REQUIRE(f.ren_extra <= 64, "tc_pack: more than 64 extra colour inputs");
-    fill_extra_cols_kernel<<<64, 256, 0, st>>>(f.ren_Wt[0], o0, f.ren_extra, Mfold, kLdM);
-    MP_LAUNCH_CHECK();
-  }
-  if (bg_chain) {
+  tb.fwd_prog = P;
+  layer(tb.fwd_prog.step[s], K_FEAT, 0, -1, tb.b8feat, f.imp_W[8], 256, 0, 1, 256, 256, 4, 257 * 256);
+  tb.fwd_prog.nsteps = s + 1;
+  if (f.tc_full && f.ren_mode == 1) {
     // background: folded colour layer 0 (view embedding + h7 -> 128, ReLU) and the rgb head (multiply.py:531)
-    const int o0 = f.ren_out[0];
-    MP_TRY(pack_layer(c, P.step[s++], K_RELU, F_EXTRA_IN | F_RGB_OUT, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, o0, kLdM, 5,
-                      256 * kLdM));
-    pad_rows_kernel<<<div_up(3 * 256, 256), 256, 0, st>>>(f.ren_W[1], o0, 3, o0, Wrgb);
-    MP_LAUNCH_CHECK();
+    layer(P.step[s++], K_RELU, F_EXTRA_IN | F_RGB_OUT, -1, f.ren_b0_fold, tb.Mfold, kLdM, 0, 0, f.ren_out[0], kLdM, 5,
+          256 * kLdM);
     P.brgb = f.ren_b[1];
     P.nsteps = s;
-    tb->full_prog = P;
+    tb.full_prog = P;
   }
-  if (fg_chain) {
+  if (f.tc_full && f.ren_mode == 0) {
     // L0..L7 save sigma' for the reverse sweep, which starts right after L7; h7 is parked (it returns as the folded
     // colour layer's input)
     for (int l = 0; l < 8; ++l) P.step[l].kind = (l == 7) ? K_SP_SEED : K_SP_SAVE;
@@ -1155,25 +1078,78 @@ int tc_pack(Field& f, Arena& a, cudaStream_t st) {
     for (int l = 7; l >= 1; --l) {
       const int in = f.imp_in[l], out = f.imp_out[l];
       // B[n][k] = W_l[k][n] : n over in (valid in), k over out (valid out)
-      MP_TRY(pack_layer(c, P.step[s++], K_BWD, (l == f.skip_layer) ? F_SKIP_GRAD : 0, l - 1, nullptr, f.imp_W[l], in, 1,
-                        0, in, out, 4, out * in));
+      layer(P.step[s++], K_BWD, (l == f.skip_layer) ? F_SKIP_GRAD : 0, l - 1, nullptr, f.imp_W[l], in, 1, 0, in, out, 4,
+            out * in);
     }
     // ---- B0: d/d embed = (g_0 * sigma'_0) . W0[:, :E] ----
-    MP_REQUIRE(f.d_in <= 4 && 1 + 2 * f.multires <= 14,
-               "tc_pack: the final-gradient step keeps 1 + 2 * multires <= 14 embedding columns per axis");
-    MP_TRY(pack_layer(c, P.step[s++], K_FINAL_GRAD, 0, -1, nullptr, f.imp_W[0], f.imp_in[0], 1, 0, E, 256, 4,
-                      256 * f.imp_in[0], /*perm16=*/f.d_in));
+    layer(P.step[s++], K_FINAL_GRAD, 0, -1, nullptr, f.imp_W[0], f.imp_in[0], 1, 0, E, 256, 4, 256 * f.imp_in[0],
+          /*perm16=*/f.d_in);
     // ---- colour net: folded layer 0, then layers 1..3 ----
-    MP_TRY(pack_layer(c, P.step[s++], K_RELU, F_EXTRA_IN, -1, f.ren_b0_fold, Mfold, kLdM, 0, 0, 256, kLdM, 5,
-                      256 * kLdM));
+    layer(P.step[s++], K_RELU, F_EXTRA_IN, -1, f.ren_b0_fold, tb.Mfold, kLdM, 0, 0, 256, kLdM, 5, 256 * kLdM);
     for (int l = 1; l < 4; ++l)
-      MP_TRY(pack_layer(c, P.step[s++], K_RELU, (l == 3) ? F_RGB_OUT : 0, -1, f.ren_b[l], f.ren_W[l], 256, 0, 0, 256,
-                        256, 4, 256 * 256));
-    // rgb head [3][256]
-    MP_CHECK_CUDA(cudaMemcpyAsync(Wrgb, f.ren_W[4], (size_t)3 * 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      layer(P.step[s++], K_RELU, (l == 3) ? F_RGB_OUT : 0, -1, f.ren_b[l], f.ren_W[l], 256, 0, 0, 256, 256, 4,
+            256 * 256);
     P.brgb = f.ren_b[4];
     P.nsteps = s;
-    tb->full_prog = P;
+    tb.full_prog = P;
+  }
+  return nslots;
+}
+
+// The tensor-core share of a field's storage, taken at the end of its carve: the chains' folded colour layer 0 and its
+// biases, the programs' constants, then one 2^-s per packed layer and the weight slots, as many as the programs assign.
+// Lays out f.tc, or on a sizing Arena (f.tc null) a blob that is thrown away.
+void tc_pack_carve(Arena& a, Field& f) {
+  TcBlob sizing{};
+  TcBlob& tb = f.tc ? *f.tc : sizing;
+  tb.Mfold = a.take<float>(256 * kLdM);
+  f.ren_cb = a.take<float>(264);
+  f.ren_b0_fold = a.take<float>(264);
+  tb.w8row = a.take<float>(256);
+  tb.Wrgb = a.take<float>(3 * 256);
+  tb.b8feat = a.take<float>(256);
+  const int nslots = tc_programs(f, tb);
+  tb.inv_scale = a.take<float>(tb.src.size());
+  tb.blob = a.take<uint8_t>((size_t)nslots * kSlotBytes);
+  for (TcProgram* P : {&tb.sdf_prog, &tb.fwd_prog, &tb.full_prog}) {
+    P->inv_scale = tb.inv_scale;
+    P->blob = (const uint4*)tb.blob;
+  }
+}
+
+// Fills what tc_pack_carve laid out in the zeroed storage, from the fp32 layers mp_field_pack has folded: the programs'
+// constants, the chains' folded colour layer 0, then every packed layer's 2^-s and weight slots.
+int tc_pack(const Field& f, cudaStream_t st) {
+  const TcBlob& tb = *f.tc;
+  MP_CHECK_CUDA(cudaMemcpyAsync(tb.w8row, f.imp_W[8], 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));  // W8[0,:]
+  MP_CHECK_CUDA(cudaMemcpyAsync(tb.b8feat, f.imp_b[8] + 1, 256 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (f.tc_full) {
+    // The feature layer L8 and the colour layer 0 have no non-linearity in between (networks.py:199-207 -> :281,:305):
+    //   C0_pre = Wc0[:, feat] (W8[1:] h7 + b8[1:]) + Wc0[:, extra] extra + b0  =  M h7 + (Wc0f b8f + b0) + ...
+    // so the fused chains run ONE layer with M = Wc0[:, feat] . W8[1:, :] instead of two: [ M | extra-input columns | 0 ]
+    // (256 x 320, K-blocks 0..3 | 4).  The feature block is colour layer 0's last 256 inputs.
+    const int in0 = f.ren_in[0], o0 = f.ren_out[0];
+    fold_mm_kernel<<<dim3(256 / 16, div_up(o0, 16)), dim3(16, 16), 0, st>>>(f.ren_W[0], in0, in0 - kHidden,
+                                                                          f.imp_W[8] + 256, 256, f.imp_b[8] + 1, o0,
+                                                                          tb.Mfold, kLdM, f.ren_cb);
+    MP_LAUNCH_CHECK();
+    fill_extra_cols_kernel<<<64, 256, 0, st>>>(f.ren_Wt[0], o0, f.ren_extra, tb.Mfold, kLdM);
+    MP_LAUNCH_CHECK();
+    // the rgb head [3][256]: the last colour layer, whose inputs are the background's 128 (o0) wide
+    const size_t w = (f.ren_mode == 0 ? kHidden : o0) * sizeof(float);
+    MP_CHECK_CUDA(cudaMemcpy2DAsync(tb.Wrgb, 256 * sizeof(float), f.ren_W[f.n_ren - 1], w, w, 3,
+                                    cudaMemcpyDeviceToDevice, st));
+  }
+  for (size_t i = 0; i < tb.src.size(); ++i) {
+    const TcSrc& c = tb.src[i];
+    absmax_kernel<<<1, 256, 0, st>>>(c.W, c.total, tb.inv_scale + i);
+    MP_LAUNCH_CHECK();
+    for (int kc = 0; kc < c.nk; ++kc) {
+      uint8_t* hi = tb.blob + (size_t)(c.slot_off + 2 * kc) * kSlotBytes;
+      pack_slot_kernel<<<64, 256, 0, st>>>(c.W, c.ld, c.transposed, c.n_off, 0, c.n_valid, c.k_valid, kc,
+                                           tb.inv_scale + i, hi, hi + kSlotBytes, c.perm16);
+      MP_LAUNCH_CHECK();
+    }
   }
   return 0;
 }
@@ -1379,17 +1355,17 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
 
 int tc_run(const Field& f, const MlpCall& c, void* ws, size_t ws_bytes, cudaStream_t st) {
   MP_REQUIRE(f.tc, "tensor-core engine: field not packed");
-  const TcBlob& tb = *(const TcBlob*)f.tc;
+  const TcBlob& tb = *f.tc;
   const MlpProg prog = mlp_prog(c);
   TcIO io{};
   static_cast<MlpCall&>(io) = c;
   if (prog == MlpProg::kSdf) return tc_launch(tb.sdf_prog, io, ws, ws_bytes, st, prog);
   if (prog == MlpProg::kForward) return tc_launch(tb.fwd_prog, io, ws, ws_bytes, st, prog);
   if (prog == MlpProg::kBg) {
-    MP_REQUIRE(tb.has_full && f.ren_mode == 1, "tensor-core engine: not a background field");
+    MP_REQUIRE(f.tc_full && f.ren_mode == 1, "tensor-core engine: not a background field");
     return tc_launch(tb.full_prog, io, ws, ws_bytes, st, prog);
   }
-  MP_REQUIRE(tb.has_full, "tensor-core engine: this field has no fused shading program");
+  MP_REQUIRE(f.tc_full, "tensor-core engine: this field has no fused shading program");
   if (c.feat) {
     // the fused program folds L8's feature rows into the colour layer and never materialises the features: the
     // forward program writes them (operator API only; the render passes no feature output)

@@ -64,7 +64,7 @@ class Field:
             pw, pb = L.dev(render_sd["lin_pose.weight"], self.device), L.dev(render_sd["lin_pose.bias"], self.device)
             keep += [pw, pb]
             ren.lin_pose_weight, ren.lin_pose_bias = L.ptr(pw), L.ptr(pb)
-        self.storage = L.workspace(L.call("mp_field_pack_bytes"), self.device)
+        self.storage = L.workspace(L.call("mp_field_pack_bytes", imp, ren, int(background)), self.device)
         self.handle = L.Handle("mp_field_free")
         L.call("mp_field_pack", imp, ren, int(background), self.storage, self.storage.numel(), C.byref(self.handle))
         torch.cuda.current_stream().synchronize()   # raw parameter tensors may be released now

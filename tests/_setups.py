@@ -1,4 +1,5 @@
-"""Set-ups the GPU tests share: scenes and their handles, the mirror's input dict, SMPL handles, points, rays, the
+"""Set-ups the GPU tests share: scenes and their handles, mp_field_pack's network descriptors (and the pairs it
+refuses, which the CPU size-query test uses too), the mirror's input dict, SMPL handles, points, rays, the
 sampler's training draws, the compositor's synthetic inputs and the fused render with canonical meshes."""
 import ctypes as C
 
@@ -28,6 +29,70 @@ def trained():
     bg = engine.Field(sc["bg_implicit"], sc["bg_render"], background=True)
     bg.set_cond(sc["frame_code"])
     return sc, fields, bg
+
+
+def field_descs(implicit_sd, render_sd, background, device=None, **imp):
+    """mp_field_pack's (implicit, render) descriptors of a state-dict pair, laid out as engine.Field lays them out, and
+    the device tensors they point to; ``imp`` overrides descriptor fields (multires, skip_layer).  device None: every
+    weight pointer NULL and lin_pose, where the state dict has it, a dummy address, since the size query reads only the
+    dimensions and whether lin_pose is given."""
+    keep = []
+
+    def put(t):
+        if device is None:
+            return None
+        keep.append(L.dev(t, device))
+        return L.ptr(keep[-1])
+
+    def stack(sd):
+        st = L.LinearStack()
+        st.n_layers = len([k for k in sd if k.startswith("lin") and k.endswith(".bias") and "pose" not in k])
+        for l in range(st.n_layers):
+            v = sd[f"lin{l}.weight_v"] if f"lin{l}.weight_v" in sd else sd[f"lin{l}.weight"]
+            st.weight_v[l], st.weight_g[l], st.bias[l] = put(v), put(sd.get(f"lin{l}.weight_g")), put(sd[f"lin{l}.bias"])
+            st.out_dim[l], st.in_dim[l] = v.shape
+        return st
+
+    d = L.ImplicitDesc(stack(implicit_sd), 4 if background else 3, 10 if background else 6, 32 if background else 69, 4)
+    for k, v in imp.items():
+        setattr(d, k, v)
+    r = L.RenderDesc(stack(render_sd), 1 if background else 0, 4 if background else -1)
+    if "lin_pose.weight" in render_sd:
+        r.lin_pose_weight = put(render_sd["lin_pose.weight"]) if device else 256
+        r.lin_pose_bias = put(render_sd["lin_pose.bias"]) if device else 256
+    return d, r, keep
+
+
+def _resized(sd, l, out, inp):
+    """sd with layer l at out x inp (zero weights)."""
+    sd = dict(sd)
+    v = f"lin{l}.weight_v" if f"lin{l}.weight_v" in sd else f"lin{l}.weight"
+    sd[v], sd[f"lin{l}.bias"] = torch.zeros(out, inp), torch.zeros(out)
+    if f"lin{l}.weight_g" in sd:
+        sd[f"lin{l}.weight_g"] = torch.ones(out, 1)
+    return sd
+
+
+def refused_fields(sc):
+    """Every kind of network pair mp_field_pack refuses, made from scene ``sc``'s: (what, field_descs arguments, the
+    message it is refused with)."""
+    p = sc["persons"][0]
+    fi, fr, bi, br = p["implicit"], p["render"], sc["bg_implicit"], sc["bg_render"]
+    e7 = 3 * (1 + 2 * 7)       # multires 7: 15 embedding columns per axis, one more than the final-gradient step keeps
+    return [
+        ("layer count", ({k: v for k, v in fi.items() if not k.startswith("lin8.")}, fr, False, {}),
+         "ImplicitNet must have 9 linear layers (got 8)"),
+        ("skip layer", (fi, fr, False, dict(skip_layer=3)), "skip_in must be [4]"),
+        ("implicit shape", (_resized(fi, 2, 255, 256), fr, False, {}), "implicit layer 2 has unsupported shape 255x256"),
+        ("pose_no_view width", (fi, _resized(fr, 0, 256, 271), False, {}),
+         "pose_no_view colour net must take 270 inputs and carry lin_pose"),
+        ("nerf_frame_encoding width", (bi, _resized(br, 0, 128, 316), True, {}),
+         "nerf_frame_encoding colour net has unsupported input width 316"),
+        ("no lin_pose", (fi, {k: v for k, v in fr.items() if not k.startswith("lin_pose")}, False, {}),
+         "pose_no_view colour net must take 270 inputs and carry lin_pose"),
+        ("multires 7", (_resized(_resized(fi, 0, 256, e7 + 69), 3, 256 - e7, 256), fr, False, dict(multires=7)),
+         "the final-gradient step keeps 1 + 2 * multires <= 14 embedding columns per axis"),
+    ]
 
 
 @pytest.fixture(scope="module")

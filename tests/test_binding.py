@@ -7,7 +7,9 @@ import re
 import pytest
 import torch
 
-from multiply_b200 import _lib as L
+from multiply_b200 import _lib as L, scene as S
+
+from _setups import field_descs, refused_fields
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 # the int-returning functions whose int is an answer, not a status
@@ -58,9 +60,15 @@ def test_table_states_the_headers_status_and_stream_conventions():
 
 def test_size_queries_are_host_calls():
     """Every workspace and storage query answers on the host: no launch, no device needed (on a machine without a GPU
-    the SM count is taken as 132), and a query of a larger problem never asks for less."""
+    the SM count is taken as 132), and a query of a larger problem never asks for less.  mp_field_pack_bytes reads only
+    the descriptors' dimensions (every weight pointer here is NULL): the background pair's storage is the smaller, and a
+    pair the pack refuses is answered 0."""
     n0 = L.call("mp_launch_count", 0)
     c = L.SamplerCfg(3.0, 0.0, 64, 128, 32, 0.1, 10, 5, 1e-6, 0.1, 1e-4)
+    sc = S.make_scene(P=1, S=16, seed=42)
+    p = sc["persons"][0]
+    fg = field_descs(p["implicit"], p["render"], False)[:2] + (0,)
+    bg = field_descs(sc["bg_implicit"], sc["bg_render"], True)[:2] + (1,)
     for name, small, large in (("mp_mlp_workspace_bytes", (1,), (32769,)),
                                ("mp_sdf_with_deformer_workspace_bytes", (1,), (129,)),
                                ("mp_sdf_grid_workspace_bytes", (8,), (101,)),
@@ -74,6 +82,9 @@ def test_size_queries_are_host_calls():
                                ("mp_smpl_bytes", (300,), (6890,)),
                                ("mp_mise_workspace_bytes", (4, 1), (16, 2)),
                                ("mp_marching_cubes_workspace_bytes", (8,), (64,)),
-                               ("mp_largest_component_workspace_bytes", (3, 1), (1000, 2000))):
+                               ("mp_largest_component_workspace_bytes", (3, 1), (1000, 2000)),
+                               ("mp_field_pack_bytes", bg, fg)):
         assert 0 < L.call(name, *small) <= L.call(name, *large), name
+    for what, (isd, rsd, background, imp), _ in refused_fields(sc):
+        assert L.call("mp_field_pack_bytes", *field_descs(isd, rsd, background, **imp)[:2], int(background)) == 0, what
     assert L.call("mp_launch_count", 0) == n0

@@ -9,7 +9,11 @@ buffer placed at the front of a larger allocation whose tail holds a sentinel:
 The MLP operator query (mp_mlp_workspace_bytes, and the MLP share of every layout that nests it) is the largest layout
 of both engines and all their programs, because the engine can change between the query and the call.  Every call runs
 under both engines.  A call whose own layout is that largest one (the gradient chains, and every layout that nests the
-MLP query) is refused one byte less under at least one engine; any other call must write nothing past that byte."""
+MLP query) is refused one byte less under at least one engine; any other call must write nothing past that byte.
+The one buffer outside this rule is mp_mesh_plan's fixed scratch (MP_MESH_PLAN_SCRATCH_BYTES), which follows the
+alignment rule."""
+import ctypes as C
+import re
 from contextlib import contextmanager
 
 import numpy as np
@@ -23,7 +27,8 @@ from multiply_b200.utils import mesh as umesh               # noqa: E402
 
 import _calls as calls                                                              # noqa: E402
 from _abi import same, sentinel, snap                                               # noqa: E402
-from _setups import Smpl, geo, points, posed_body, pts, train_rng, trained        # noqa: E402,F401
+from _setups import (Smpl, field_descs, geo, points, posed_body, pts, refused_fields, train_rng,   # noqa: E402,F401
+                     trained)
 
 TAIL = 4096 + 256
 SENT = 0xA5
@@ -315,13 +320,71 @@ def test_mesh_storage_bounds(monkeypatch):
     check_bounds(monkeypatch, "mp_mesh_create", run, pos=-3)
 
 
-def test_pack_and_plan_refuse_a_misaligned_base(monkeypatch, trained):
-    """The two buffers outside the query rule, mp_field_pack's storage (sized by an upper bound) and mp_mesh_plan's
-    fixed scratch, follow the alignment rule too."""
-    p = trained[0]["persons"][0]
-    with pytest.raises(L.MpError, match="mp_field_pack: storage base .* not 256-byte aligned"):
-        with placed(monkeypatch, ("mp_field_pack",), "misaligned", pos=-3):
-            engine.Field(p["implicit"], p["render"])
+def test_field_storage_bounds(monkeypatch, geo, trained):
+    """mp_field_pack's storage: foreground fields on geometric and trained weights, the background field, and the
+    mirror's fields whose partner network is a zero stand-in without weight norm (weight_g NULL).  Every field is
+    evaluated by implicit_forward with and without the gradient and render_forward, or bg_forward, under both engines."""
+    from multiply_b200.model import networks
+    N = 129
+    x, nrm, feat, x4 = pts(N, 3, 1), pts(N, 3, 2), pts(N, 256, 3), pts(N, 4, 4)
+    view = pts(N, 3, 5)
+    view = (view / view.norm(dim=1, keepdim=True)).contiguous()
+
+    def mirror(cls, opt, sd):
+        net = cls(S.MODEL_OPT[opt])
+        net.load_state_dict(sd, strict=True)
+        return net.field("cuda")
+
+    def run(o):
+        fields = []
+        for sc in (geo[0], trained[0]):
+            p = sc["persons"][0]
+            fields += [("fg", engine.Field(p["implicit"], p["render"]), p["cond"])]
+        sc, p = trained[0], trained[0]["persons"][0]
+        fields += [("bg", engine.Field(sc["bg_implicit"], sc["bg_render"], background=True), sc["frame_code"]),
+                   ("fg", mirror(networks.ImplicitNet, "implicit_network", p["implicit"]), p["cond"]),
+                   ("fg", mirror(networks.RenderingNet, "rendering_network", p["render"]), p["cond"]),
+                   ("bg", mirror(networks.ImplicitNet, "bg_implicit_network", sc["bg_implicit"]), sc["frame_code"]),
+                   ("bg", mirror(networks.RenderingNet, "bg_rendering_network", sc["bg_render"]), sc["frame_code"])]
+        out = {}
+        try:
+            for eng in ("tc", "simt"):
+                engine.set_engine(eng)
+                for i, (kind, f, cond) in enumerate(fields):
+                    f.set_cond(cond)
+                    if kind == "bg":
+                        out.update({f"{i}/{eng}/bg/{k}": v for k, v in zip(("sdf", "rgb"), f.bg_forward(x4, view))})
+                        continue
+                    out.update({f"{i}/{eng}/fwd/{k}": v for k, v in zip(("sdf", "feat"), f.implicit_forward(x))})
+                    out.update({f"{i}/{eng}/grad/{k}": v
+                                for k, v in zip(("sdf", "feat", "grad"), f.implicit_forward(x, want_grad=True))})
+                    out[f"{i}/{eng}/rgb"] = f.render_forward(x, nrm, feat)
+        finally:
+            engine.set_engine("tc")
+        return out
+
+    check_bounds(monkeypatch, "mp_field_pack", run, pos=-3)
+
+
+def test_pack_refuses_unsupported_networks_before_any_launch(geo):
+    """Every kind of network pair mp_field_pack refuses is refused with its message before anything is enqueued: no
+    launch, the storage untouched, and no handle."""
+    storage = torch.full((32 << 20,), SENT, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    for what, (isd, rsd, background, imp), msg in refused_fields(geo[0]):
+        d, r, keep = field_descs(isd, rsd, background, "cuda", **imp)
+        h = L.Handle("mp_field_free")
+        n0 = _launches()
+        with pytest.raises(L.MpError, match=re.escape("mp_field_pack failed") + ".*" + re.escape(msg)):
+            L.call("mp_field_pack", d, r, int(background), storage, storage.numel(), C.byref(h))
+        assert _launches() == n0, what
+        assert not h.value, what
+    torch.cuda.synchronize()
+    assert bool((storage == SENT).all())
+
+
+def test_mesh_plan_refuses_a_misaligned_scratch():
+    """mp_mesh_plan's fixed scratch, the one buffer outside the query rule, follows the alignment rule."""
     v, f = S.make_body_mesh(100)
     vd, fd = torch.as_tensor(v).float().cuda(), torch.as_tensor(f).long().cuda()
     scratch = L.workspace(L.MP_MESH_PLAN_SCRATCH_BYTES + 16, "cuda")

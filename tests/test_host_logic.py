@@ -6,7 +6,9 @@ import re
 import numpy as np
 import torch
 
-from multiply_b200 import _lib as L
+from multiply_b200 import _lib as L, scene as S
+
+from _setups import field_descs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -39,14 +41,22 @@ def test_errors_are_reported_not_thrown():
     assert lib.mp_set_engine(1) == 0 and lib.mp_get_engine() == 1
 
 
-def test_workspace_queries_are_pure_host():
+def test_workspace_and_storage_queries_are_pure_host():
+    """The queries answer from shapes alone; mp_field_pack_bytes from the two network descriptors, whose weight pointers
+    are NULL here."""
     lib = L.lib()
     c = L.SamplerCfg(3.0, 0.0, 64, 128, 32, 0.1, 10, 5, 1e-6, 0.1, 1e-4)
     a = lib.mp_sampler_workspace_bytes(C.byref(c), 512)
     b = lib.mp_sampler_workspace_bytes(C.byref(c), 1024)
     assert 0 < a < b
     assert lib.mp_body_bytes(6890) > 6890 * 16 * 2
-    assert lib.mp_field_pack_bytes() > 0
+    sc = S.make_scene(P=1, S=16, seed=42)
+    p = sc["persons"][0]
+    fg_imp, fg_ren, _ = field_descs(p["implicit"], p["render"], False)
+    bg_imp, bg_ren, _ = field_descs(sc["bg_implicit"], sc["bg_render"], True)
+    fg = lib.mp_field_pack_bytes(C.byref(fg_imp), C.byref(fg_ren), 0)
+    bg = lib.mp_field_pack_bytes(C.byref(bg_imp), C.byref(bg_ren), 1)
+    assert fg > bg > 0
 
 
 def test_product_path_has_no_oracle_import():
