@@ -421,3 +421,112 @@ def flags_from_taps(sc, r, inp, hits, meshes, out, plist, thr=0.05, xc_out=None)
         off[h, k] = o
         inn[h, k] = i
     return off.all(1), inn.any(1)
+
+
+# ---------------------------------------------------------------------------------------------
+# mesh-extraction grids
+# ---------------------------------------------------------------------------------------------
+#
+# Analytic shapes on the (R+1)^3 lattice of the unit cube (x-major, point i at i / R), stored as MESH_SCALE x their
+# signed distance so that a level l moves every surface outward by l / MESH_SCALE: levels up to 0.125 keep each shape
+# and its holes well inside the cube.  "surfaces" gives, for that offset, each closed surface's signed enclosed volume
+# (negative for a surface that bounds a cavity) and Euler characteristic, in increasing order of volume; "min_R" is the
+# smallest R at which the shape's thinnest part spans enough cells for its topology and volume to hold.
+
+MESH_SCALE = 4.0
+
+
+def _unit_lattice(R):
+    u = np.arange(R + 1, dtype=np.float64) / R
+    return np.meshgrid(u, u, u, indexing="ij")
+
+
+def _ball(X, Y, Z, c, r):
+    return np.sqrt((X - c[0]) ** 2 + (Y - c[1]) ** 2 + (Z - c[2]) ** 2) - r
+
+
+def _ring(X, Y, Z, c, a, b):
+    """Solid torus about the z axis through c: major radius a, minor radius b."""
+    return np.sqrt((np.sqrt((X - c[0]) ** 2 + (Y - c[1]) ** 2) - a) ** 2 + (Z - c[2]) ** 2) - b
+
+
+def _ball_volume(r):
+    return 4.0 / 3.0 * np.pi * r ** 3
+
+
+_RING_VOLUME = {}
+
+
+def _two_rings_volume(a, b, d):
+    """Volume of the union of two coplanar solid tori (a, b) whose centres lie 2d apart: twice a torus less their
+    overlap, integrated over the plane as 2 min(h1, h2), h the half-height of each solid torus (scipy dblquad)."""
+    key = (a, b, d)
+    if key not in _RING_VOLUME:
+        from scipy import integrate
+
+        def h(x, y, cx):
+            r = np.hypot(x - cx, y) - a
+            return np.sqrt(max(b * b - r * r, 0.0))
+
+        ov, _ = integrate.dblquad(lambda y, x: 2.0 * min(h(x, y, -d), h(x, y, d)), 0.0, a + b - d, 0.0, a + b,
+                                  epsabs=1e-10, epsrel=1e-10)
+        _RING_VOLUME[key] = 2.0 * (2.0 * np.pi ** 2 * a * b * b) - 4.0 * ov
+    return _RING_VOLUME[key]
+
+
+_ELL_C, _ELL_A = (0.45, 0.53, 0.52), (0.32, 0.22, 0.16)
+_DT_C, _DT_A, _DT_B, _DT_D = (0.5, 0.503, 0.497), 0.15, 0.07, 0.17
+_TS = ((0.25, 0.5, 0.49), 0.13), ((0.69, 0.52, 0.51), 0.19)
+_SH_C, _SH_R1, _SH_R2 = (0.51, 0.5, 0.49), 0.18, 0.34
+
+MESH_SHAPES = {
+    "sphere": dict(
+        sdf=lambda X, Y, Z: _ball(X, Y, Z, (0.48, 0.51, 0.505), 0.3),
+        surfaces=lambda o: [(_ball_volume(0.3 + o), 2)], min_R=37),
+    "ellipsoid": dict(      # min(axes) x (ellipsoidal radius - 1): the level scales the ellipsoid by 1 + o / 0.16
+        sdf=lambda X, Y, Z: _ELL_A[2] * (np.sqrt(((X - _ELL_C[0]) / _ELL_A[0]) ** 2 + ((Y - _ELL_C[1]) / _ELL_A[1]) ** 2
+                                                 + ((Z - _ELL_C[2]) / _ELL_A[2]) ** 2) - 1.0),
+        surfaces=lambda o: [(_ball_volume(1.0) * np.prod(_ELL_A) * (1.0 + o / _ELL_A[2]) ** 3, 2)], min_R=37),
+    "torus": dict(
+        sdf=lambda X, Y, Z: _ring(X, Y, Z, (0.5, 0.49, 0.51), 0.28, 0.1),
+        surfaces=lambda o: [(2.0 * np.pi ** 2 * 0.28 * (0.1 + o) ** 2, 0)], min_R=64),
+    "double_torus": dict(   # two tori side by side whose tubes merge between them: genus 2
+        sdf=lambda X, Y, Z: np.minimum(_ring(X, Y, Z, (_DT_C[0] - _DT_D, _DT_C[1], _DT_C[2]), _DT_A, _DT_B),
+                                       _ring(X, Y, Z, (_DT_C[0] + _DT_D, _DT_C[1], _DT_C[2]), _DT_A, _DT_B)),
+        surfaces=lambda o: [(_two_rings_volume(_DT_A, _DT_B + o, _DT_D), -2)], min_R=64),
+    "two_spheres": dict(
+        sdf=lambda X, Y, Z: np.minimum(_ball(X, Y, Z, *_TS[0]), _ball(X, Y, Z, *_TS[1])),
+        surfaces=lambda o: [(_ball_volume(_TS[0][1] + o), 2), (_ball_volume(_TS[1][1] + o), 2)], min_R=37),
+    "shell": dict(          # below between r1 and r2: the inner surface faces the centre and encloses -V(r1)
+        sdf=lambda X, Y, Z: np.maximum(_SH_R1 - np.sqrt((X - _SH_C[0]) ** 2 + (Y - _SH_C[1]) ** 2 + (Z - _SH_C[2]) ** 2),
+                                       np.sqrt((X - _SH_C[0]) ** 2 + (Y - _SH_C[1]) ** 2 + (Z - _SH_C[2]) ** 2) - _SH_R2),
+        surfaces=lambda o: [(-_ball_volume(_SH_R1 - o), 2), (_ball_volume(_SH_R2 + o), 2)], min_R=37),
+}
+
+
+def lattice_boundary(R):
+    b = np.zeros((R + 1,) * 3, bool)
+    b[0], b[-1], b[:, 0], b[:, -1], b[:, :, 0], b[:, :, -1] = True, True, True, True, True, True
+    return b
+
+
+def mesh_grid(name, R, level, variant="closed"):
+    """An fp32 grid [R+1]^3 at ``level``: an entry of MESH_SHAPES, "random" (standard normal noise) or "quantised"
+    (level + multiples of 0.5: values on the level, t = 0 / 1 vertices, asymptotic-decider ties).  "closed": no
+    boundary point below the level (those of a coarse shape or of noise are lifted to level + 1); "open": a shape's
+    closed grid with a patch of the x = 0 face set below the level, or the noise as drawn."""
+    if name in MESH_SHAPES:
+        g = (MESH_SCALE * MESH_SHAPES[name]["sdf"](*_unit_lattice(R))).astype(np.float32)
+    else:
+        rng = np.random.default_rng(1000 * R + {"random": 1, "quantised": 2}[name])
+        g = rng.standard_normal((R + 1,) * 3).astype(np.float32)
+        if name == "quantised":
+            g = np.float32(level) + np.round(g * 2).astype(np.float32) / np.float32(2)
+        if variant == "open":
+            return g
+    lift = lattice_boundary(R) & (g.astype(np.float64) < level)
+    g[lift] = np.float32(level + 1.0)
+    if variant == "open":
+        h = R // 2 + 1
+        g[0, :h, :h] = np.float32(level - 1.0)
+    return g

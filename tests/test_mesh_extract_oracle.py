@@ -7,6 +7,9 @@ import pytest
 
 from oracle import build_ref, mesh_extract as M
 
+import _mesh_ref as X
+from _setups import MESH_SHAPES, mesh_grid
+
 
 @pytest.fixture(scope="module")
 def ref_mise():
@@ -199,3 +202,44 @@ def test_edges_table():
     assert all(sum(1 for q in M.FACES for j in range(4) if M._edge(q[j], q[(j + 1) % 4]) == e) == 2
                for e in range(12))
     assert list(itertools.chain(*M.FACES)).count(0) == 3
+
+
+@pytest.mark.parametrize("name", sorted(MESH_SHAPES) + ["quantised", "random"])
+def test_invariant_references_agree_with_the_oracle(name):
+    """tests/_mesh_ref.py's vertex rule equals the oracle's vertices in both calling forms, and its locality, count and
+    balance checks accept the oracle's faces, on small closed and open grids at every level the GPU tests use."""
+    world = ((0.1, -0.2, 0.3), 1.7, 1.1)
+    for R in (1, 2, 3, 9, 14):
+        for level in (0.0, 0.125, -0.0625, -0.0):
+            for variant in ("closed", "open"):
+                g = mesh_grid(name, R, level, variant)
+                v, f = M.marching_cubes(g, level)
+                vr, eid = X.vertex_rule(g, level)
+                assert np.array_equal(v, vr)
+                assert np.array_equal(M.marching_cubes(g, level, *world)[0], X.vertex_rule(g, level, *world)[0])
+                X.face_cubes(g, level, f, eid)
+                assert (X.balance(g, f, eid, variant == "closed") > 0) == (variant == "open" and len(f) > 0)
+
+
+def test_invariant_references_reject_broken_meshes():
+    """The checks fail on what they exist to catch (one face reversed, a vertex id moved to the next crossed edge,
+    faces out of cube order), and the largest-component reference picks the oracle's component."""
+    g = mesh_grid("quantised", 9, 0.0)
+    v, f = M.marching_cubes(g, 0.0)
+    _, eid = X.vertex_rule(g, 0.0)
+    X.face_cubes(g, 0.0, f, eid)
+    X.balance(g, f, eid, True)
+    bad = f.copy()
+    bad[len(f) // 2] = bad[len(f) // 2, ::-1]
+    with pytest.raises(AssertionError):
+        X.balance(g, bad, eid, True)
+    moved = f.copy()
+    moved[0, 0] = (moved[0, 0] + 1) % len(eid)
+    with pytest.raises(AssertionError):
+        X.face_cubes(g, 0.0, moved, eid)
+        X.balance(g, moved, eid, True)
+    with pytest.raises(AssertionError):
+        X.face_cubes(g, 0.0, f[::-1], eid)
+    vk, fk = X.largest_component(v, f)[0]
+    vc, fc = M.largest_component(v, f)
+    assert np.array_equal(vk, vc) and np.array_equal(fk, fc)
