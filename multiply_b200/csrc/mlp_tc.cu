@@ -125,6 +125,11 @@ constexpr size_t kScratchPerCta = kSigBytes + kFeatBytes + kGeBytes + kEmbBytes;
 // stmatrix stores: issued in place, every load would start only after the previous one returned.  So they are issued
 // kAhead of the epilogue's 16 column groups (16 columns each) ahead of their use.
 constexpr int kAhead = 4;
+// The epilogue issues the arithmetic of kEpiW column groups before their stores, and loads the per-step constants a
+// group reads (bias, W8 row, rgb weights) kCAhead groups ahead of their use, in registers the epilogue frees as it
+// stores the accumulator's column groups.
+constexpr int kEpiW = 2;
+constexpr int kCAhead = 3;
 
 // shared memory carve-up
 constexpr int kABytes = 2 * 4 * 128 * 128;                   // hi + lo, 4 K-blocks of [128 x 128B]
@@ -188,12 +193,9 @@ __device__ __forceinline__ void acc_fence(float* d) {
 
 #define MP_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
 #define MP_D16(i) MP_D4(i), MP_D4(i + 4), MP_D4(i + 8), MP_D4(i + 12)
-// D[64 x 256] (+)= A[64 x 16] . B[256 x 16]^T, both operands K-major in shared memory
-__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+// D[64 x 256] += A[64 x 16] . B[256 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %130, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
@@ -203,10 +205,32 @@ __device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_
       "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
       "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
       "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n"
-      "}\n"
+      "%128, %129, 1, 1, 1, 0, 0;\n"
       : MP_D16(0), MP_D16(16), MP_D16(32), MP_D16(48), MP_D16(64), MP_D16(80), MP_D16(96), MP_D16(112)
-      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+      : "l"(a_desc), "l"(b_desc));
+}
+#undef MP_D16
+#undef MP_D4
+// D[64 x 256] = A[64 x 16] . B[256 x 16]^T: the first MMA of a layer step (scale-d 0).  Its outputs are write-only, so
+// the previous step's accumulator is dead once its epilogue has read it, and the registers of the column groups an
+// epilogue has already stored are free for the rest of that epilogue.  The MMA writes them asynchronously: the "+f"
+// operands of the step's later MMAs and of acc_fence keep them in place until the wait.
+#define MP_D4(i) "=f"(d[i]), "=f"(d[i + 1]), "=f"(d[i + 2]), "=f"(d[i + 3])
+#define MP_D16(i) MP_D4(i), MP_D4(i + 4), MP_D4(i + 8), MP_D4(i + 12)
+__device__ __forceinline__ void wgmma_f16_first(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, 0, 1, 1, 0, 0;\n"
+      : MP_D16(0), MP_D16(16), MP_D16(32), MP_D16(48), MP_D16(64), MP_D16(80), MP_D16(96), MP_D16(112)
+      : "l"(a_desc), "l"(b_desc));
 }
 #undef MP_D16
 #undef MP_D4
@@ -246,6 +270,10 @@ __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
 __device__ __forceinline__ void sts128(uint32_t A32, uint32_t off, const uint4& v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(A32 + off), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
 }
+// one fp16 element of the operand image (same ordering as sts128)
+__device__ __forceinline__ void sts16(uint32_t A32, uint32_t off, __half v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(A32 + off), "h"(__half_as_ushort(v)));
+}
 // eight consecutive columns of one row
 __device__ __forceinline__ void store_a8(uint32_t A32, int row, int col, const float* v) {
   uint4 hi, lo;
@@ -273,6 +301,20 @@ __device__ __forceinline__ void store_acc16(uint32_t lane_base, uint32_t lane_x,
   store_pairs(lane_base, lane_x, jp, hi, lo);
 }
 
+template <int V>
+using IntC = std::integral_constant<int, V>;
+// f(IntC<flags & MASK>): one instantiation of f for every subset of the flags in MASK
+template <int MASK, int FL = 0, class F>
+__device__ __forceinline__ void with_flags(int flags, F&& f) {
+  if constexpr (MASK == 0) {
+    f(IntC<FL>{});
+  } else {
+    constexpr int bit = MASK & -MASK;
+    if (flags & bit) with_flags<MASK & ~bit, FL | bit>(flags, f);
+    else with_flags<MASK & ~bit, FL>(flags, f);
+  }
+}
+
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   v += __shfl_xor_sync(0xffffffffu, v, 2);
@@ -292,11 +334,13 @@ __device__ __forceinline__ uint4 ld_stream(const uint4* p) {
   asm volatile("ld.global.cg.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
   return v;
 }
+// (volatile, no memory clobber: the scratch these stores write is read back only by ld_stream, whose volatile asm stays
+// in program order with them, and by no C++ access.)
 __device__ __forceinline__ void st_stream(float4* p, const float4& v) {
-  asm volatile("st.global.cg.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+  asm volatile("st.global.cg.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w));
 }
 __device__ __forceinline__ void st_stream(uint4* p, const uint4& v) {
-  asm volatile("st.global.cg.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+  asm volatile("st.global.cg.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
 }
 
 // The scratch lines of a tile are dead once read (sigma' and the stashed features are written once and read once):
@@ -514,9 +558,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   float* emb = (float*)(scr + kSigBytes + kFeatBytes + kGeBytes);   // [96][128]
   const int d = P.d_in, E = P.E;
 
-  float acc[128];
-#pragma unroll
-  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  float acc[128];                                // written by each step's first MMA (wgmma_f16_first)
   uint32_t it = 0;                               // ring position
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -599,7 +641,6 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       long long c_full = 0, c_wgmma = 0, c_bar = 0;     // PROF: clocks of this step blocked in each phase
       // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
       const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
-      const bool one_term = st.terms == 1;
       // The 132 CTAs' stash (1.2 MB each) does not fit in L2: the sigma' this reverse step's epilogue reads, and the
       // features the final-gradient step reloads, were mostly evicted to DRAM since the forward sweep wrote them.  Pull
       // this warpgroup's 64 KB block back into L2 while the step's MMAs run, so the epilogue's loads hit L2.  (Issued
@@ -639,8 +680,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         held = true;
         held_slot = slot_it;
       };
-      for (int kc = 0; kc < st.nk; ++kc) {
-        if (kc == 4) {
+      // The MMAs over K-chunk kc.  FIRST (kc = 0): its first MMA starts the accumulator, so that no accumulator value
+      // lives from one step into the next.  ONE_TERM: A_hi.W_hi only.  Both are compile-time, so that no MMA sits on a
+      // branch between two others (ptxas would serialise the MMAs to move the accumulator registers there).
+      auto chunk = [&](int kc, auto first, auto one) {
+        constexpr bool FIRST = decltype(first)::value, ONE_TERM = decltype(one)::value;
+        if (!FIRST && kc == 4) {
           // extra-input K-block (colour layer 0): once the MMAs over K-block 0 have drained it, this row's extra inputs
           // (16 columns per lane of the quad, zero padded to 64) take its place and accumulate into the same tile
           {
@@ -688,11 +733,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
           const uint64_t bd = make_desc(wb + ks * 32);
-          wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), bd, (kc | ks) != 0);
-          if (!one_term) wgmma_f16(acc, make_desc(a_lo + ka + ks * 32), bd, 1);
+          if (FIRST && ks == 0) wgmma_f16_first(acc, make_desc(a_hi + ka + ks * 32), bd);
+          else wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), bd);
+          if constexpr (!ONE_TERM) wgmma_f16(acc, make_desc(a_lo + ka + ks * 32), bd);
         }
         slot_issued(it++);
-        if (!one_term) {
+        if constexpr (!ONE_TERM) {
           // lo slot: A_hi.W_lo
           r = it % kRing;
           t0 = stall_clock<PROF>();
@@ -700,10 +746,16 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
           c_full += stall_clock<PROF>() - t0;
           wb = smem_u32(ring + (size_t)r * kSlotBytes);
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), make_desc(wb + ks * 32), 1);
+          for (int ks = 0; ks < 4; ++ks) wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), make_desc(wb + ks * 32));
           slot_issued(it++);
         }
-      }
+      };
+      auto mmas = [&](auto one) {
+        chunk(0, std::true_type{}, one);
+        for (int kc = 1; kc < st.nk; ++kc) chunk(kc, std::false_type{}, one);
+      };
+      if (st.terms == 1) mmas(std::true_type{});
+      else mmas(std::false_type{});
       {
         const long long t0 = stall_clock<PROF>();
         wgmma_wait<0>();
@@ -759,9 +811,38 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         continue;
       }
 
-      auto run_epi = [&](auto kind) {
+      // The epilogue of one step kind.  FL: the step's flags that change the column loop (F_SDF_DOT, F_RGB_OUT), fixed
+      // at compile time so that the unrolled loop holds no branch on them.  The 16 column groups are taken W at a
+      // time: the arithmetic of all W groups first, then their stores (sigma', the feature stash, stmatrix), so that
+      // the MUFU work of several groups overlaps.  The per-step constants a group reads (bias, W8 row, rgb weights)
+      // are loaded kCAhead groups ahead of their use.
+      auto run_epi = [&](auto kind, auto flags) {
         constexpr int KIND = decltype(kind)::value;
+        constexpr int FL = decltype(flags)::value;
+        constexpr bool kBias = KIND != K_BWD;
+        constexpr bool kW8 = KIND == K_SP_SEED || (FL & F_SDF_DOT) != 0;
+        constexpr bool kRgb = KIND == K_RELU && (FL & F_RGB_OUT) != 0;
+        // the reverse step stores nothing but the next A: batching its groups gains nothing there and measured slower
+        constexpr int W = KIND == K_BWD ? 1 : kEpiW;
         float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};     // sdf / rgb partial dots of the two rows
+        struct Consts {
+          float2 b[2], w8[2], rgb[2][3];     // of the group's two 8-column halves
+        };
+        auto load_consts = [&](int jp, Consts& k) {
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int c = 16 * jp + 8 * jj + 2 * q;
+            if constexpr (kBias) k.b[jj] = __ldg((const float2*)(st.bias + c));
+            if constexpr (kW8) k.w8[jj] = __ldg((const float2*)(P.w8row + c));
+            if constexpr (kRgb) {
+#pragma unroll
+              for (int kk = 0; kk < 3; ++kk) k.rgb[jj][kk] = __ldg((const float2*)(P.Wrgb + 256 * kk + c));
+            }
+          }
+        };
+        Consts cpre[kCAhead];
+#pragma unroll
+        for (int k = 0; k < kCAhead; ++k) load_consts(k, cpre[k]);
         // K_BWD: this step's sigma' groups j = 0 .. 31 (8 columns each), loaded 2 kAhead groups ahead of their use
         const float4* sig_g = &sig[((size_t)(st.sig < 0 ? 0 : st.sig) * kConsumers + g) * 32 * 128 + t];
         float4 sig_pre[2 * kAhead];
@@ -771,138 +852,167 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
             sig_pre[k] = st.sig >= 0 ? ld_stream(sig_g + (size_t)k * 128) : make_float4(1.f, 1.f, 1.f, 1.f);
         }
 #pragma unroll
-        for (int jp = 0; jp < 16; ++jp) {
-          float* v = acc + 8 * jp;
-          float yv[8];                       // K_SP_SEED: h7 (the stashed features); A receives the seed
+        for (int jp0 = 0; jp0 < 16; jp0 += W) {
+          float dsv[W][2][4];            // K_SP_SAVE: sigma' of the groups' two 8-column halves
+          float yv[W][8];                // K_SP_SEED: h7 (the stashed features); A receives the seed
 #pragma unroll
-          for (int jj = 0; jj < 2; ++jj) {
-            const int j = 2 * jp + jj;
-            const int c = 8 * j + 2 * q;     // columns c, c + 1 of u[0], u[1] (row 0) and u[2], u[3] (row 1)
-            float* u = v + 4 * jj;
-            float b[2] = {0.f, 0.f};
-            if constexpr (KIND != K_BWD) {
-              const float2 b2 = __ldg((const float2*)(st.bias + c));
-              b[0] = b2.x;
-              b[1] = b2.y;
-            }
-            if constexpr (KIND == K_SP_SEED) {
-              // last SDF layer of the fused chain: sigma'_7 is consumed right here -- the reverse sweep starts from
-              // A = W8[0,:] * sigma'_7 (d sdf / d z7), h7 only feeds the sdf dot and the feature stash
-              const float2 w2 = __ldg((const float2*)(P.w8row + c));
-              const float w[2] = {w2.x, w2.y};
+          for (int wi = 0; wi < W; ++wi) {
+            const int jp = jp0 + wi;
+            float* v = acc + 8 * jp;
+            const Consts cs = cpre[jp % kCAhead];
+            if (jp + kCAhead < 16) load_consts(jp + kCAhead, cpre[jp % kCAhead]);
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float y, dd;
-                softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), y, dd);
-                dot[e >> 1][0] = fmaf(y, w[e & 1], dot[e >> 1][0]);
-                yv[4 * jj + e] = y;
-                u[e] = dd * w[e & 1];
+            for (int jj = 0; jj < 2; ++jj) {
+              const int j = 2 * jp + jj;
+              const int c = 8 * j + 2 * q;     // columns c, c + 1 of u[0], u[1] (row 0) and u[2], u[3] (row 1)
+              float* u = v + 4 * jj;
+              float b[2] = {0.f, 0.f};
+              if constexpr (kBias) {
+                b[0] = cs.b[jj].x;
+                b[1] = cs.b[jj].y;
               }
-            } else if constexpr (KIND == K_SP_SAVE || KIND == K_SP_PLAIN) {
-              if constexpr (KIND == K_SP_SAVE) {
-                float dd[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), u[e], dd[e]);
-                st_stream(&sig[(((size_t)st.sig * kConsumers + g) * 32 + j) * 128 + t], make_float4(dd[0], dd[1], dd[2], dd[3]));
-              } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) u[e] = softplus_fast(fmaf(u[e], isc, b[e & 1]));
-              }
-              if ((st.flags & F_INJECT_EMB) && c + 1 >= P.inj_col) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  if (c + (e & 1) >= P.inj_col) u[e] = emb[(size_t)(c + (e & 1) - P.inj_col) * 128 + rowt[e >> 1]];
-              }
-              if (st.flags & F_SDF_DOT) {
-                const float2 w2 = __ldg((const float2*)(P.w8row + c));
-                dot[0][0] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][0]));
-                dot[1][0] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][0]));
-              }
-            } else if constexpr (KIND == K_FEAT) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) u[e] = fmaf(u[e], isc, b[e & 1]);
-              if (io.feat) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                  if (valid[h]) *(float2*)(io.feat + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
-              }
-            } else if constexpr (KIND == K_BWD) {
-              const float4 s4 = sig_pre[j % (2 * kAhead)];
-              if (j + 2 * kAhead < 32 && st.sig >= 0)
-                sig_pre[j % (2 * kAhead)] = ld_stream(sig_g + (size_t)(j + 2 * kAhead) * 128);
-              const float4* sp = sig_g + (size_t)j * 128;
-              const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
-              if ((st.flags & F_SKIP_GRAD) && c + 1 >= P.inj_col) {
-                // columns >= inj_col are d/d embed through the skip connection: park them, zero them in A
+              if constexpr (KIND == K_SP_SEED) {
+                // last SDF layer of the fused chain: sigma'_7 is consumed right here -- the reverse sweep starts from
+                // A = W8[0,:] * sigma'_7 (d sdf / d z7), h7 only feeds the sdf dot and the feature stash
+                const float w[2] = {cs.w8[jj].x, cs.w8[jj].y};
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                  const float gval = u[e] * isc;
-                  const int col = c + (e & 1);
-                  if (col >= P.inj_col) {
-                    ge[(size_t)(col - P.inj_col) * 128 + rowt[e >> 1]] = gval;
-                    u[e] = 0.f;
-                  } else {
-                    u[e] = gval * sv[e];
-                  }
+                  float y, dd;
+                  softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), y, dd);
+                  dot[e >> 1][0] = fmaf(y, w[e & 1], dot[e >> 1][0]);
+                  yv[wi][4 * jj + e] = y;
+                  u[e] = dd * w[e & 1];
                 }
-              } else {
+              } else if constexpr (KIND == K_SP_SAVE || KIND == K_SP_PLAIN) {
+                if constexpr (KIND == K_SP_SAVE) {
 #pragma unroll
-                for (int e = 0; e < 4; ++e) u[e] *= isc * sv[e];
-              }
-              // this group's sigma' line is dead: drop it from L2
-              if (st.sig >= 0 && (lane & 7) == 0) discard_line(sp, s4.x);
-            } else {   // K_RELU
+                  for (int e = 0; e < 4; ++e) softplus_fast_grad(fmaf(u[e], isc, b[e & 1]), u[e], dsv[wi][jj][e]);
+                } else {
 #pragma unroll
-              for (int e = 0; e < 4; ++e) u[e] = fmaxf(fmaf(u[e], isc, b[e & 1]), 0.f);
-              if (st.flags & F_RGB_OUT) {
+                  for (int e = 0; e < 4; ++e) u[e] = softplus_fast(fmaf(u[e], isc, b[e & 1]));
+                }
+                if constexpr ((FL & F_SDF_DOT) != 0) {
+                  const float2 w2 = cs.w8[jj];
+                  dot[0][0] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][0]));
+                  dot[1][0] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][0]));
+                }
+              } else if constexpr (KIND == K_FEAT) {
 #pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                  const float2 w2 = __ldg((const float2*)(P.Wrgb + 256 * k + c));
-                  dot[0][k] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][k]));
-                  dot[1][k] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][k]));
+                for (int e = 0; e < 4; ++e) u[e] = fmaf(u[e], isc, b[e & 1]);
+                if (io.feat) {
+#pragma unroll
+                  for (int h = 0; h < 2; ++h)
+                    if (valid[h]) *(float2*)(io.feat + (size_t)pt[h] * 256 + c) = make_float2(u[2 * h], u[2 * h + 1]);
+                }
+              } else if constexpr (KIND == K_BWD) {
+                const float4 s4 = sig_pre[j % (2 * kAhead)];
+                if (j + 2 * kAhead < 32 && st.sig >= 0)
+                  sig_pre[j % (2 * kAhead)] = ld_stream(sig_g + (size_t)(j + 2 * kAhead) * 128);
+                const float4* sp = sig_g + (size_t)j * 128;
+                const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
+                if ((st.flags & F_SKIP_GRAD) && c + 1 >= P.inj_col) {
+                  // columns >= inj_col are d/d embed through the skip connection: park them, zero them in A
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) {
+                    const float gval = u[e] * isc;
+                    const int col = c + (e & 1);
+                    if (col >= P.inj_col) {
+                      ge[(size_t)(col - P.inj_col) * 128 + rowt[e >> 1]] = gval;
+                      u[e] = 0.f;
+                    } else {
+                      u[e] = gval * sv[e];
+                    }
+                  }
+                } else {
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) u[e] *= isc * sv[e];
+                }
+                // this group's sigma' line is dead: drop it from L2
+                if (st.sig >= 0 && (lane & 7) == 0) discard_line(sp, s4.x);
+              } else {   // K_RELU
+#pragma unroll
+                for (int e = 0; e < 4; ++e) u[e] = fmaxf(fmaf(u[e], isc, b[e & 1]), 0.f);
+                if constexpr (kRgb) {
+#pragma unroll
+                  for (int k = 0; k < 3; ++k) {
+                    const float2 w2 = cs.rgb[jj][k];
+                    dot[0][k] = fmaf(u[0], w2.x, fmaf(u[1], w2.y, dot[0][k]));
+                    dot[1][k] = fmaf(u[2], w2.x, fmaf(u[3], w2.y, dot[1][k]));
+                  }
                 }
               }
             }
           }
-          if constexpr (KIND == K_SP_SEED) {
-            uint4 fh, fl;
-            split8(yv, fh, fl);
-            st_stream(&fsc[(size_t)jp * 128 + t], fh);
-            st_stream(&fsc[(size_t)(16 + jp) * 128 + t], fl);
+#pragma unroll
+          for (int wi = 0; wi < W; ++wi) {
+            const int jp = jp0 + wi;
+            if constexpr (KIND == K_SP_SAVE) {
+#pragma unroll
+              for (int jj = 0; jj < 2; ++jj)
+                st_stream(&sig[(((size_t)st.sig * kConsumers + g) * 32 + 2 * jp + jj) * 128 + t],
+                          make_float4(dsv[wi][jj][0], dsv[wi][jj][1], dsv[wi][jj][2], dsv[wi][jj][3]));
+            }
+            if constexpr (KIND == K_SP_SEED) {
+              uint4 fh, fl;
+              split8(yv[wi], fh, fl);
+              st_stream(&fsc[(size_t)jp * 128 + t], fh);
+              st_stream(&fsc[(size_t)(16 + jp) * 128 + t], fl);
+            }
+            // activations of these 16 columns -> A (fp16 hi/lo, swizzled) unless this is the last layer
+            if constexpr (!kRgb) store_acc16(lane_base, lane_x, jp, acc + 8 * jp);
           }
-          // activations of these 16 columns -> A (fp16 hi/lo, swizzled) unless this is the last layer
-          bool to_a = true;
-          if constexpr (KIND == K_RELU) to_a = !(st.flags & F_RGB_OUT);
-          if (to_a) store_acc16(lane_base, lane_x, jp, v);
         }
         // ---- step-specific tails: per-row dots reduced over the quad ----
-        if (st.flags & F_SDF_DOT) {
+        if (kW8 && (st.flags & F_SDF_DOT)) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const float sdot = quad_sum(dot[h][0]);
             if (q == 0 && valid[h] && io.sdf) io.sdf[slot[h]] = __ldg(P.b8) + sdot;
           }
         }
-        if constexpr (KIND == K_RELU) {
-          if (st.flags & F_RGB_OUT) {
+        if constexpr (kRgb) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
+          for (int h = 0; h < 2; ++h) {
 #pragma unroll
-              for (int k = 0; k < 3; ++k) {
-                const float z = __ldg(P.brgb + k) + quad_sum(dot[h][k]);
-                if (q == 0 && valid[h] && io.rgb) io.rgb[3 * (size_t)slot[h] + k] = 1.f / (1.f + __expf(-z));
-              }
+            for (int k = 0; k < 3; ++k) {
+              const float z = __ldg(P.brgb + k) + quad_sum(dot[h][k]);
+              if (q == 0 && valid[h] && io.rgb) io.rgb[3 * (size_t)slot[h] + k] = 1.f / (1.f + __expf(-z));
             }
           }
         }
       };
+      // Skip connection (F_INJECT_EMB, softplus kinds): columns >= inj_col of this warpgroup's rows of A receive the
+      // input embedding, split into fp16 hi / lo element by element exactly as split2 splits an activation.  Done after
+      // the column loop, over the injected columns only, so that the loop holds no test of the column against inj_col.
+      // The barrier orders these stores after every lane's stmatrix stores of the same rows.  (The SDF dot of a step
+      // reads the activations before injection; mp_field_pack fixes the skip at layer 4, so F_INJECT_EMB (layer 3) and
+      // F_SDF_DOT (layer 7) never meet in one step.)
+      auto inject_emb = [&]() {
+        wg_sync(bar_id);
+        const int row = 64 * g + (t >> 1);
+        for (int col = P.inj_col + (t & 1); col < kHidden; col += 2) {
+          const float v = emb[(size_t)(col - P.inj_col) * 128 + row];
+          const __half h = __float2half_rn(v);
+          const __half l = __float2half_rn(v - __half2float(h));
+          const uint32_t o = a_off(row, col >> 6, (col >> 3) & 7) + 2u * (uint32_t)(col & 7);
+          sts16(A32, o, h);
+          sts16(A32, 65536u + o, l);
+        }
+      };
+      // each kind's epilogue instantiated for every combination of the flags its column loop reads
       switch (st.kind) {
-        case K_SP_PLAIN: run_epi(std::integral_constant<int, K_SP_PLAIN>{}); break;
-        case K_SP_SAVE: run_epi(std::integral_constant<int, K_SP_SAVE>{}); break;
-        case K_SP_SEED: run_epi(std::integral_constant<int, K_SP_SEED>{}); break;
-        case K_FEAT: run_epi(std::integral_constant<int, K_FEAT>{}); break;
-        case K_BWD: run_epi(std::integral_constant<int, K_BWD>{}); break;
-        default: run_epi(std::integral_constant<int, K_RELU>{}); break;
+        case K_SP_PLAIN:
+          with_flags<F_SDF_DOT>(st.flags, [&](auto fl) { run_epi(IntC<K_SP_PLAIN>{}, fl); });
+          if (st.flags & F_INJECT_EMB) inject_emb();
+          break;
+        case K_SP_SAVE:
+          with_flags<F_SDF_DOT>(st.flags, [&](auto fl) { run_epi(IntC<K_SP_SAVE>{}, fl); });
+          if (st.flags & F_INJECT_EMB) inject_emb();
+          break;
+        case K_SP_SEED: run_epi(IntC<K_SP_SEED>{}, IntC<0>{}); break;
+        case K_FEAT: run_epi(IntC<K_FEAT>{}, IntC<0>{}); break;
+        case K_BWD: run_epi(IntC<K_BWD>{}, IntC<0>{}); break;
+        default: with_flags<F_RGB_OUT>(st.flags, [&](auto fl) { run_epi(IntC<K_RELU>{}, fl); }); break;
       }
       // the skip gradient parked in `ge` is read by other lanes of the quad at the final-gradient step
       if (st.flags & F_SKIP_GRAD) __threadfence_block();
