@@ -73,6 +73,17 @@ struct TcStep {
                         // 1 = A_hi.W_hi only (the lo weight slots are then neither loaded nor issued)
 };
 
+// A step's weight slots: K-chunk kc owns two slots of the blob, hi then lo, from slot_off on (tc_programs reserves them,
+// whatever the precision mode, and tc_pack writes them).  The step consumes chunk by chunk the hi slot and,
+// unless it is single-term, the lo slot: the loader fetches the j-th of them in the order in which the consumers wait.
+__host__ __device__ inline bool tc_one_term(const TcStep& st) { return st.terms == 1; }
+__host__ __device__ inline int tc_packed_slots(int nk) { return 2 * nk; }     // the blob slots of nk K-chunks
+__host__ __device__ inline int tc_slots(const TcStep& st) { return tc_one_term(st) ? st.nk : tc_packed_slots(st.nk); }
+__host__ __device__ inline int tc_chunk_slot(const TcStep& st, int kc, bool lo) { return st.slot_off + 2 * kc + lo; }
+__host__ __device__ inline int tc_slot(const TcStep& st, int j) {
+  return tc_one_term(st) ? tc_chunk_slot(st, j, false) : tc_chunk_slot(st, j >> 1, j & 1);
+}
+
 struct TcProgram {
   int nsteps;
   TcStep step[kMaxSteps];
@@ -104,14 +115,46 @@ static_assert(MP_STALL_WARPS == kStallWarps && MP_STALL_KINDS == K_RELU + 1 && M
                   MP_STALL_PROLOGUE == MP_STALL_KINDS * MP_STALL_PHASES && MP_STALL_ELAPSED == MP_STALL_PROLOGUE + 1 &&
                   MP_STALL_WORDS == MP_STALL_ELAPSED + 1,
               "stall record layout of include/multiply_b200.h");
+// One warp's stall record (PROF): its whole run, its tile prologues, and per step the whole step, the clocks blocked in
+// each phase's waits and the epilogue, added by the lead thread (the loader lane, lane 0 of a consumer warp) to record w
+// of its CTA (0 the loader lane, 1.. the consumer warps).  The default build's recorder reads no clock and adds nothing.
 template <bool PROF>
-__device__ __forceinline__ long long stall_clock() {
-  if constexpr (PROF) return clock64();
-  else return 0;
-}
-__device__ __forceinline__ void stall_add(unsigned long long* rec, int word, long long clocks) {
-  atomicAdd(rec + word, (unsigned long long)clocks);
-}
+struct StallRec {
+  unsigned long long* rec;
+  bool lead;
+  long long t_run, t_tile = 0, t_step = 0, t_epi = 0, c[PH_EMPTY + 1] = {};     // c: this step's clocks in each phase
+  __device__ StallRec(const TcIO& io, int w, bool lead)
+      : rec(io.stalls + ((size_t)blockIdx.x * kStallWarps + w) * MP_STALL_WORDS), lead(lead), t_run(now()) {}
+  static __device__ long long now() {
+    if constexpr (PROF) return clock64();
+    return 0;
+  }
+  template <int PH, class F>
+  __device__ __forceinline__ void wait(F&& f) {
+    const long long t0 = now();
+    f();
+    c[PH] += now() - t0;
+  }
+  __device__ void tile_start() { t_tile = now(); }
+  __device__ void prologue_done() { add(MP_STALL_PROLOGUE, now() - t_tile); }
+  __device__ void step_start() {
+    t_step = now();
+    for (long long& v : c) v = 0;
+  }
+  __device__ void epilogue_start() { t_epi = now(); }
+  // the step's whole time and phases PH0 .. PH1 of its kind: the loader's PH_EMPTY, the consumers' PH_FULL .. PH_EPI
+  template <int PH0, int PH1>
+  __device__ void step_done(int kind) {
+    const long long t = now();
+    if constexpr (PH1 >= PH_EPI) c[PH_EPI] = t - t_epi;
+    add(kind * MP_STALL_PHASES + PH_STEP, t - t_step);
+    for (int ph = PH0; ph <= PH1; ++ph) add(kind * MP_STALL_PHASES + ph, c[ph]);
+  }
+  __device__ void run_done() { add(MP_STALL_ELAPSED, now() - t_run); }
+  __device__ void add(int word, long long clocks) {
+    if (PROF && lead) atomicAdd(rec + word, (unsigned long long)clocks);
+  }
+};
 
 // per-CTA scratch layout (bytes); sigma' and the stashed features are indexed by (warpgroup, register group, thread)
 constexpr size_t kSigBytes = (size_t)8 * kConsumers * 32 * 128 * 16;   // sigma' [8][2][32][128] float4
@@ -241,6 +284,74 @@ __device__ __forceinline__ void wgmma_f16_first(float* d, uint64_t a_desc, uint6
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
+
+// ---------------------------------------------------------------------------------------------
+// the weight ring
+// ---------------------------------------------------------------------------------------------
+// kRing shared-memory slots, each with a `full` barrier (the loader's expect_tx, completed by the bulk copy) and an
+// `empty` barrier.  The loader and each consumer warpgroup walk the same ring positions, one per slot of the tc_slot
+// schedule: position it is slot it % kRing in round it / kRing.
+constexpr int kEmptyArrivals = 4 * kConsumers;     // one release per consumer warp
+struct Ring {
+  char* slots;           // [kRing][kSlotBytes]
+  uint64_t* full;        // [kRing]
+  uint64_t* empty;       // [kRing]
+  uint32_t it = 0;
+  __device__ __forceinline__ static int slot(uint32_t pos) { return pos % kRing; }
+  __device__ __forceinline__ uint32_t phase() const { return (it / kRing) & 1; }
+  __device__ __forceinline__ char* data() const { return slots + (size_t)slot(it) * kSlotBytes; }
+  __device__ __forceinline__ void init() const {
+    for (int i = 0; i < kRing; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], kEmptyArrivals);
+    }
+  }
+  // loader: wait until the previous round of position it has been released, then fill it from src
+  __device__ __forceinline__ void wait_empty() const { mbar_wait(&empty[slot(it)], phase() ^ 1); }
+  __device__ __forceinline__ void fill(const char* src) {
+    mbar_expect_tx(&full[slot(it)], kSlotBytes);
+    bulk_g2s(data(), src, kSlotBytes, &full[slot(it)]);
+    ++it;
+  }
+  // consumers
+  __device__ __forceinline__ void wait_full() const { mbar_wait(&full[slot(it)], phase()); }
+  __device__ __forceinline__ void release(uint32_t pos) const {
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[slot(pos)]);
+  }
+};
+
+// A consumer warpgroup's side of the ring, one per layer step.  Every weight slot's MMAs form one commit group.  A slot
+// is released as soon as the group after it has been committed and all but that newest group have completed, so a
+// warpgroup holds at most one slot in flight while it waits for the next: the ring (3 slots) never waits on a slot
+// that its own reader still holds.  The waits are timed by the warp's stall recorder.
+template <bool PROF>
+struct RingReader {
+  Ring& ring;
+  StallRec<PROF>& rec;
+  bool held = false;       // a slot whose MMAs may still be running
+  uint32_t held_pos = 0;
+  // the shared address of the next slot, once it is filled
+  __device__ __forceinline__ uint32_t wait_full() {
+    rec.template wait<PH_FULL>([&] { ring.wait_full(); });
+    return smem_u32(ring.data());
+  }
+  // the MMAs over the slot of wait_full() have been issued
+  __device__ __forceinline__ void issued() {
+    wgmma_commit();
+    if (held) {
+      rec.template wait<PH_WGMMA>([] { wgmma_wait<1>(); });
+      ring.release(held_pos);
+    }
+    held = true;
+    held_pos = ring.it++;
+  }
+  // wait for every MMA issued into acc, and release the slot still held
+  __device__ __forceinline__ void drain(float* acc) {
+    rec.template wait<PH_WGMMA>([&] { wgmma_wait<0>(); acc_fence(acc); });
+    if (held) ring.release(held_pos);
+    held = false;
+  }
+};
 
 // ---------------------------------------------------------------------------------------------
 // epilogue helpers
@@ -471,6 +582,25 @@ __device__ __forceinline__ void final_grad(const TcProgram& P, const TcIO& io, c
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
+// The loader lane: every step's weight slots of every tile, in tc_slot order, each into the next ring position once
+// it is free.
+template <bool PROF>
+__device__ __forceinline__ void load_weights(const TcProgram& P, const TcIO& io, Ring ring, int ntiles) {
+  StallRec<PROF> rec(io, 0, true);
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    for (int s = 0; s < P.nsteps; ++s) {
+      const TcStep& st = P.step[s];
+      rec.step_start();
+      for (int j = 0; j < tc_slots(st); ++j) {
+        rec.template wait<PH_EMPTY>([&] { ring.wait_empty(); });
+        ring.fill((const char*)P.blob + (size_t)tc_slot(st, j) * kSlotBytes);
+      }
+      rec.template step_done<PH_EMPTY, PH_EMPTY>(st.kind);
+    }
+  }
+  rec.run_done();
+}
+
 // PROF: the stall-accounting build (mp_profile_enable(2)); the default build reads no clock.
 template <bool PROF>
 __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_constant__ TcProgram P,
@@ -481,19 +611,15 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   char* base = (char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   char* A = base;                                   // [hi | lo] x 4 K-blocks
   const uint32_t A32 = smem_u32(A);
-  char* ring = base + kABytes;                      // kRing weight slots
-  uint64_t* bars = (uint64_t*)(ring + kRing * kSlotBytes);
-  uint64_t* full = bars;                            // [kRing]
-  uint64_t* empty = bars + kRing;                   // [kRing]
+  char* slots = base + kABytes;                     // kRing weight slots, then their full and empty barriers
+  uint64_t* bars = (uint64_t*)(slots + kRing * kSlotBytes);
+  Ring ring{slots, bars, bars + kRing};
 
   const int count = io.count ? min(io.cap, *io.count) : io.cap;
   const int ntiles = (count + 127) >> 7;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kRing; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 4 * kConsumers);      // one arrival per consumer warp
-    }
+    ring.init();
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -501,43 +627,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   if (warp < 4) {
     // ===================== weight loader =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (warp == 0 && lane == 0) {
-      const long long t_run = stall_clock<PROF>();
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        for (int s = 0; s < P.nsteps; ++s) {
-          const long long t_step = stall_clock<PROF>();
-          long long c_empty = 0;
-          const char* src = (const char*)P.blob + (size_t)P.step[s].slot_off * kSlotBytes;
-          const int nslot = 2 * P.step[s].nk;
-          const int jstep = P.step[s].terms == 1 ? 2 : 1;
-          for (int j = 0; j < nslot; j += jstep, ++it) {
-            int r = it % kRing;
-            uint32_t ph = (it / kRing) & 1;
-            const long long t0 = stall_clock<PROF>();
-            mbar_wait(&empty[r], ph ^ 1);
-            c_empty += stall_clock<PROF>() - t0;
-            mbar_expect_tx(&full[r], kSlotBytes);
-            bulk_g2s(ring + (size_t)r * kSlotBytes, src + (size_t)j * kSlotBytes, kSlotBytes, &full[r]);
-          }
-          if constexpr (PROF) {
-            unsigned long long* rec = io.stalls + (size_t)blockIdx.x * kStallWarps * MP_STALL_WORDS +
-                                      P.step[s].kind * MP_STALL_PHASES;
-            stall_add(rec, PH_STEP, clock64() - t_step);
-            stall_add(rec, PH_EMPTY, c_empty);
-          }
-        }
-      }
-      if constexpr (PROF)
-        stall_add(io.stalls + (size_t)blockIdx.x * kStallWarps * MP_STALL_WORDS, MP_STALL_ELAPSED, clock64() - t_run);
-    }
+    if (warp == 0 && lane == 0) load_weights<PROF>(P, io, ring, ntiles);
     return;
   }
   // ===================== consumer warpgroups: MMAs + epilogue =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-  const long long t_run = stall_clock<PROF>();
-  // this warp's stall record (PROF): lane 0 adds to it
-  auto srec = [&]() { return io.stalls + ((size_t)blockIdx.x * kStallWarps + warp - 3) * MP_STALL_WORDS; };
+  StallRec<PROF> rec(io, warp - 3, lane == 0);
   const int g = (warp >> 2) - 1;                 // consumer warpgroup: tile rows 64 g .. 64 g + 63
   const int t = threadIdx.x & 127;               // thread in the warpgroup
   const int wq = warp & 3, q = lane & 3;
@@ -559,10 +654,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
   const int d = P.d_in, E = P.E;
 
   float acc[128];                                // written by each step's first MMA (wgmma_f16_first)
-  uint32_t it = 0;                               // ring position
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const long long t_tile = stall_clock<PROF>();
+    rec.tile_start();
     int pt[2], slot[2];
     bool valid[2];
     float x[2][4];
@@ -633,14 +727,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
     // colour-net extra inputs: foreground [x_c, n] (networks.py:281) live in registers (n arrives at the end of the
     // reverse sweep); the background view-dir embedding (:275) was parked in `ge` by the prologue
     float nrm[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-    if constexpr (PROF)
-      if (lane == 0) stall_add(srec(), MP_STALL_PROLOGUE, clock64() - t_tile);
+    rec.prologue_done();
     for (int s = 0; s < P.nsteps; ++s) {
       const TcStep st = P.step[s];
-      const long long t_step = stall_clock<PROF>();
-      long long c_full = 0, c_wgmma = 0, c_bar = 0;     // PROF: clocks of this step blocked in each phase
+      rec.step_start();
       // 2^-s of the weight scaling, times the compensation of the accumulator's round-toward-zero (kRzPerMma)
-      const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (st.terms == 1 ? 1 : 3)), 1.f);
+      const float isc = P.inv_scale[st.sc] * fmaf(io.rz, (float)(4 * st.nk * (tc_one_term(st) ? 1 : 3)), 1.f);
       // The 132 CTAs' stash (1.2 MB each) does not fit in L2: the sigma' this reverse step's epilogue reads, and the
       // features the final-gradient step reloads, were mostly evicted to DRAM since the forward sweep wrote them.  Pull
       // this warpgroup's 64 KB block back into L2 while the step's MMAs run, so the epilogue's loads hit L2.  (Issued
@@ -655,31 +747,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       // ---------------- MMAs: acc = A . W^T over st.nk K-blocks ----------------
       // this warpgroup's rows of A are complete: publish them to the tensor cores
       fence_async_smem();
-      {
-        const long long t0 = stall_clock<PROF>();
-        wg_sync(bar_id);
-        c_bar += stall_clock<PROF>() - t0;
-      }
+      rec.template wait<PH_BAR>([&] { wg_sync(bar_id); });
       wgmma_fence();
-      // Every weight slot's MMAs form one commit group.  A slot is released as soon as the group after it has been
-      // committed and all but that newest group have completed, so a warpgroup holds at most one slot in flight while
-      // it waits for the next: the ring (3 slots) never waits on a slot that its own reader still holds.
-      bool held = false;                         // a slot whose MMAs may still be running
-      uint32_t held_slot = 0;
-      auto release = [&](uint32_t slot_it) {
-        if (lane == 0) mbar_arrive(&empty[slot_it % kRing]);
-      };
-      auto slot_issued = [&](uint32_t slot_it) {
-        wgmma_commit();
-        if (held) {
-          const long long t0 = stall_clock<PROF>();
-          wgmma_wait<1>();
-          c_wgmma += stall_clock<PROF>() - t0;
-          release(held_slot);
-        }
-        held = true;
-        held_slot = slot_it;
-      };
+      RingReader<PROF> rd{ring, rec};
       // The MMAs over K-chunk kc.  FIRST (kc = 0): its first MMA starts the accumulator, so that no accumulator value
       // lives from one step into the next.  ONE_TERM: A_hi.W_hi only.  Both are compile-time, so that no MMA sits on a
       // branch between two others (ptxas would serialise the MMAs to move the accumulator registers there).
@@ -688,14 +758,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         if (!FIRST && kc == 4) {
           // extra-input K-block (colour layer 0): once the MMAs over K-block 0 have drained it, this row's extra inputs
           // (16 columns per lane of the quad, zero padded to 64) take its place and accumulate into the same tile
-          {
-            const long long t0 = stall_clock<PROF>();
-            wgmma_wait<0>();
-            acc_fence(acc);
-            c_wgmma += stall_clock<PROF>() - t0;
-          }
-          if (held) release(held_slot);
-          held = false;
+          rd.drain(acc);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -716,20 +779,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
             }
           }
           fence_async_smem();
-          {
-            const long long t0 = stall_clock<PROF>();
-            wg_sync(bar_id);
-            c_bar += stall_clock<PROF>() - t0;
-          }
+          rec.template wait<PH_BAR>([&] { wg_sync(bar_id); });
           wgmma_fence();
         }
         const uint32_t ka = (uint32_t)(kc & 3) * 16384u;
-        // hi slot: A_hi.W_hi + A_lo.W_hi
-        int r = it % kRing;
-        long long t0 = stall_clock<PROF>();
-        mbar_wait(&full[r], (it / kRing) & 1);
-        c_full += stall_clock<PROF>() - t0;
-        uint32_t wb = smem_u32(ring + (size_t)r * kSlotBytes);
+        // hi slot (tc_chunk_slot(st, kc, false)): A_hi.W_hi + A_lo.W_hi
+        uint32_t wb = rd.wait_full();
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
           const uint64_t bd = make_desc(wb + ks * 32);
@@ -737,48 +792,25 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
           else wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), bd);
           if constexpr (!ONE_TERM) wgmma_f16(acc, make_desc(a_lo + ka + ks * 32), bd);
         }
-        slot_issued(it++);
+        rd.issued();
         if constexpr (!ONE_TERM) {
-          // lo slot: A_hi.W_lo
-          r = it % kRing;
-          t0 = stall_clock<PROF>();
-          mbar_wait(&full[r], (it / kRing) & 1);
-          c_full += stall_clock<PROF>() - t0;
-          wb = smem_u32(ring + (size_t)r * kSlotBytes);
+          // lo slot (tc_chunk_slot(st, kc, true)): A_hi.W_lo
+          wb = rd.wait_full();
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) wgmma_f16(acc, make_desc(a_hi + ka + ks * 32), make_desc(wb + ks * 32));
-          slot_issued(it++);
+          rd.issued();
         }
       };
       auto mmas = [&](auto one) {
         chunk(0, std::true_type{}, one);
         for (int kc = 1; kc < st.nk; ++kc) chunk(kc, std::false_type{}, one);
       };
-      if (st.terms == 1) mmas(std::true_type{});
+      if (tc_one_term(st)) mmas(std::true_type{});
       else mmas(std::false_type{});
-      {
-        const long long t0 = stall_clock<PROF>();
-        wgmma_wait<0>();
-        acc_fence(acc);
-        c_wgmma += stall_clock<PROF>() - t0;
-      }
-      if (held) release(held_slot);
+      rd.drain(acc);
 
       // ---------------- epilogue ----------------
-      const long long t_epi = stall_clock<PROF>();
-      auto step_done = [&]() {
-        if constexpr (PROF) {
-          if (lane == 0) {
-            const long long now = clock64();
-            unsigned long long* rec = srec() + st.kind * MP_STALL_PHASES;
-            stall_add(rec, PH_STEP, now - t_step);
-            stall_add(rec, PH_FULL, c_full);
-            stall_add(rec, PH_WGMMA, c_wgmma);
-            stall_add(rec, PH_BAR, c_bar);
-            stall_add(rec, PH_EPI, now - t_epi);
-          }
-        }
-      };
+      rec.epilogue_start();
       auto reload_features = [&]() {
         // loaded kAhead groups ahead of their use: a load issued after the previous group's discard and stmatrix
         // would wait for that group's load to return (see kAhead)
@@ -807,7 +839,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
         final_grad(P, io, acc, isc, q, ge, emb, rowt, valid, pt, slot, nrm);
         // the MMAs of the reverse sweep are done with A: the features return as the colour net's input
         if (s + 1 < P.nsteps) reload_features();
-        step_done();
+        rec.template step_done<PH_FULL, PH_EPI>(st.kind);
         continue;
       }
 
@@ -1016,22 +1048,22 @@ __global__ void __launch_bounds__(kThreads, 1) tc_chain_kernel(const __grid_cons
       }
       // the skip gradient parked in `ge` is read by other lanes of the quad at the final-gradient step
       if (st.flags & F_SKIP_GRAD) __threadfence_block();
-      step_done();
+      rec.template step_done<PH_FULL, PH_EPI>(st.kind);
     }
   }
-  if constexpr (PROF)
-    if (lane == 0) stall_add(srec(), MP_STALL_ELAPSED, clock64() - t_run);
+  rec.run_done();
 }
 
 // ---------------------------------------------------------------------------------------------
 // packing
 // ---------------------------------------------------------------------------------------------
-// Where one packed layer's weights come from: its nk K-chunks of hi/lo weight slots, from slot slot_off on, hold
+// Where one packed layer's weights come from: the weight slots of its step hold
 // B[n][k] = W[n_off + n][k] (transposed: W[k][n_off + n]) for n < n_valid, k < k_valid, zero elsewhere, scaled by the
 // 2^s of max |W[0, total)|.
 struct TcSrc {
   const float* W;
-  int ld, transposed, n_off, n_valid, k_valid, nk, total, perm16, slot_off;
+  int ld, transposed, n_off, n_valid, k_valid, total, perm16;
+  TcStep step;     // as tc_programs packed it; tc_pack reads its slot layout (nk, slot_off) only
 };
 
 constexpr int kLdM = 320;     // row stride of the chains' folded colour layer 0 (see tc_pack)
@@ -1145,8 +1177,8 @@ static int tc_programs(const Field& f, TcBlob& tb) {
   auto layer = [&](TcStep& stp, int kind, int flags, int sig, const float* bias, const float* W, int ld, int transposed,
                    int n_off, int n_valid, int k_valid, int nk, int total, int perm16 = 0) {
     stp = TcStep{nk, kind, flags, sig, bias, nslots, (int)tb.src.size(), 3};
-    tb.src.push_back(TcSrc{W, ld, transposed, n_off, n_valid, k_valid, nk, total, perm16, nslots});
-    nslots += 2 * nk;
+    tb.src.push_back(TcSrc{W, ld, transposed, n_off, n_valid, k_valid, total, perm16, stp});
+    nslots += tc_packed_slots(nk);
   };
   const int E = f.emb_dim;
   TcProgram P{};
@@ -1254,10 +1286,11 @@ int tc_pack(const Field& f, cudaStream_t st) {
     const TcSrc& c = tb.src[i];
     absmax_kernel<<<1, 256, 0, st>>>(c.W, c.total, tb.inv_scale + i);
     MP_LAUNCH_CHECK();
-    for (int kc = 0; kc < c.nk; ++kc) {
-      uint8_t* hi = tb.blob + (size_t)(c.slot_off + 2 * kc) * kSlotBytes;
+    for (int kc = 0; kc < c.step.nk; ++kc) {
       pack_slot_kernel<<<64, 256, 0, st>>>(c.W, c.ld, c.transposed, c.n_off, 0, c.n_valid, c.k_valid, kc,
-                                           tb.inv_scale + i, hi, hi + kSlotBytes, c.perm16);
+                                           tb.inv_scale + i,
+                                           tb.blob + (size_t)tc_chunk_slot(c.step, kc, false) * kSlotBytes,
+                                           tb.blob + (size_t)tc_chunk_slot(c.step, kc, true) * kSlotBytes, c.perm16);
       MP_LAUNCH_CHECK();
     }
   }
@@ -1394,14 +1427,11 @@ static int tc_launch(const TcProgram& P0, TcIO io, void* ws, size_t ws_bytes, cu
       P.step[s].terms = (mode == 2 || (mode == 1 && P.step[s].kind == K_RELU)) ? 1 : 3;
   }
   int grid = tc_max_grid(io.cap);
-  {
-    static int grid_override = -1;
-    if (grid_override < 0) {
-      const char* eg = getenv("MP_TC_GRID");     // experiment knob: number of persistent CTAs
-      grid_override = eg ? atoi(eg) : 0;
-    }
-    if (grid_override > 0 && grid_override < grid) grid = grid_override;
-  }
+  static const int grid_override = [] {
+    const char* eg = getenv("MP_TC_GRID");     // experiment knob: number of persistent CTAs
+    return eg ? atoi(eg) : 0;
+  }();
+  if (grid_override > 0 && grid_override < grid) grid = grid_override;
   if (grid < 1) return 0;
   Arena a(ws, ws_bytes);
   tc_carve(a, grid, g_prof_stalls.load(), io);
