@@ -146,6 +146,36 @@ size_t mp_mlp_workspace_bytes(int N);
 int mp_bg_nets_forward(mp_net_t* bg_field, const float* pts, const float* view_dirs, int N, float* sdf, float* rgb,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* First-order backward of the networks (DESIGN.md §3.9): layer-major wgmma GEMMs in split fp16 with fp32 accumulation,
+ * every operand scaled into fp16's range by a power of two (so the accuracy does not depend on the loss's scale),
+ * the forward's pre-activations recomputed in chunks of points, every sum over points bounded per tensor-core accumulator
+ * and added in fp64 in a fixed order, so results are bit-identical from run to run and independent of the workspace's
+ * contents.  Outputs are overwritten, not accumulated; a NULL output is not computed.  N = 0 writes zero parameter
+ * gradients (the query answers 0, and a NULL workspace is accepted).  mp_set_engine does not affect these calls. */
+typedef struct {             /* gradients of one linear stack; every pointer may be NULL (not wanted) */
+  float* d_weight[MP_MAX_LAYERS];   /* [out,in]: dL/dW_l of the W the reference's lin{l} applies (g v/||v|| when weight-normed) */
+  float* d_bias[MP_MAX_LAYERS];     /* [out] */
+} mp_linear_grads_t;
+/* Workspace of mp_implicit_backward over N points (either field kind). */
+size_t mp_implicit_backward_workspace_bytes(int N);
+/* VJP of ImplicitNet.forward (networks.py:126-208) at x [N,d_in] with the field's cond (mp_field_set_cond), for the
+ * foreground (d_in 3, 'smpl' cond) and the background (d_in 4, 'frame' cond) field: d_sdf [N] and d_feat [N,256] are
+ * dL/d out[:, 0] and dL/d out[:, 1:] (NULL: zero) -> d_x [N,d_in], grads (all nine layers; d_weight[0] covers the
+ * cond columns, d_weight[4] is of the reference's W4, before the skip's 1/sqrt(2)) and d_cond [cond_dim]. */
+int mp_implicit_backward(mp_net_t* f, const float* x, int N, const float* d_sdf /*[N] or NULL*/,
+                         const float* d_feat /*[N,256] or NULL*/, float* d_x /*[N,d_in] or NULL*/,
+                         mp_linear_grads_t* grads, float* d_cond /*[cond_dim] or NULL*/,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace of mp_render_backward over N points. */
+size_t mp_render_backward_workspace_bytes(int N);
+/* VJP of RenderingNet.forward 'pose_no_view' (networks.py:263-312; 270 -> 4 x 256 -> 3) with the field's cond as
+ * body_pose: d_rgb [N,3] -> d_points, d_normals [N,3], d_feat [N,256], grads of lin0..lin4, lin_pose's d weight [8,69]
+ * and d bias [8], d_body_pose [69].  A background field is refused before anything is enqueued. */
+int mp_render_backward(mp_net_t* f, const float* points, const float* normals, const float* feat, int N,
+                       const float* d_rgb /*[N,3]*/, float* d_points, float* d_normals, float* d_feat,
+                       mp_linear_grads_t* grads, float* d_lin_pose_weight /*[8,69]*/, float* d_lin_pose_bias /*[8]*/,
+                       float* d_body_pose /*[69]*/, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Canonical SDF on the dense lattice of lib/utils/mesh.py:generate_mesh (:78-105; the values MISE's octree queries
  * through Multiply.query_oc, multiply.py:169-172, batch by batch): values[(ix*(res+1)+iy)*(res+1)+iz] =
  * ImplicitNet(p)[0] with p = ((idx/res - 0.5) * pad) * extent + centre (fp32, rounded step by step as numpy does;

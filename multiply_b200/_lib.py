@@ -46,6 +46,10 @@ class RenderDesc(C.Structure):
                 ("lin_pose_weight", C.c_void_p), ("lin_pose_bias", C.c_void_p)]
 
 
+class LinearGrads(C.Structure):
+    _fields_ = [("d_weight", C.c_void_p * MP_MAX_LAYERS), ("d_bias", C.c_void_p * MP_MAX_LAYERS)]
+
+
 class SamplerCfg(C.Structure):
     _fields_ = [("scene_bounding_sphere", C.c_float), ("near", C.c_float), ("N_samples", C.c_int),
                 ("N_samples_eval", C.c_int), ("N_samples_extra", C.c_int), ("eps", C.c_float),
@@ -134,6 +138,11 @@ SIGNATURES = {
     "mp_render_forward": (STATUS, [_VP, _VP, _VP, _VP, _I, _VP, _VP, _SZ, STREAM]),
     "mp_mlp_workspace_bytes": (_SZ, [_I]),
     "mp_bg_nets_forward": (STATUS, [_VP, _VP, _VP, _I, _VP, _VP, _VP, _SZ, STREAM]),
+    "mp_implicit_backward_workspace_bytes": (_SZ, [_I]),
+    "mp_implicit_backward": (STATUS, [_VP, _VP, _I, _VP, _VP, _VP, C.POINTER(LinearGrads), _VP, _VP, _SZ, STREAM]),
+    "mp_render_backward_workspace_bytes": (_SZ, [_I]),
+    "mp_render_backward": (STATUS, [_VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP, C.POINTER(LinearGrads), _VP, _VP, _VP,
+                                    _VP, _SZ, STREAM]),
     "mp_sdf_grid_workspace_bytes": (_SZ, [_I]),
     "mp_sdf_grid": (STATUS, [_VP, c_float_p, _F, _F, _I, _VP, _VP, _SZ, STREAM]),
     "mp_body_bytes": (_SZ, [_I]),

@@ -23,7 +23,7 @@ COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 # (projections, inside tests and depths against oracle/raster.py, distances against oracle/port.py:knn_points)
 NO_FMAD = {"sampler.cu", "composite.cu", "rays.cu", "background.cu", "deform.cu", "mesh.cu", "mesh_extract.cu",
            "raster.cu"}
-SOURCES = ["host_util.cu", "rays.cu", "deform.cu", "mlp_pack.cu", "mlp_simt.cu", "mlp_tc.cu", "sampler.cu",
+SOURCES = ["host_util.cu", "rays.cu", "deform.cu", "mlp_pack.cu", "mlp_simt.cu", "mlp_tc.cu", "mlp_grad.cu", "sampler.cu",
            "composite.cu", "background.cu", "render.cu", "smpl.cu", "mesh.cu", "mesh_extract.cu", "raster.cu"]
 
 

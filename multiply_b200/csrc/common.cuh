@@ -145,6 +145,9 @@ struct Field {
   int ren_cond_dim;
   float* ren_cb;                   // [out0] Wc0[:, feat] . b8[1:]  (colour layer 0 folded onto the feature layer)
   float* ren_b0_fold;              // [out0] ren_b0_eff + ren_cb : bias of the folded layer (tensor-core chains)
+  float* cond;                     // [max(cond_dim, ren_cond_dim)] the cond of the last mp_field_set_cond (backward)
+  float* ren_pose_W;               // [8][69] lin_pose weight (mode 0; backward)
+  float* ren_pose_b;               // [8] lin_pose bias (mode 0; backward)
   bool tc_full;                    // the tensor-core engine has a full program: the fused shade chain (foreground) or the
                                    // background chain
   TcBlob* tc;                      // tensor-core programs (mlp_tc.cu); null until packed

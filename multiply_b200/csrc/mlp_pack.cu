@@ -158,6 +158,11 @@ static void field_carve(Arena& a, Field& f) {
   f.ren_b0_base = a.take<float>(out0);
   f.ren_W0cond = a.take<float>((size_t)f.ren_cond_dim * out0);
   tc_pack_carve(a, f);
+  // read by the backward only (mlp_grad.cu), which needs the raw cond and lin_pose the folded biases hide; after every
+  // buffer the forward reads, so none of those moves
+  f.cond = a.take<float>(f.cond_dim > f.ren_cond_dim ? f.cond_dim : f.ren_cond_dim);
+  f.ren_pose_W = a.take<float>(f.ren_mode == 0 ? 8 * 69 : 0);
+  f.ren_pose_b = a.take<float>(f.ren_mode == 0 ? 8 : 0);
 }
 
 // The fp32 layers into the zeroed storage: weight norm and the skip's 1/sqrt(2) folded in, natural and transposed, and
@@ -189,6 +194,8 @@ static int field_fold(const mp_implicit_desc_t* imp, const mp_render_desc_t* ren
     pose_fold_kernel<<<div_up(out0, 128), 128, 0, st>>>(f.ren_W[0], in0, out0, f.ren_b[0], ren->lin_pose_weight,
                                                         ren->lin_pose_bias, 8, 69, 6, f.ren_W0cond, f.ren_b0_base);
     MP_LAUNCH_CHECK();
+    MP_TRY(copy(f.ren_pose_W, ren->lin_pose_weight, 8 * 69, st));
+    MP_TRY(copy(f.ren_pose_b, ren->lin_pose_bias, 8, st));
   } else {
     MP_TRY(tcols(f.ren_W[0], out0, in0, f.ren_extra, 32, f.ren_W0cond, out0, st));
     MP_TRY(copy(f.ren_b0_base, f.ren_b[0], out0, st));
@@ -249,6 +256,6 @@ int mp_field_set_cond(mp_net_t* h, const float* cond, void* stream) {
     add_vec_kernel<<<div_up(out0, 128), 128, 0, st>>>(f.ren_b0_eff, f.ren_cb, out0, f.ren_b0_fold);
     MP_LAUNCH_CHECK();
   }
-  return 0;
+  return copy(f.cond, cond, f.cond_dim > f.ren_cond_dim ? f.cond_dim : f.ren_cond_dim, st);
 }
 }

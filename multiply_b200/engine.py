@@ -4,6 +4,7 @@ PyTorch is used for device memory and streams only; every computation is a call 
 libmultiply_b200.so (see _lib.py).  No fallback path exists.
 """
 import ctypes as C
+import functools
 import math
 
 import numpy as np
@@ -69,6 +70,9 @@ class Field:
         L.call("mp_field_pack", imp, ren, int(background), self.storage, self.storage.numel(), C.byref(self.handle))
         torch.cuda.current_stream().synchronize()   # raw parameter tensors may be released now
         self.background = background
+        self.d_in, self.cond_dim = imp.d_in, imp.cond_dim
+        self.imp_shapes = [(imp.lin.out_dim[l], imp.lin.in_dim[l]) for l in range(imp.lin.n_layers)]
+        self.ren_shapes = [(ren.lin.out_dim[l], ren.lin.in_dim[l]) for l in range(ren.lin.n_layers)]
 
     def set_cond(self, cond):
         c = L.dev(cond.reshape(-1), self.device)
@@ -145,6 +149,46 @@ class Field:
         ws = L.workspace(L.call("mp_mlp_workspace_bytes", N), self.device)
         L.call("mp_render_forward", self.handle, points, normals, feat, N, rgb, ws, ws.numel())
         return rgb
+
+    def _grads(self, shapes, want):
+        g = L.LinearGrads()
+        dW = [torch.empty(o, i, device=self.device) if want else None for o, i in shapes]
+        db = [torch.empty(o, device=self.device) if want else None for o, _ in shapes]
+        for l in range(len(shapes)):
+            g.d_weight[l], g.d_bias[l] = L.ptr(dW[l]), L.ptr(db[l])
+        return g, dW, db
+
+    def implicit_backward(self, x, d_sdf=None, d_feat=None, want_x=True, want_params=True, want_cond=True):
+        """VJP of ImplicitNet.forward at x [N,d_in] with the current cond (mp_implicit_backward): d_sdf [N] and d_feat
+        [N,256] (None: zero) -> dict(d_x [N,d_in], d_weight [9 x [out,in]] of the effective weights, d_bias, d_cond
+        [cond_dim]); what is not wanted is None."""
+        x = L.dev(x, self.device)
+        N = x.shape[0]
+        d_sdf, d_feat = L.dev(d_sdf, self.device), L.dev(d_feat, self.device)
+        d_x = torch.empty(N, self.d_in, device=self.device) if want_x else None
+        d_cond = torch.empty(self.cond_dim, device=self.device) if want_cond else None
+        g, dW, db = self._grads(self.imp_shapes, want_params)
+        ws = L.workspace(L.call("mp_implicit_backward_workspace_bytes", N), self.device)
+        L.call("mp_implicit_backward", self.handle, x if N else None, N, d_sdf if N else None,
+               d_feat if N else None, d_x if N else None, g, d_cond, ws, ws.numel())
+        return dict(d_x=d_x, d_weight=dW, d_bias=db, d_cond=d_cond)
+
+    def render_backward(self, points, normals, feat, d_rgb, want_inputs=True, want_params=True, want_pose=True):
+        """VJP of RenderingNet.forward 'pose_no_view' with the current cond as body_pose (mp_render_backward): d_rgb
+        [N,3] -> dict(d_points, d_normals [N,3], d_feat [N,256], d_weight / d_bias of lin0.., d_lin_pose_weight [8,69],
+        d_lin_pose_bias [8], d_body_pose [69]); what is not wanted is None."""
+        points, normals, feat, d_rgb = (L.dev(t, self.device) for t in (points, normals, feat, d_rgb))
+        N = points.shape[0]
+        e = lambda *s: torch.empty(*s, device=self.device)      # noqa: E731
+        d_p, d_n, d_f = (e(N, 3), e(N, 3), e(N, 256)) if want_inputs else (None, None, None)
+        d_lpw, d_lpb, d_bp = (e(8, 69), e(8), e(69)) if want_pose else (None, None, None)
+        g, dW, db = self._grads(self.ren_shapes, want_params)
+        ws = L.workspace(L.call("mp_render_backward_workspace_bytes", N), self.device)
+        nz = lambda t: t if N else None                          # noqa: E731
+        L.call("mp_render_backward", self.handle, nz(points), nz(normals), nz(feat), N, nz(d_rgb), nz(d_p), nz(d_n),
+               nz(d_f), g, d_lpw, d_lpb, d_bp, ws, ws.numel())
+        return dict(d_points=d_p, d_normals=d_n, d_feat=d_f, d_weight=dW, d_bias=db, d_lin_pose_weight=d_lpw,
+                    d_lin_pose_bias=d_lpb, d_body_pose=d_bp)
 
 
 class Body:
@@ -723,6 +767,85 @@ class RenderComposite(torch.autograd.Function):
 def _grad_like(g, t):
     """A gradient computed on the device, in the shape, dtype and device of the input ``t`` it belongs to."""
     return g.reshape(t.shape).to(device=t.device, dtype=t.dtype)
+
+
+def _first_order(name):
+    """Refuses a backward that builds a graph (create_graph=True): the networks' backward is first order only."""
+    def wrap(fn):
+        @functools.wraps(fn)
+        def backward(ctx, *grads):
+            if torch.is_grad_enabled():
+                raise NotImplementedError("%s: second-order gradients (create_graph=True) are not implemented; the "
+                                          "networks' backward is first order (DESIGN.md §7)" % name)
+            return fn(ctx, *grads)
+        return backward
+    return wrap
+
+
+class ImplicitFunction(torch.autograd.Function):
+    """ImplicitNet.forward on a packed ``Field`` as one autograd node: inputs x [N,d_in], cond [cond_dim] (any shape of
+    that size) and the effective parameters W_0, b_0, ..., W_8, b_8 (W = g v / ||v|| where weight-normed, so autograd
+    carries dW to g and v); output [N,257] = (sdf | feature), from the field's forward call.  The backward runs
+    mp_implicit_backward on the current stream with the cond of this forward."""
+
+    @staticmethod
+    def forward(ctx, field, x, cond, *params):
+        field.set_cond(cond)
+        sdf, feat = field.implicit_forward(x)
+        ctx.field, ctx.inputs = field, (x, cond) + params
+        ctx.save_for_backward(L.dev(x, field.device), L.dev(cond, field.device))
+        return torch.cat([sdf[:, None], feat], 1)
+
+    @staticmethod
+    @_first_order("ImplicitFunction")
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_out):
+        x, cond = ctx.saved_tensors
+        f, need = ctx.field, ctx.needs_input_grad
+        with torch.cuda.device(f.device):
+            f.set_cond(cond)         # a later forward may have conditioned the field differently
+            d = L.dev(d_out, f.device)
+            r = f.implicit_backward(x, d[:, 0].contiguous(), d[:, 1:].contiguous(), want_x=need[1],
+                                    want_params=any(need[3:]), want_cond=need[2])
+        grads = [None, None if r["d_x"] is None else _grad_like(r["d_x"], ctx.inputs[0]),
+                 None if r["d_cond"] is None else _grad_like(r["d_cond"], ctx.inputs[1])]
+        for l in range(len(f.imp_shapes)):
+            for g, t in ((r["d_weight"][l], ctx.inputs[2 + 2 * l]), (r["d_bias"][l], ctx.inputs[3 + 2 * l])):
+                grads.append(None if g is None else _grad_like(g, t))
+        return tuple(grads)
+
+
+class RenderFunction(torch.autograd.Function):
+    """RenderingNet.forward 'pose_no_view' on a packed ``Field`` as one autograd node: inputs points [N,3], normals
+    [N,3], body_pose [69] (any shape of that size), feature_vectors [N,256] and the parameters W_0, b_0, ..., W_4, b_4
+    (effective weights), lin_pose.weight [8,69], lin_pose.bias [8]; output rgb [N,3] from the field's forward call.  The
+    backward runs mp_render_backward on the current stream with the body_pose of this forward."""
+
+    @staticmethod
+    def forward(ctx, field, points, normals, body_pose, feat, *params):
+        field.set_cond(body_pose)
+        rgb = field.render_forward(points, normals, feat)
+        ctx.field, ctx.inputs = field, (points, normals, body_pose, feat) + params
+        ctx.save_for_backward(*(L.dev(t, field.device) for t in (points, normals, body_pose, feat)))
+        return rgb
+
+    @staticmethod
+    @_first_order("RenderFunction")
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_rgb):
+        points, normals, body_pose, feat = ctx.saved_tensors
+        f, need = ctx.field, ctx.needs_input_grad
+        with torch.cuda.device(f.device):
+            f.set_cond(body_pose)
+            r = f.render_backward(points, normals, feat, d_rgb, want_inputs=any(need[1:3]) or need[4],
+                                  want_params=any(need[5:-2]), want_pose=need[3] or any(need[-2:]))
+        n = len(f.ren_shapes)
+        outs = [r["d_points"], r["d_normals"], r["d_body_pose"], r["d_feat"]]
+        for l in range(n):
+            outs += [r["d_weight"][l], r["d_bias"][l]]
+        outs += [r["d_lin_pose_weight"], r["d_lin_pose_bias"]]
+        return (None,) + tuple(None if g is None or not nd else _grad_like(g, t)
+                               for g, t, nd in zip(outs, ctx.inputs, need[1:]))
 
 
 class SmplFunction(torch.autograd.Function):

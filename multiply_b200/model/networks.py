@@ -1,7 +1,9 @@
 """Mirror of /root/reference/code/lib/model/networks.py: ``ImplicitNet`` and ``RenderingNet`` with the
 reference's constructor options, parameter names (``lin{l}.weight_g / weight_v / bias``, ``lin_pose.*``)
-and forward signatures, so reference checkpoints load unchanged.  ``forward`` runs on the C-ABI library
-(eval only, no autograd) — there is no PyTorch fallback."""
+and forward signatures, so reference checkpoints load unchanged.  ``forward`` runs on the C-ABI library — there is no
+PyTorch fallback.  When grad mode is on and an input or a parameter requires grad, it runs as one autograd node
+(engine.ImplicitFunction / engine.RenderFunction: the same forward call, a first-order backward on the device);
+otherwise it issues exactly the plain forward's launches."""
 import math
 import numpy as np
 import torch
@@ -34,6 +36,23 @@ class _Lin(nn.Module):
             else:
                 self.weight.copy_(w)
             self.bias.copy_(b)
+
+
+def _wants_grad(module, *inputs):
+    """Grad mode is on and an input or a parameter requires grad: the forward goes through the autograd function."""
+    return torch.is_grad_enabled() and (any(t.requires_grad for t in inputs if torch.is_tensor(t)) or
+                                        any(p.requires_grad for p in module.parameters()))
+
+
+def _effective(module):
+    """W_0, b_0, W_1, b_1, ... of the module's lin{l}: the weight the layer applies (torch._weight_norm(v, g, 0) where
+    weight-normed, as nn.utils.weight_norm computes it) and the bias."""
+    out = []
+    for l in range(module.num_layers - 1):
+        lin = getattr(module, "lin%d" % l)
+        w = torch._weight_norm(lin.weight_v, lin.weight_g, 0) if hasattr(lin, "weight_v") else lin.weight
+        out += [w, lin.bias]
+    return out
 
 
 def _get(opt, k, default=None):
@@ -113,6 +132,9 @@ class ImplicitNet(nn.Module):
             return input                       # networks.py:131
         assert nb == 1, "the hot path always runs with batch size 1 (multiply.py:208)"
         f = self.field(input.device)
+        if _wants_grad(self, input, cond[self.cond]):
+            out = engine.ImplicitFunction.apply(f, input.reshape(-1, nd), cond[self.cond], *_effective(self))
+            return out.reshape(nb, npnt, -1)
         f.set_cond(cond[self.cond])
         sdf, feat = f.implicit_forward(input.reshape(-1, nd))
         return torch.cat([sdf[:, None], feat], 1).reshape(nb, npnt, -1)
@@ -166,5 +188,8 @@ class RenderingNet(nn.Module):
         if self.mode != "pose_no_view":
             raise NotImplementedError("standalone background colour net: use Multiply.forward / mp_background")
         f = self.field(points.device)
+        if _wants_grad(self, points, normals, body_pose, feature_vectors):
+            return engine.RenderFunction.apply(f, points, normals, body_pose, feature_vectors, *_effective(self),
+                                               self.lin_pose.weight, self.lin_pose.bias)
         f.set_cond(body_pose)
         return f.render_forward(points, normals, feature_vectors)
