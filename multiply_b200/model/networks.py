@@ -8,6 +8,7 @@ import math
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from .. import engine
 
@@ -53,6 +54,28 @@ def _effective(module):
         w = torch._weight_norm(lin.weight_v, lin.weight_g, 0) if hasattr(lin, "weight_v") else lin.weight
         out += [w, lin.bias]
     return out
+
+
+# Optimizer steps taken in this process.  A fused optimizer step (torch.optim.Adam(fused=True)) updates the parameters
+# in place without bumping their version counters, so the packed field's cache key also holds this count, bumped after
+# every step by a hook; it is read on the host, so keeping it costs no synchronisation.
+_optimizer_steps = 0
+
+
+def _count_step(optimizer, args, kwargs):
+    global _optimizer_steps
+    _optimizer_steps += 1
+
+
+register_optimizer_step_post_hook(_count_step)
+
+
+def _field_key(module, device):
+    """When a mirror module's packed field is stale: a parameter changed in place (its version), was replaced
+    (``p.data = t``: its storage), or an optimizer stepped.  An in-place change that bumps no version counter outside an
+    optimizer step, such as ``p.data.mul_(2)``, is not seen: rebuild the module's field by hand after one
+    (``module._field = None``)."""
+    return (str(device), _optimizer_steps, tuple((int(p._version), p.data_ptr()) for p in module.parameters()))
 
 
 def _get(opt, k, default=None):
@@ -117,7 +140,7 @@ class ImplicitNet(nn.Module):
         return sd
 
     def field(self, device):
-        key = (str(device), tuple(int(p._version) for p in self.parameters()))
+        key = _field_key(self, device)
         if self._field is None or self._field_key != key:
             self._field = engine.Field({k: v.detach() for k, v in self.state_dict().items()}, self._dummy_render_sd(),
                                        background=(self.cond == "frame"), device=device)
@@ -176,7 +199,7 @@ class RenderingNet(nn.Module):
         return sd
 
     def field(self, device):
-        key = (str(device), tuple(int(p._version) for p in self.parameters()))
+        key = _field_key(self, device)
         if self._field is None or self._field_key != key:
             self._field = engine.Field(self._dummy_implicit_sd(), {k: v.detach() for k, v in self.state_dict().items()},
                                        background=(self.mode == "nerf_frame_encoding"), device=device)

@@ -67,6 +67,52 @@ def bg_nets_forward(bg, N):
     return Case("mp_bg_nets_forward", _mlp_query(N), dict(sdf=(N, F32), rgb=((N, 3), F32)), call, inputs)
 
 
+def _grads(shapes, o):
+    """mp_linear_grads_t on the output buffers dW{l} / db{l}."""
+    g = L.LinearGrads()
+    for l in range(len(shapes)):
+        g.d_weight[l], g.d_bias[l] = L.ptr(o["dW%d" % l]), L.ptr(o["db%d" % l])
+    return g
+
+
+def _param_outs(shapes):
+    outs = {}
+    for l, (o, i) in enumerate(shapes):
+        outs["dW%d" % l], outs["db%d" % l] = ((o, i), F32), (o, F32)
+    return outs
+
+
+def implicit_backward(field, N):
+    """mp_implicit_backward of a foreground or background field on N points, every output wanted; inputs(seed): points
+    in [-1, 1)^d_in and upstreams d_sdf, d_feat in [-1, 1)."""
+    outs = dict(d_x=((N, field.d_in), F32), d_cond=(field.cond_dim, F32), **_param_outs(field.imp_shapes))
+
+    def call(x, o, ws):
+        p, d_sdf, d_feat = x
+        L.call("mp_implicit_backward", field.handle, p, N, d_sdf, d_feat, o["d_x"], _grads(field.imp_shapes, o),
+               o["d_cond"], ws, ws.numel())
+        return dict(o)
+
+    return Case("mp_implicit_backward", lambda: L.call("mp_implicit_backward_workspace_bytes", N), outs, call,
+                lambda seed: (pts(N, field.d_in, seed), pts(N, 1, seed + 1).reshape(N), pts(N, 256, seed + 2)))
+
+
+def render_backward(field, N):
+    """mp_render_backward of a foreground field on N points, every output wanted; inputs(seed): points, normals,
+    features and d_rgb in [-1, 1)."""
+    outs = dict(d_points=((N, 3), F32), d_normals=((N, 3), F32), d_feat=((N, 256), F32), d_lpw=((8, 69), F32),
+                d_lpb=(8, F32), d_bp=(69, F32), **_param_outs(field.ren_shapes))
+
+    def call(x, o, ws):
+        p, n, f, d_rgb = x
+        L.call("mp_render_backward", field.handle, p, n, f, N, d_rgb, o["d_points"], o["d_normals"], o["d_feat"],
+               _grads(field.ren_shapes, o), o["d_lpw"], o["d_lpb"], o["d_bp"], ws, ws.numel())
+        return dict(o)
+
+    return Case("mp_render_backward", lambda: L.call("mp_render_backward_workspace_bytes", N), outs, call,
+                lambda seed: (pts(N, 3, seed), pts(N, 3, seed + 1), pts(N, 256, seed + 2), pts(N, 3, seed + 3)))
+
+
 def person_box(sc, fields, pid):
     """Person pid's field and the lattice box of generate_mesh around its canonical body."""
     center, extent, pad = umesh.bounds(sc["persons"][pid]["verts_c"])

@@ -203,6 +203,16 @@ def test_sdf_with_deformer_bounds(monkeypatch, geo, N):
                   lambda: dict(sdf=_full(N), xc=_full((N, 3)), feat=_full((N, 256))))
 
 
+@pytest.mark.parametrize("N", EDGES)
+@pytest.mark.parametrize("net", ["implicit", "bg_implicit", "render"])
+def test_network_backward_bounds(monkeypatch, trained, net, N):
+    """The networks' backward runs on the tensor cores only (it has no SIMT path), and its layout holds one chunk of
+    32768 points at most: N = 32769 runs two chunks in it."""
+    f = trained[2] if net == "bg_implicit" else trained[1][0]
+    c = calls.render_backward(f, N) if net == "render" else calls.implicit_backward(f, N)
+    check_bounds(monkeypatch, *_case(c, c.inputs(30 + N)))
+
+
 @pytest.mark.parametrize("R", [1, 301])
 def test_background_bounds(monkeypatch, trained, R):
     c = calls.background(trained[2], R)

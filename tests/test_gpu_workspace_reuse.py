@@ -163,6 +163,15 @@ def test_bg_nets_forward_reuse(trained, N):
     check_reuse(c, c.inputs(30 + N), c.inputs(40 + N))
 
 
+@pytest.mark.parametrize("N", [1, 129, 32769])
+@pytest.mark.parametrize("net", ["implicit", "bg_implicit", "render"])
+def test_network_backward_reuse(trained, net, N):
+    """N = 32769: two chunks, the second run in the workspace the first left."""
+    f = trained[2] if net == "bg_implicit" else trained[1][0]
+    c = calls.render_backward(f, N) if net == "render" else calls.implicit_backward(f, N)
+    check_reuse(c, c.inputs(50 + N), c.inputs(60 + N))
+
+
 def test_background_reuse(trained):
     """Rays from cameras inside the r = 3 sphere, R = 301 (not a multiple of the 8 rays per block)."""
     c = calls.background(trained[2], 301)
